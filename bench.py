@@ -5,6 +5,8 @@ batch=10000): BASELINE.json's metric on BASELINE.json configs[2].
   python bench.py --gpus N --steps K --warmup W            our arm (CUDA path through the C ABI)
   python bench.py --impl reference --gpus N ...           the reference's CPU implementation (oracle/_ref =
                                                           the unmodified faiss/knowhere sources) on the host cores
+  python bench.py ... --dump-outputs DIR                  also write the last timed step's result (ids.npy as float64,
+                                                          distances.npy as float32) to DIR, to compare two builds
 
 A "step" = one Search() of the whole 10000-query batch.  `value` times the search with queries and
 outputs resident in HBM; `e2e` times the same call with pinned HOST buffers (H2D of the queries and
@@ -65,7 +67,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback: H100 SXM data sheet (3.35 TB/s HBM3, 700 W card), not measured"
 
 
 def peaks_tensor():
@@ -75,11 +77,18 @@ def peaks_tensor():
         j = json.load(open(p))
         if "bf16_tflops" in j:
             return float(j["bf16_tflops"]), "measured (MEASURED_PEAKS.json bf16_tflops, burst)"
-    return 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s dense bf16)"
+    return 989.0, "fallback: H100 SXM data sheet (989 TFLOP/s dense bf16, 700 W card), not measured"
+
+
+def dump_outputs(dirname, ids, dist):
+    """the arrays the timed path returned in its last step: ids (int64, exact in float64) and distances"""
+    os.makedirs(dirname, exist_ok=True)
+    np.save(os.path.join(dirname, "ids.npy"), np.asarray(ids).astype(np.float64))
+    np.save(os.path.join(dirname, "distances.npy"), np.asarray(dist).astype(np.float32))
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle sampling DURING the timed region."""
 
     def __init__(self, gpu_index):
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
@@ -329,6 +338,8 @@ def run_ours(args):
     barrier()
     if os.environ.get("KB2_PROFILE"):
         torch.cuda.cudart().cudaProfilerStop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ids.cpu().numpy(), dis.cpu().numpy())
     clocks = sampler.stop() if sampler else None
     ms_total = e0.elapsed_time(e1)
     if world > 1:
@@ -397,29 +408,20 @@ def run_ours(args):
     #  * query-major scan kernels (ivfpq_scan / ivfflat_scan): HBM view, algorithmic bytes per launch = codes scanned x
     #    code_size (SURVEY §8d: 16 B per PQ code, ids excluded);
     #  * list-major tensor-core engine (ivfpq_tc_filter_kernel): tensor view, algorithmic flops per launch =
-    #    (query, code) pairs x 2 x d — the bf16 contraction the kernel issues on tcgen05 — against the measured dense
-    #    bf16 peak; the HBM view of the same launch is reported beside it.
+    #    (query, code) pairs x 2 x d — the bf16 contraction the kernel issues on the tensor cores — against the data-sheet
+    #    dense bf16 peak; the HBM view of the same launch is reported beside it.
     k_ms = statistics.mean(kernel_ms)
     st_ms = statistics.mean(stage_ms)
     engine = stage_info["engine"] if stage_info else "scan"
     alg_bytes = ctr["code_bytes"]
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "scan_kernel_traffic.json")
-    if os.path.exists(tp):
-        try:
-            traffic = json.load(open(tp)).get(args.workload + ("_tc" if engine == "tc" else ""))
-        except Exception:
-            traffic = None
     if engine == "tc" and wl["index"] == "IVF_FLAT":
-        # list-major tcgen05 IVF_FLAT engine: HBM view on SURVEY 8(d)'s algorithmic bytes (rows scanned x d x 4 per (query, list)
+        # list-major tensor-core IVF_FLAT engine: HBM view on SURVEY 8(d)'s algorithmic bytes (rows scanned x d x 4 per (query, list)
         # pair); every list is physically read once per batch, so the algorithmic figure exceeds the HBM peak by design
         achieved = alg_bytes / (k_ms / 1e3) / 1e9
         tpeak, tsrc = peaks_tensor()
         flops = ctr["codes"] * 2.0 * d * 3.0       # 3 x TF32 MMAs per product
         roofline = {"bound": "hbm", "kernel": "ivfflat_tc_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                    "frac": achieved / peak, "peak_source": peak_src, "traffic": traffic, "kernel_ms": k_ms,
-                    "traffic_source": "constant from profiles/scan_kernel_traffic.json (ncu --set full of this kernel at this "
-                                      "workload), not measured in this run",
+                    "frac": achieved / peak, "peak_source": peak_src, "kernel_ms": k_ms,
                     "algorithmic_bytes_per_launch": alg_bytes, "rows_scanned_per_launch": ctr["codes"],
                     "physical_index_bytes": n * d * 4, "physical_frac_of_hbm_peak": n * d * 4 / (k_ms / 1e3) / 1e9 / peak,
                     "tf32_tflops_issued": flops / (k_ms / 1e3) / 1e12,
@@ -430,12 +432,10 @@ def run_ours(args):
         achieved = alg_flops / (k_ms / 1e3) / 1e12
         tpeak, tsrc = peaks_tensor()
         roofline = {"bound": "tensor", "kernel": "ivfpq_tc_filter_kernel", "achieved": achieved, "peak": tpeak,
-                    "unit": "TFLOP/s", "frac": achieved / tpeak, "peak_source": tsrc, "traffic": traffic,
+                    "unit": "TFLOP/s", "frac": achieved / tpeak, "peak_source": tsrc,
                     "kernel_ms": k_ms, "algorithmic_flops_per_launch": alg_flops,
                     "codes_scanned_per_launch": ctr["codes"], "kernel_share_of_step": k_ms / (ms_total / args.steps),
                     "scan_stage_ms": st_ms, "survivors_re_evaluated": ctr["survivors"], "queries_redone": ctr["flagged"],
-                    "traffic_source": "constant from profiles/scan_kernel_traffic.json (ncu --set full of this kernel at this "
-                                      "workload), not measured in this run",
                     "hbm_algorithmic": {"bytes_per_launch": alg_bytes, "achieved_gbs": alg_bytes / (k_ms / 1e3) / 1e9,
                                         "frac_of_hbm_peak": alg_bytes / (k_ms / 1e3) / 1e9 / peak,
                                         "frac_whole_step": alg_bytes / (ms_total / args.steps / 1e3) / 1e9 / peak,
@@ -447,7 +447,7 @@ def run_ours(args):
         kname = {"IVF_PQ": "ivfpq_scan_kernel", "IVF_FLAT": "ivfflat_scan_kernel", "HNSW": "hnsw_search_kernel"}.get(wl["index"], "?")
         roofline = {"bound": "hbm", "kernel": kname,
                     "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "peak_source": peak_src, "traffic": traffic, "kernel_ms": k_ms,
+                    "peak_source": peak_src, "kernel_ms": k_ms,
                     "algorithmic_bytes_per_launch": alg_bytes, "codes_scanned_per_launch": ctr["codes"],
                     "kernel_share_of_step": k_ms / (ms_total / args.steps)}
     out = {
@@ -577,10 +577,13 @@ def run_reference(args):
     rk = float(cfg.get("refine_k", 0) or 0)
     for _ in range(args.warmup):
         r.search(xq_np, k, cfg["nprobe"], refine_k=rk, nthreads=nthreads)
+    I = D = None
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        r.search(xq_np, k, cfg["nprobe"], refine_k=rk, nthreads=nthreads)
+        I, D = r.search(xq_np, k, cfg["nprobe"], refine_k=rk, nthreads=nthreads)
     el = time.perf_counter() - t0
+    if args.dump_outputs and I is not None:
+        dump_outputs(args.dump_outputs, I, D)
     qps = nq * args.steps / el
     out = {"impl": "reference", "metric": METRIC_NAME if args.workload == "ivf_pq_10m" else f"queries/sec, {args.workload}",
            "value": qps, "unit": "queries/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -609,6 +612,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="ivf_pq_10m", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's ids and distances as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * knowhere_b200.h — C ABI of the B200-native ANN search core (libknowhere_b200.so).
+ * knowhere_b200.h — C ABI of the H100-native ANN search core (libknowhere_b200.so).
  *
  * This is the drop-in boundary.  Every entry point is plain C (pointers + sizes, no
  * C++/torch types) and names the reference interface it stands in for.  A Knowhere
@@ -239,7 +239,7 @@ int kb2_index_last_stage_info(kb2_index_t h, float* out4);
 
 /* validation hook: writes the full key matrix [nq][round_up(nb,4)] of the dense contraction
  * (|q|^2+|x|^2-2qx for L2, -qx for IP) computed by the fp32 CUDA-core kernel (use_tc=0) or by the
- * tcgen05 tensor-core kernel (use_tc=1).  Device pointers only.  Used by tests to hold the tensor-core
+ * wgmma tensor-core kernel (use_tc=1).  Device pointers only.  Used by tests to hold the tensor-core
  * path to the fp32 one (the reference computes these distances with src/simd fvec_L2sqr_ny). */
 int kb2_debug_gemm_keys(const float* q, int64_t nq, const float* x, int64_t nb, int dim, int metric, int use_tc,
                         float* out_keys, int device);

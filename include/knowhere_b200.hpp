@@ -560,7 +560,7 @@ class IndexFactory {
         if (it == map_.end())
             return expected<Index<IndexNode>>::Err(Status::invalid_index_error, "index " + name + " not registered");
         if (kb2_device_count() <= 0)   // index_factory.cc:29-45,62-66: GPU index without a device
-            return expected<Index<IndexNode>>::Err(Status::cuda_runtime_error, "gpu index is not supported: no sm_100 device");
+            return expected<Index<IndexNode>>::Err(Status::cuda_runtime_error, "gpu index is not supported: no sm_90 device");
         return it->second(version, object);
     }
     template <typename DataType>

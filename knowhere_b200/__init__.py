@@ -1,8 +1,8 @@
-"""knowhere_b200 — host-side Python binding of the B200-native ANN search core.
+"""knowhere_b200 — host-side Python binding of the H100-native ANN search core.
 
 This is only the ctypes stub over the C ABI in include/knowhere_b200.h (the product is the
 CUDA library).  There is NO CPU fallback: if the shared library is missing the import fails
-loudly, and every call fails with status 22 (cuda_runtime_error) when no sm_100 GPU is present.
+loudly, and every call fails with status 22 (cuda_runtime_error) when no sm_90 GPU is present.
 """
 import ctypes
 import json

@@ -1,4 +1,4 @@
-"""Build of the in-tree CUDA library (sm_100a only, no multi-arch fallbacks)."""
+"""Build of the in-tree CUDA library (sm_90a only, no multi-arch fallbacks)."""
 import os
 import shutil
 import subprocess
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libknowhere_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fopenmp,-O3,-mavx2,-mfma", "-shared",
 ]
 

@@ -23,7 +23,7 @@ namespace kb2 {
 #ifndef KB2_DEFAULT_GEMM_MODE
 #define KB2_DEFAULT_GEMM_MODE 1
 #endif
-// 0 = fp32 CUDA-core contraction, 1 = tcgen05 (3xTF32) contraction.  KB2_GEMM=fp32|tc overrides.
+// 0 = fp32 CUDA-core contraction, 1 = wgmma (3xTF32) contraction.  KB2_GEMM=fp32|tc overrides.
 inline int
 gemm_mode() {
     static int mode = [] {
@@ -366,7 +366,7 @@ assign_nearest(const float* x, int64_t n, int d, const float* cent, int k, int m
     row_norms_kernel<<<grid1d((int64_t)k * 32, 256), 256, 0, st>>>(cent, k, d, sc.cn.p);
     int64_t chunk = std::max<int64_t>(128, std::min<int64_t>(n, (int64_t)(64ll << 20) / std::max(k, 1)));
     chunk = std::min<int64_t>(chunk, 1 << 20);
-    // wide codebooks (IVF coarse quantizers): the tcgen05 3xTF32 contraction (keys to ~5e-6 relative; the reference's own
+    // wide codebooks (IVF coarse quantizers): the wgmma 3xTF32 contraction (keys to ~5e-6 relative; the reference's own
     // add()/k-means assignment goes through BLAS sgemm, F/utils/distances.cpp:400-520).  Narrow ones (PQ sub-quantizers,
     // k = 256, d = 2..8) stay on the fp32 CUDA-core kernel.
     const int mode = (k >= 512 && (d & 3) == 0 && n >= 1024) ? gemm_mode() : 0;

@@ -1,5 +1,5 @@
 // kb2_capi.cu — the extern "C" boundary declared in include/knowhere_b200.h.
-// Everything behind it is CUDA; there is no CPU fallback: without a usable sm_100 device every
+// Everything behind it is CUDA; there is no CPU fallback: without a usable sm_90 device every
 // entry point fails with KB2_CUDA_RUNTIME_ERROR.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -50,7 +50,7 @@ usable_devices() {
     int ok = 0;
     for (int i = 0; i < n; i++) {
         cudaDeviceProp p;
-        if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 10) ok++;
+        if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 9 && p.minor == 0) ok++;
     }
     return ok;
 }
@@ -72,8 +72,8 @@ require_device(int device) {
     KB2_REQUIRE(device >= 0 && device < n, KB2_INVALID_ARGS, "bad device ordinal");
     cudaDeviceProp p;
     KB2_CUDA_CHECK(cudaGetDeviceProperties(&p, device));
-    KB2_REQUIRE(p.major == 10, KB2_CUDA_RUNTIME_ERROR,
-                "device is not sm_100 (this library ships sm_100a SASS only)");
+    KB2_REQUIRE(p.major == 9 && p.minor == 0, KB2_CUDA_RUNTIME_ERROR,
+                "device is not sm_90 (this library ships sm_90a SASS only)");
     KB2_CUDA_CHECK(cudaSetDevice(device));
     if (device < 64) ok_mask.fetch_or(1ull << device, std::memory_order_relaxed);
 }
@@ -111,7 +111,7 @@ extern "C" {
 
 const char*
 kb2_version(void) {
-    return "knowhere_b200 0.1 (sm_100a)";
+    return "knowhere_b200 0.1 (sm_90a)";
 }
 const char*
 kb2_last_error(void) {

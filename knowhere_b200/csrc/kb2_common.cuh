@@ -1,10 +1,11 @@
-// kb2_common.cuh — shared host/device utilities of the B200-native search core.
+// kb2_common.cuh — shared host/device utilities of the H100-native search core.
 // (product code; never includes anything under oracle/)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
 #include <mutex>
 #include <stdexcept>
 #include <string>
@@ -37,7 +38,6 @@ struct Error : std::runtime_error {
 constexpr int kWarp = 32;
 constexpr int kScanThreads = 256;  // 8 warps per scan CTA
 constexpr int kScanWarps = kScanThreads / kWarp;
-constexpr int kNumSMs = 148;       // B200: 2 dies x 74 SMs
 constexpr uint64_t kEmpty = ~0ull; // empty slot of a top-k list (worst possible key)
 constexpr uint32_t kNoPos = 0xffffffffu;
 
@@ -218,6 +218,27 @@ struct PerDeviceOnce {
         std::call_once(flags[dev], f);
     }
 };
+
+// SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe): sizes the persistent grids and the per-CTA
+// buffers that go with them.  Read once per device.
+inline int
+num_sms() {
+    static std::atomic<int> cache[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); dev = 0; }
+    const bool cached = dev >= 0 && dev < 64;
+    if (cached) {
+        const int v = cache[dev].load(std::memory_order_relaxed);
+        if (v > 0) return v;
+    }
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+        cudaGetLastError();
+        throw Error(KB2_CUDA_RUNTIME_ERROR, "cannot read the SM count of the current device");
+    }
+    if (cached) cache[dev].store(n, std::memory_order_relaxed);
+    return n;
+}
 
 inline bool
 is_device_ptr(const void* p) {

@@ -9,7 +9,7 @@
 // finalize_kernel so that returned distances are the directly accumulated sum((q-x)^2)
 // (self-distance is exactly 0 like fvec_L2sqr, src/simd/distances_ref.cc:31-38).
 //
-// This file holds the fp32 CUDA-core contraction (bit-for-bit deterministic); the tcgen05
+// This file holds the fp32 CUDA-core contraction (bit-for-bit deterministic); the wgmma
 // tensor-core contraction lives in kb2_gemm_tc.cuh and produces the same key matrix.
 #pragma once
 #include "kb2_topk.cuh"

@@ -1,4 +1,4 @@
-// kb2_gemm_tc.cuh — the dense query x base contraction on the 5th-generation tensor cores.
+// kb2_gemm_tc.cuh — the dense query x base contraction on the Hopper tensor cores (wgmma).
 //
 //   keys[q][j] = |q|^2 + |x_j|^2 - 2 <q, x_j>   (L2)        keys[q][j] = -<q, x_j>   (IP)
 //
@@ -6,18 +6,17 @@
 // fp32 reference / fallback (d % 4 != 0).  Used by FLAT, BruteForce and the IVF coarse quantizer
 // (reference: F/utils/distances.cpp:326-363,834-875; F/IndexIVF.cpp:336-342).
 //
-// sm_100a mapping
+// sm_90a mapping
 //   * operands: fp32 rows, K-major.  TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) brings 128 x 32-float
-//     boxes (one 128-byte swizzle row per tensor row) of Q and X into a 3-stage shared-memory ring.
-//   * fp32 fidelity on a tf32 pipe: 4 "converter" warps split every element into hi = top 19 bits and
-//     lo = x - hi (both rounded to tf32), writing hi in place and lo to a twin tile; the MMA warp issues
-//     D += hi*hi + hi*lo + lo*hi  (3 x tcgen05.mma.kind::tf32, M=128 N=128 K=8) — error ~2^-21 relative,
-//     and the k+16 best candidates are re-ranked exactly afterwards anyway (finalize_kernel).
-//   * accumulator: 128 lanes x 128 columns of TMEM (fp32); tcgen05.commit signals stage release and
-//     accumulator completion through mbarriers; the same 4 warps then drain TMEM with tcgen05.ld
-//     (32x32b.x32), apply the key epilogue (+norms, bitset) and store 128-bit rows.
+//     boxes (one 128-byte swizzle row per tensor row) of Q and X into a shared-memory ring; warp 8 is the producer.
+//   * fp32 fidelity on a tf32 pipe: the two consumer warpgroups split every element into hi = top 19 bits and
+//     lo = x - hi (both rounded to tf32), writing hi in place and lo to a twin tile, then issue
+//     D += hi*hi + hi*lo + lo*hi  (3 x wgmma m64n128k8 tf32 per k-step, warpgroup w owns rows 64w..64w+63) — error
+//     ~2^-21 relative, and the k+16 best candidates are re-ranked exactly afterwards anyway (finalize_kernel).
+//   * accumulator: 64 fp32 registers per thread; the split of stage i+1 runs while the wgmmas of stage i are in flight
+//     (wgmma.wait_group 1), then the same threads apply the key epilogue (+norms, bitset) straight from registers.
 //   * one 128x128 output tile per CTA (K = d is short: 4 k-blocks at d=128, so the kernel is bound by
-//     operand/epilogue traffic, not by the tensor pipe — see DESIGN.md 4.1).
+//     operand/epilogue traffic, not by the tensor pipe).
 #pragma once
 #include <cuda.h>
 
@@ -30,14 +29,14 @@ constexpr int BM = 128, BN = 128, BK = 32;
 constexpr int STAGES = 3;                      // ring depth of the long-K instantiation (1 CTA/SM)
 constexpr int TILE_BYTES = 128 * BK * 4;       // 16 KB: a 128-row x 128-byte tile (A or B)
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;    // A_hi | B_hi | A_lo | B_lo
-constexpr int THREADS = 192;                   // warp 0: TMA   warp 1: MMA + TMEM alloc   warps 2-5: convert + epilogue
-constexpr int CONV_THREADS = 128;
-constexpr int TMEM_COLS = 128;
+constexpr int THREADS = 288;                   // warps 0-7: two consumer warpgroups (split + wgmma + epilogue)   warp 8: TMA
+constexpr int CONS_THREADS = 256;
+constexpr int PRODUCER_WARP = 8;
 constexpr size_t smem_bytes(int nst) { return (size_t)nst * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/; }
 constexpr size_t SMEM_BYTES = smem_bytes(STAGES);
-// Short contractions (d <= 192: the IVF coarse quantizer, k-means assignment) run a single-stage instantiation with three
-// CTAs per SM instead: a 128x128 tile is then ~8 us of strictly serial TMA -> split -> MMA -> store, and with one CTA per SM
-// (ncu r2: 9 % warps active, 17 waves) nothing overlaps the 64 KB epilogue store; three resident CTAs overlap each other.
+// Short contractions (d <= 192: the IVF coarse quantizer, k-means assignment) run a single-stage instantiation with two
+// CTAs per SM instead: a 128x128 tile is then a strictly serial TMA -> split -> MMA -> store chain, and a second resident
+// CTA overlaps its epilogue store with the other's loads.
 
 __device__ __forceinline__ uint32_t
 smem_u32(const void* p) {
@@ -80,47 +79,80 @@ __device__ __forceinline__ void
 fence_proxy_async() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// ---------------------------------------------------------------- wgmma (sm_90a)
 __device__ __forceinline__ void
-tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+wgmma_fence() {
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
 __device__ __forceinline__ void
-tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+wgmma_commit() {
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
+template <int N>
 __device__ __forceinline__ void
-tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by ONE thread
+// keeps the compiler from moving accesses of a wgmma accumulator across wgmma issue / wait (the registers are written
+// asynchronously between the two)
+template <int N>
 __device__ __forceinline__ void
-tc_mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+fence_operand(float (&acc)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; i++) asm volatile("" : "+f"(acc[i])::"memory");
 }
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart, sm_100 version bit
+// wgmma shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (tile base 1024-byte aligned; a K step
+// inside the 128-byte swizzle row advances the start address)
 __device__ __forceinline__ uint64_t
 make_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address, 16-byte units        bits  0-13
     d |= (uint64_t)1 << 16;                         // leading byte offset (unused here)   bits 16-29
     d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset = 1024 B         bits 32-45
-    d |= (uint64_t)1 << 46;                         // descriptor version 1 (sm_100)       bits 46-47
-    d |= (uint64_t)2 << 61;                         // layout type SWIZZLE_128B            bits 61-63
+    d |= (uint64_t)1 << 62;                         // layout type SWIZZLE_128B            bits 62-63
     return d;
 }
-// instruction descriptor: D=f32, A=B=tf32, both K-major, M=128, N=128
-__device__ __forceinline__ uint32_t
-make_idesc() {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+// D (+)= A * B, one warpgroup, A = 64 rows, B = N rows, both K-major in shared memory; D in registers (fragment layout:
+// d[4 j + 2 i + c] = row 16 (warp % 4) + lane / 4 + 8 i, column 8 j + 2 (lane % 4) + c)
+__device__ __forceinline__ void
+wgmma_tf32_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
 }
-
+__device__ __forceinline__ void
+wgmma_tf32_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+__device__ __forceinline__ void
+wgmma_bf16_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
 // round-to-nearest into the 19-bit tf32 container (low 13 mantissa bits cleared)
 __device__ __forceinline__ float
 tf32_rn(float x) {
@@ -128,7 +160,7 @@ tf32_rn(float x) {
 }
 
 template <int METRIC, int STAGES = 3>
-__global__ void __launch_bounds__(THREADS, STAGES == 1 ? 3 : 1)
+__global__ void __launch_bounds__(THREADS, STAGES == 1 ? 2 : 1)
 gemm_keys_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                     const float* __restrict__ qn, const float* __restrict__ xn, int nq, int nb, int d,
                     float* __restrict__ keys, int64_t ldk, const uint8_t* __restrict__ bitset,
@@ -138,13 +170,9 @@ gemm_keys_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     const uint32_t base = (raw + 1023u) & ~1023u;          // SWIZZLE_128B tiles need 1024-byte alignment
     unsigned char* base_ptr = smem_dyn + (base - raw);
     const uint32_t bars = base + STAGES * STAGE_BYTES;      // barrier block after the ring
-    // barrier layout (8 bytes each): full_raw[S] | full_conv[S] | empty[S] | tmem_full | tmem slot(4B)
-    auto bar_full_raw = [&](int s) { return bars + 8u * s; };
-    auto bar_full_conv = [&](int s) { return bars + 8u * (STAGES + s); };
-    auto bar_empty = [&](int s) { return bars + 8u * (2 * STAGES + s); };
-    const uint32_t bar_tmem_full = bars + 8u * (3 * STAGES);
-    const uint32_t tmem_slot = bars + 8u * (3 * STAGES + 1);
-    volatile uint32_t* tmem_slot_ptr = (volatile uint32_t*)(base_ptr + STAGES * STAGE_BYTES + 8 * (3 * STAGES + 1));
+    // barrier layout (8 bytes each): full[S] | empty[S]
+    auto bar_full = [&](int s) { return bars + 8u * s; };
+    auto bar_empty = [&](int s) { return bars + 8u * (STAGES + s); };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.y * BM;
@@ -153,24 +181,14 @@ gemm_keys_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; s++) {
-            mbar_init(bar_full_raw(s), 1);
-            mbar_init(bar_full_conv(s), CONV_THREADS);
-            mbar_init(bar_empty(s), 1);
+            mbar_init(bar_full(s), 1);
+            mbar_init(bar_empty(s), CONS_THREADS);
         }
-        mbar_init(bar_tmem_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         // ================= TMA producer =================
         if (lane == 0) {
             for (int it = 0; it < nkb; it++) {
@@ -178,118 +196,101 @@ gemm_keys_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                 const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
                 mbar_wait(bar_empty(s), ph ^ 1u);
                 const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
-                mbar_expect_tx(bar_full_raw(s), 2 * TILE_BYTES);
-                tma_load_2d(st, &tmap_q, it * BK, q0, bar_full_raw(s));                  // A_hi slot (raw fp32)
-                tma_load_2d(st + TILE_BYTES, &tmap_x, it * BK, j0, bar_full_raw(s));     // B_hi slot (raw fp32)
+                mbar_expect_tx(bar_full(s), 2 * TILE_BYTES);
+                tma_load_2d(st, &tmap_q, it * BK, q0, bar_full(s));                  // A_hi slot (raw fp32)
+                tma_load_2d(st + TILE_BYTES, &tmap_x, it * BK, j0, bar_full(s));     // B_hi slot (raw fp32)
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        const uint32_t idesc = make_idesc();
-        for (int it = 0; it < nkb; it++) {
-            const int s = it % STAGES;
-            const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-            mbar_wait(bar_full_conv(s), ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
-#pragma unroll
-                for (int kk = 0; kk < BK / 8; kk++) {
-                    const uint32_t ko = (uint32_t)kk * 32u;   // 8 tf32 = 32 bytes inside the 128-byte swizzle row
-                    const uint64_t a_hi = make_desc(st + ko);
-                    const uint64_t b_hi = make_desc(st + TILE_BYTES + ko);
-                    const uint64_t a_lo = make_desc(st + 2 * TILE_BYTES + ko);
-                    const uint64_t b_lo = make_desc(st + 3 * TILE_BYTES + ko);
-                    tc_mma_tf32(tmem_base, a_hi, b_hi, idesc, (it > 0 || kk > 0) ? 1u : 0u);
-                    tc_mma_tf32(tmem_base, a_hi, b_lo, idesc, 1u);
-                    tc_mma_tf32(tmem_base, a_lo, b_hi, idesc, 1u);
-                }
-                tc_commit(bar_empty(s));                       // frees the smem stage when these MMAs retire
-                if (it == nkb - 1) tc_commit(bar_tmem_full);   // accumulator complete
-            }
-            __syncwarp();
-        }
-    } else {
-        // ================= converters (hi/lo split), then epilogue =================
-        const int t = threadIdx.x - 64;  // 0..127
-        for (int it = 0; it < nkb; it++) {
-            const int s = it % STAGES;
-            const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-            mbar_wait(bar_full_raw(s), ph);
-            float4* hi = reinterpret_cast<float4*>(base_ptr + (size_t)s * STAGE_BYTES);        // A_hi|B_hi contiguous
-            float4* lo = reinterpret_cast<float4*>(base_ptr + (size_t)s * STAGE_BYTES + 2 * TILE_BYTES);
-#pragma unroll 4
-            for (int i = t; i < 2 * TILE_BYTES / 16; i += CONV_THREADS) {
-                float4 v = hi[i];
-                float4 h, l;
-                // hi = x rounded to tf32 (nearest), lo = (x - hi) rounded to tf32: both exactly representable,
-                // so the tensor core's own truncation of the low 13 bits changes nothing
-                h.x = tf32_rn(v.x); l.x = tf32_rn(v.x - h.x);
-                h.y = tf32_rn(v.y); l.y = tf32_rn(v.y - h.y);
-                h.z = tf32_rn(v.z); l.z = tf32_rn(v.z - h.z);
-                h.w = tf32_rn(v.w); l.w = tf32_rn(v.w - h.w);
-                hi[i] = h;
-                lo[i] = l;
-            }
-            fence_proxy_async();            // generic-proxy writes -> visible to the tensor core (async proxy)
-            mbar_arrive(bar_full_conv(s));
-        }
-        // ---- epilogue: TMEM -> registers -> keys
-        mbar_wait(bar_tmem_full, 0);
-        tc_fence_after();
-        const int quarter = warp & 3;                       // TMEM lane quarter this warp may access
-        const int row = q0 + quarter * 32 + lane;
-        const float qq = (METRIC == KB2_METRIC_L2 && row < nq) ? qn[row] : 0.f;
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                  "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                  "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-                  "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-                  "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (row < nq) {
-                float* out = keys + (int64_t)row * ldk + j0 + c;
-#pragma unroll
-                for (int v4 = 0; v4 < 8; v4++) {
-                    float o[4];
-#pragma unroll
-                    for (int u = 0; u < 4; u++) {
-                        const int col = j0 + c + v4 * 4 + u;
-                        const float acc = __uint_as_float(r[v4 * 4 + u]);
-                        float key = INFINITY;
-                        if (col < nb) {
-                            key = (METRIC == KB2_METRIC_L2) ? (qq + xn[col] - 2.f * acc) : -acc;
-                            if (bitset) {
-                                const int64_t rr = rows ? (int64_t)rows[row_base + col] : (row_base + col);
-                                if (bit_is_set(bitset, rr)) key = INFINITY;
-                            }
-                        }
-                        o[u] = key;
-                    }
-                    const int col0 = j0 + c + v4 * 4;
-                    if (col0 + 3 < ldk) {
-                        *reinterpret_cast<float4*>(out + v4 * 4) = make_float4(o[0], o[1], o[2], o[3]);
-                    } else {
-                        for (int u = 0; u < 4; u++)
-                            if (col0 + u < ldk) out[v4 * 4 + u] = o[u];
-                    }
-                }
-            }
-        }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+    // ================= consumers: hi/lo split, wgmma, epilogue =================
+    const int t = threadIdx.x;           // 0..255
+    const int wg = t >> 7;               // warpgroup: rows 64 wg .. 64 wg + 63 of the tile
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] = 0.f;
+    for (int it = 0; it < nkb; it++) {
+        const int s = it % STAGES;
+        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
+        mbar_wait(bar_full(s), ph);
+        float4* hi = reinterpret_cast<float4*>(base_ptr + (size_t)s * STAGE_BYTES);        // A_hi|B_hi contiguous
+        float4* lo = reinterpret_cast<float4*>(base_ptr + (size_t)s * STAGE_BYTES + 2 * TILE_BYTES);
+#pragma unroll 4
+        for (int i = t; i < 2 * TILE_BYTES / 16; i += CONS_THREADS) {
+            float4 v = hi[i];
+            float4 h, l;
+            // hi = x rounded to tf32 (nearest), lo = (x - hi) rounded to tf32: both exactly representable,
+            // so the tensor core's own truncation of the low 13 bits changes nothing
+            h.x = tf32_rn(v.x); l.x = tf32_rn(v.x - h.x);
+            h.y = tf32_rn(v.y); l.y = tf32_rn(v.y - h.y);
+            h.z = tf32_rn(v.z); l.z = tf32_rn(v.z - h.z);
+            h.w = tf32_rn(v.w); l.w = tf32_rn(v.w - h.w);
+            hi[i] = h;
+            lo[i] = l;
+        }
+        fence_proxy_async();            // generic-proxy writes -> visible to the tensor core (async proxy)
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // both halves of the stage are split
+        const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
+        const uint32_t a_off = (uint32_t)wg * 64u * 128u;
+        fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 8; kk++) {
+            const uint32_t ko = (uint32_t)kk * 32u;   // 8 tf32 = 32 bytes inside the 128-byte swizzle row
+            const uint64_t a_hi = make_desc(st + a_off + ko);
+            const uint64_t b_hi = make_desc(st + TILE_BYTES + ko);
+            const uint64_t a_lo = make_desc(st + 2 * TILE_BYTES + a_off + ko);
+            const uint64_t b_lo = make_desc(st + 3 * TILE_BYTES + ko);
+            wgmma_tf32_n128(acc, a_hi, b_hi, (it > 0 || kk > 0) ? 1u : 0u);
+            wgmma_tf32_n128(acc, a_hi, b_lo, 1u);
+            wgmma_tf32_n128(acc, a_lo, b_hi, 1u);
+        }
+        wgmma_commit();
+        fence_operand(acc);
+        if constexpr (STAGES == 1) {
+            wgmma_wait<0>();
+            mbar_arrive(bar_empty(s));
+        } else {
+            // the previous stage's wgmmas have retired once at most one group is pending: release its slot
+            wgmma_wait<1>();
+            if (it > 0) mbar_arrive(bar_empty((it - 1) % STAGES));
+        }
+    }
+    wgmma_wait<0>();
+    fence_operand(acc);
+    // ---- epilogue: registers -> keys
+    const int r0 = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int row = r0 + 8 * i;
+        if (row >= nq) continue;
+        const float qq = (METRIC == KB2_METRIC_L2) ? qn[row] : 0.f;
+        float* out = keys + (int64_t)row * ldk;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+            const int col0 = j0 + j * 8 + 2 * (lane & 3);
+            float o[2];
+#pragma unroll
+            for (int c = 0; c < 2; c++) {
+                const int col = col0 + c;
+                const float a = acc[4 * j + 2 * i + c];
+                float key = INFINITY;
+                if (col < nb) {
+                    key = (METRIC == KB2_METRIC_L2) ? (qq + xn[col] - 2.f * a) : -a;
+                    if (bitset) {
+                        const int64_t rr = rows ? (int64_t)rows[row_base + col] : (row_base + col);
+                        if (bit_is_set(bitset, rr)) key = INFINITY;
+                    }
+                }
+                o[c] = key;
+            }
+            if (col0 + 1 < ldk && (ldk & 1) == 0) {
+                *reinterpret_cast<float2*>(out + col0) = make_float2(o[0], o[1]);
+            } else {
+                for (int c = 0; c < 2; c++)
+                    if (col0 + c < ldk) out[col0 + c] = o[c];
+            }
+        }
     }
 }
 

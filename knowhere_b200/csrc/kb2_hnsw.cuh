@@ -1528,7 +1528,7 @@ struct HnswIndex : IndexBase {
         L.smem = kHnswWarps * ((size_t)dpad * 4 + (size_t)ef_cap * (two_pools ? 16 : 8));
         KB2_REQUIRE(L.smem <= (size_t)kMaxDynSmem, KB2_OUT_OF_RANGE_IN_JSON, "ef / dim too large for shared memory");
         const int ctas_per_sm = (int)std::max<size_t>(1, std::min<size_t>(8, (size_t)kMaxDynSmem / std::max<size_t>(L.smem, 1)));
-        L.grid = (int)std::min<int64_t>((nq + kHnswWarps - 1) / kHnswWarps, (int64_t)kNumSMs * ctas_per_sm);
+        L.grid = (int)std::min<int64_t>((nq + kHnswWarps - 1) / kHnswWarps, (int64_t)num_sms() * ctas_per_sm);
         L.total_warps = (int64_t)L.grid * kHnswWarps;
         L.nwords = (n + 31) / 32;
         L.log_cap = (int)std::min<int64_t>(n, (int64_t)ef_cap * h_cum[1] * 4 + 256);

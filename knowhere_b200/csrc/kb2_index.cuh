@@ -279,7 +279,7 @@ dense_candidates(IndexBase& ix, const float* Q, int64_t nq, const float* X, cons
     if (chunk < n) chunk = std::max<int64_t>(128, chunk / 128 * 128);
     const int64_t ldk = (chunk + 3) & ~(int64_t)3;   // 16-byte aligned key rows (vector stores in the epilogues)
     ix.s_keys.ensure((size_t)nq * ldk);
-    int nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * kNumSMs + nq - 1) / nq),
+    int nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nq - 1) / nq),
                                         std::max<int64_t>(1, chunk / 512));
     nsplit = std::min(nsplit, pl.S - 1);
     {
@@ -290,8 +290,7 @@ dense_candidates(IndexBase& ix, const float* Q, int64_t nq, const float* X, cons
         KB2_CUDA_CHECK(cudaMemset2DAsync(ix.s_partial.p, (size_t)pl.stride() * 8, 0xFF, (size_t)slots * pl.Ksel * 8, (size_t)nq, st));
     }
     const size_t sel_smem = (size_t)kScanWarps * 2 * pl.Ksel * 8;
-    // chunk-minimum fast path of the wide select (KB2_SELECT_FAST=0: level-wise histogram only).  Measured at C3's coarse stage
-    // (ncu, profiles/r2_summary.md): 0.218 ms -> 0.123 (128-bit loads) -> 0.087 (fast path)
+    // chunk-minimum fast path of the wide select (KB2_SELECT_FAST=0: level-wise histogram only)
     static const bool select_fast = [] { const char* e = getenv("KB2_SELECT_FAST"); return !(e && atoi(e) == 0); }();
     for (int64_t c0 = 0; c0 < n; c0 += chunk) {
         const int64_t cols = std::min(chunk, n - c0);
@@ -345,8 +344,8 @@ launch_finalize(IndexBase& ix, FinalizeParams fp, int64_t nq) {
     }
     const size_t smem = (size_t)fp.n_sort * 8 + (size_t)fp.k_sel * 16 + (size_t)fp.d * 4 + 16;
     unsigned grid = (unsigned)nq;
-    if (fp.split_small > 0 && nq > 8 * kNumSMs) {   // tail pass: a few CTAs per SM walk the rows, most of which they skip
-        grid = 8u * kNumSMs;
+    if (fp.split_small > 0 && nq > 8 * num_sms()) {   // tail pass: a few CTAs per SM walk the rows, most of which they skip
+        grid = 8u * num_sms();
         fp.row_loop_nq = nq;
     }
     finalize_kernel<<<grid, 256, smem, ix.stream>>>(fp);
@@ -950,7 +949,7 @@ struct IvfIndex : IndexBase {
                 pqtc::transpose_codebook_kernel<<<grid1d((int64_t)M * 256 * dsub, 256), 256, 0, st>>>(pqc.p, M, dsub, tc_pqc_t.p);
             }
             if (metric == KB2_METRIC_L2 && npad > 0)
-                pqtc::max_abs_kernel<<<kNumSMs * 2, 256, 0, st>>>(t1.p, npad, (uint32_t*)(tc_maxn2.p + M));
+                pqtc::max_abs_kernel<<<num_sms() * 2, 256, 0, st>>>(t1.p, npad, (uint32_t*)(tc_maxn2.p + M));
             if (dsub < 8) {
                 tc_codes_plain.alloc_exact((size_t)G * npad * 16);
                 pqtc::unrotate_codes_kernel<<<grid1d((int64_t)G * npad * 16, 256), 256, 0, st>>>(codes.p, (int64_t)G * npad, npad,
@@ -1012,17 +1011,16 @@ struct IvfIndex : IndexBase {
             pqtc::fill_f32_kernel<<<grid1d(nq, 256), 256, 0, st>>>(s_bound.p, nq, INFINITY);
             qlist = s_resp.p + 1;
             qcount = (const uint32_t*)s_resp.p;
-            bound_grid = (unsigned)std::min<int64_t>(nq, std::max<int64_t>(4 * kNumSMs, 2 * nq / shard_world));
+            bound_grid = (unsigned)std::min<int64_t>(nq, std::max<int64_t>(4 * num_sms(), 2 * nq / shard_world));
             last.launches += 2;
         }
         {
             const char* e_rw = getenv("KB2_BOUND_ROWW");
-            const int roww = (e_rw && atoi(e_rw) == 64) ? 64 : 32;   // measured at C3: 0.37 ms (32, 3 CTAs/SM) vs 0.52 ms (64, 2 CTAs/SM)
+            const int roww = (e_rw && atoi(e_rw) == 64) ? 64 : 32;   // 32 rows: 3 CTAs/SM, 64 rows: 2 CTAs/SM
             const size_t smem = pqtc::bound_smem(roww, pqtc::bound_kmax(a_codes, k_base));
-            // measured at C3 (profiles/r2_summary.md): 0.274 ms with 128 threads, 0.234 ms with 256
             static const int bound_nt = [] { const char* e = getenv("KB2_BOUND_NT"); return e ? atoi(e) : 256; }();
 #define KB2_BOUND_LAUNCH(MM, RW)                                                                                                    \
-    pqtc::lut_build_kernel<MM><<<kNumSMs, 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
+    pqtc::lut_build_kernel<MM><<<num_sms(), 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
     mark("lut");                                                                                                                    \
     pqtc::bound_kernel<MM, RW><<<bound_grid, 128, smem, st>>>(s_lut.p, qlist, qcount, nq, sp.probe_ids, sp.probe_dis, nprobe, p0,   \
                                                              a_codes, k_base, list_off.p, list_len.p, (const uint4*)codes.p, t1.p, \
@@ -1038,7 +1036,7 @@ struct IvfIndex : IndexBase {
             } else if (bound_nt == 256 && roww == 32) {
                 // 8 warps per CTA over the same tables (default; KB2_BOUND_NT=128 for the 4-warp instance)
 #define KB2_BOUND_LAUNCH256(MM)                                                                                                     \
-    pqtc::lut_build_kernel<MM><<<kNumSMs, 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
+    pqtc::lut_build_kernel<MM><<<num_sms(), 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
     mark("lut");                                                                                                                    \
     pqtc::bound_kernel<MM, 32, 1, 8, 256><<<bound_grid, 256, smem, st>>>(s_lut.p, qlist, qcount, nq, sp.probe_ids, sp.probe_dis,     \
                                                                          nprobe, p0, a_codes, k_base, list_off.p, list_len.p,       \
@@ -1097,7 +1095,7 @@ struct IvfIndex : IndexBase {
             // per tile: decode ~ constant, contraction ~ columns (+ the test K-step)
             // dynamic draw (default): items in descending cost order, CTAs take the next one when free; KB2_TC_SCHED=static
             // keeps the fixed round-robin assignment with the snake deal
-            int32_t* bal = balance_items(s_items.p, max_items, tc_dynamic_sched() ? 0 : kNumSMs, 600, 5, ps);
+            int32_t* bal = balance_items(s_items.p, max_items, tc_dynamic_sched() ? 0 : num_sms(), 600, 5, ps);
             item_list = bal;
             item_q0 = bal + max_items;
             item_nq = bal + 2 * max_items;
@@ -1144,7 +1142,7 @@ struct IvfIndex : IndexBase {
         tp.pqc16 = (const uint4*)tc_pqc16.p;
         tp.bitset = sp.bitset;
         tp.rows = rows.p;
-        const int n_logs = 2 * kNumSMs;   // one per epilogue group (+ 1 legacy slot that stays empty)
+        const int n_logs = 2 * num_sms();   // one per epilogue group (+ 1 legacy slot that stays empty)
         const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(nq * 1024 / n_logs, 16384), 1 << 19);
         s_log.ensure((size_t)(n_logs + 1) * log_cap);
         s_logcnt.ensure(n_logs + 8);
@@ -1158,9 +1156,9 @@ struct IvfIndex : IndexBase {
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
 #define KB2_TC_LAUNCH(GG, DD)                                                                                                         \
     if (metric == KB2_METRIC_L2)                                                                                                     \
-        pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_L2, GG, DD><<<kNumSMs, pqtc::THREADS, pqtc::TcCfg<GG, DD>::SMEM_BYTES, st>>>(tp);    \
+        pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_L2, GG, DD><<<num_sms(), pqtc::THREADS, pqtc::TcCfg<GG, DD>::SMEM_BYTES, st>>>(tp);    \
     else                                                                                                                             \
-        pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, GG, DD><<<kNumSMs, pqtc::THREADS, pqtc::TcCfg<GG, DD>::SMEM_BYTES, st>>>(tp);
+        pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, GG, DD><<<num_sms(), pqtc::THREADS, pqtc::TcCfg<GG, DD>::SMEM_BYTES, st>>>(tp);
         if (tc_geom_18()) { KB2_TC_LAUNCH(1, 8) } else { KB2_TC_LAUNCH(3, 2) }
 #undef KB2_TC_LAUNCH
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev3, st));
@@ -1201,7 +1199,7 @@ struct IvfIndex : IndexBase {
             f.qperm = nullptr;
             f.lut_global = nullptr;   // the redo pass builds its own tables (a handful of queries)
             f.counters = d_counter.p + 4;
-            launch_scan(f, (unsigned)std::min<int64_t>(nq * f.nsplit, 3 * kNumSMs), Ksel, (nprobe + f.nsplit - 1) / f.nsplit, has_bits);
+            launch_scan(f, (unsigned)std::min<int64_t>(nq * f.nsplit, 3 * num_sms()), Ksel, (nprobe + f.nsplit - 1) / f.nsplit, has_bits);
         }
         mark("fallback");
         if (verbose) {
@@ -1281,7 +1279,7 @@ struct IvfIndex : IndexBase {
         int32_t* item_nq = s_items.p + 2 * max_items;
         fltc::plan_kernel<<<1, 1024, 0, st>>>(s_lcount.p, (int)nlist, item_cap, s_lstart.p, item_list, item_q0, item_nq, s_plan_out.p);
         {
-            int32_t* bal = balance_items(s_items.p, max_items, tc_dynamic_sched() ? 0 : kNumSMs, 1000, 2);   // a tile is bound by its HBM stream
+            int32_t* bal = balance_items(s_items.p, max_items, tc_dynamic_sched() ? 0 : num_sms(), 1000, 2);   // a tile is bound by its HBM stream
             item_list = bal;
             item_q0 = bal + max_items;
             item_nq = bal + 2 * max_items;
@@ -1315,17 +1313,17 @@ struct IvfIndex : IndexBase {
         fpar.xnorm2 = vnorm2.p;
         fpar.bitset = sp.bitset;
         fpar.rows = rows.p;
-        const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(nq * 1024 / kNumSMs, 32768), 1 << 20);
-        s_log.ensure((size_t)kNumSMs * log_cap);
-        s_logcnt.ensure(kNumSMs + 8);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (kNumSMs + 8) * 4, st));
+        const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(nq * 1024 / num_sms(), 32768), 1 << 20);
+        s_log.ensure((size_t)num_sms() * log_cap);
+        s_logcnt.ensure(num_sms() + 8);
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (num_sms() + 8) * 4, st));
         fpar.log = s_log.p;
         fpar.log_cnt = s_logcnt.p;
         fpar.log_cap = log_cap;
         fpar.counters = d_counter.p;
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
 #define KB2_FL_LAUNCH(MM, BR) \
-    fltc::ivfflat_tc_kernel<MM, BR><<<kNumSMs, fltc::THREADS, fltc::FlCfg<BR>::SMEM_BYTES, st>>>(tx, thi, tlo, fpar);
+    fltc::ivfflat_tc_kernel<MM, BR><<<num_sms(), fltc::THREADS, fltc::FlCfg<BR>::SMEM_BYTES, st>>>(tx, thi, tlo, fpar);
         if (metric == KB2_METRIC_L2) {
             if (item_cap == 32) { KB2_FL_LAUNCH(KB2_METRIC_L2, 32) } else { KB2_FL_LAUNCH(KB2_METRIC_L2, 128) }
         } else {
@@ -1335,8 +1333,8 @@ struct IvfIndex : IndexBase {
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev3, st));
         KB2_CUDA_CHECK(cudaGetLastError());
         uint32_t* qflag = s_cand_cnt.p + nq;
-        fltc::scatter_kernel<<<dim3(16, kNumSMs), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p, kTcCandCap, qflag);
-        fltc::count_flags_kernel<<<grid1d(nq, 256), 256, 0, st>>>(qflag, nq, s_logcnt.p + kNumSMs, s_cand_cnt.p + 2 * nq);
+        fltc::scatter_kernel<<<dim3(16, num_sms()), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p, kTcCandCap, qflag);
+        fltc::count_flags_kernel<<<grid1d(nq, 256), 256, 0, st>>>(qflag, nq, s_logcnt.p + num_sms(), s_cand_cnt.p + 2 * nq);
         last.launches += 9;
         uint32_t* hflag = (uint32_t*)h_counter.p + 12;
         KB2_CUDA_CHECK(cudaMemcpyAsync(hflag, s_cand_cnt.p + 2 * nq, 4, cudaMemcpyDeviceToHost, st));
@@ -1362,8 +1360,8 @@ struct IvfIndex : IndexBase {
         const char* e = getenv("KB2_COARSE");
         if (coarse_tc_disabled || (e && !strcmp(e, "dense"))) return false;
         if (dim % fltc::BK != 0 || nlist < 1024 || nprobe + 16 > 256 || nprobe + 16 > nlist / 8) return false;
-        // opt-in (KB2_COARSE=tc): measured at C3 (10000 x 4096 centroids) the list-major kernel + its sample bound cost
-        // 0.75 ms against 0.43 ms of the dense GEMM + select it would replace (profiles/r2_summary.md)
+        // opt-in (KB2_COARSE=tc): at C3 (10000 x 4096 centroids) the list-major kernel + its sample bound cost more than the
+        // dense GEMM + select it would replace
         return e && !strcmp(e, "tc") && m >= 296;
     }
     void
@@ -1378,7 +1376,7 @@ struct IvfIndex : IndexBase {
         s_cbound.ensure((size_t)m);
         fltc::extract_bound_kernel<<<grid1d(m, 256), 256, 0, st>>>(s_partial.p, pl.stride(), k_sample, m, s_cbound.p);
         // ---- items: chunks of consecutive queries over the single pseudo-list [0, nlist)
-        const int item_cap = (m / 128 < 2 * kNumSMs) ? 32 : 128;
+        const int item_cap = (m / 128 < 2 * num_sms()) ? 32 : 128;
         const int64_t n_it = (m + item_cap - 1) / item_cap;
         const int64_t npairs_pad = m + fltc::NQ_ITEM;
         s_items.ensure((size_t)3 * n_it);
@@ -1428,11 +1426,11 @@ struct IvfIndex : IndexBase {
         fpar.xnorm2 = cnorms.p;
         fpar.bitset = nullptr;
         fpar.rows = nullptr;
-        const int grid = (int)std::min<int64_t>(kNumSMs, n_it);
+        const int grid = (int)std::min<int64_t>(num_sms(), n_it);
         const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(m * 1024 / grid, 32768), 1 << 20);
-        s_log.ensure((size_t)kNumSMs * log_cap);
-        s_logcnt.ensure(kNumSMs + 8);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (kNumSMs + 8) * 4, st));
+        s_log.ensure((size_t)num_sms() * log_cap);
+        s_logcnt.ensure(num_sms() + 8);
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (num_sms() + 8) * 4, st));
         fpar.log = s_log.p;
         fpar.log_cnt = s_logcnt.p;
         fpar.log_cap = log_cap;
@@ -1551,7 +1549,7 @@ struct IvfIndex : IndexBase {
         //      time probe the same lists (L2 reuse of codes; results are order-independent)
         const int32_t* qperm = nullptr;
         const bool tc_engine = use_tc_engine(nq, nprobe, next_pow2(std::max(32, k_base)));
-        if (nq >= 2 * kNumSMs && !tc_engine) {
+        if (nq >= 2 * num_sms() && !tc_engine) {
             s_qkey.ensure(nq); s_qkey2.ensure(nq); s_qidx.ensure(nq); s_qperm.ensure(nq);
             first_probe_kernel<<<grid1d(nq, 256), 256, 0, st>>>(s_probe_ids.p, nprobe, nq, s_qkey.p, s_qidx.p);
             size_t tmp_bytes = 0;
@@ -1567,7 +1565,7 @@ struct IvfIndex : IndexBase {
 
         // ---- list scan
         int nsplit = 1;
-        if (nq < 2 * kNumSMs) nsplit = (int)std::min<int64_t>(nprobe, (2 * kNumSMs + nq - 1) / nq);
+        if (nq < 2 * num_sms()) nsplit = (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq);
         const int Ksel = next_pow2(std::max(32, k_base));
         while ((int64_t)nsplit * Ksel > kMaxSortEntries) nsplit--;
         const int np_max = (nprobe + nsplit - 1) / nsplit;

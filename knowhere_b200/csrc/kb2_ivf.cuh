@@ -109,7 +109,7 @@ setup_probes(const IvfScanParams& p, int64_t q, int j0, int j1, ProbeSmem ps) {
     return (int)ps.start[np];
 }
 
-// Shared-window address of the dynamic shared memory of a non-cluster CTA on sm_100: the first
+// Shared-window address of the dynamic shared memory of a non-cluster CTA on sm_90 (as on every GPU since sm_80): the first
 // 1 KB of the window is reserved by the system, so `extern __shared__` starts at 0x400.  The scan
 // kernel checks this at run time (and reports through counters[1]) because the LUT gather folds
 // the base into the LDS immediate:  LDS dst, [ (code<<8 | lane<<2) + KB2_SMEM_BASE + g*64K + 4*s ].

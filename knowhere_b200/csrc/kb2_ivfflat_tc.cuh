@@ -6,18 +6,19 @@
 //
 // Here the query x list distance is what it is, a dense contraction: the (query, probe) pairs are grouped by list
 // (same plan as the IVF_PQ engine), and every list is read ONCE per batch — a [128 rows] x [N queries of the list] x d
-// tile product on tcgen05 with the operands brought by TMA.
+// tile product on the Hopper tensor cores (wgmma) with the operands brought by TMA.
 //   * A operand: 128 consecutive rows of the list, fp32, straight from the list-order vector store (TMA, 128-byte swizzle).
 //   * B operand: the item's queries, gathered pair-major beforehand and already split hi/lo (two TMA tiles).
-//   * fp32 fidelity on the tf32 pipe: converter warps split the A tile into hi = tf32(x), lo = tf32(x - hi); the MMA warp
-//     issues hi*hi + hi*lo + lo*hi (3 x kind::tf32, M=128, N=16..128, K=8), error ~2^-21 relative (kb2_gemm_tc.cuh).
-//   * accumulators: two 128-column TMEM buffers; the epilogue warps of tile i run under the MMAs of tile i+1.
+//   * fp32 fidelity on the tf32 pipe: each consumer warpgroup splits its 64 rows of the A tile into hi = tf32(x),
+//     lo = tf32(x - hi) and issues hi*hi + hi*lo + lo*hi (3 x wgmma m64nBROWSk8 tf32), error ~2^-21 relative
+//     (kb2_gemm_tc.cuh); the split of k-block i+1 runs while the wgmmas of k-block i are in flight.
+//   * accumulators: BROWS / 2 fp32 registers per thread; the producer keeps the stage ring full while the epilogue runs.
 //   * epilogue: key = |q|^2 + |x|^2 - 2 acc (L2) / -acc (IP); keys within the per-query admission bound (exact k-th best
 //     key of the query's nearest probed lists, from the query-major kernel, + a 3e-5 relative slack for the tf32 split)
 //     are logged as survivors; finalize_kernel re-ranks the k+16 best of them EXACTLY from the fp32 rows, so the result
 //     is the exact scan's (same guarantee as FLAT).
-// Work item = (list, <=128 of the queries probing it).  One persistent CTA per SM, 320 threads:
-//   warp 0 TMA producer | warp 1 MMA issuer + TMEM owner | warps 2-5 converters | warps 6-9 epilogue.
+// Work item = (list, <=128 of the queries probing it).  One persistent CTA per SM, 288 threads:
+//   warps 0-7 two consumer warpgroups (rows 0-63 | 64-127 of a tile: split, wgmma, epilogue) | warp 8 TMA producer.
 #pragma once
 #include "kb2_gemm_tc.cuh"
 #include "kb2_ivfpq_tc.cuh"
@@ -25,11 +26,12 @@
 namespace kb2 {
 namespace fltc {
 
-constexpr int TM = 128;         // list rows per tile (UMMA M)
-constexpr int NQ_ITEM = 128;    // most queries per item (UMMA N max)
+constexpr int TM = 128;         // list rows per tile (two wgmma M=64 halves)
+constexpr int NQ_ITEM = 128;    // most queries per item
 constexpr int BK = 32;          // floats per k-block (one 128-byte swizzle row)
 constexpr int TILE_BYTES = 128 * BK * 4;        // 16 KB: 128 rows of one k-block
-constexpr int THREADS = 320;
+constexpr int THREADS = 288;
+constexpr int PRODUCER_WARP = 8;
 // BROWS = query rows per item the instance is built for (its B tiles are BROWS x 128 B): 32 -> 40 KB stages, 5 in flight
 // (few queries per list: C2 has ~31); 128 -> 64 KB stages, 3 in flight.  The kernel is bound by the latency of the
 // TMA -> convert -> MMA -> release chain of a stage, so the number of stages in flight sets the HBM rate it reaches.
@@ -131,15 +133,18 @@ plan_kernel(const int32_t* __restrict__ lcount, int nlist, int item_cap, int32_t
     if (threadIdx.x == 0) *n_items = carry_b;
 }
 
-__device__ __forceinline__ uint32_t
-make_idesc_tf32(int n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
+template <int BROWS>
+__device__ __forceinline__ void
+wgmma_tf32(float (&acc)[BROWS / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    if constexpr (BROWS == 128) tc::wgmma_tf32_n128(acc, a_desc, b_desc, accumulate);
+    else tc::wgmma_tf32_n32(acc, a_desc, b_desc, accumulate);
 }
 
 template <int METRIC, int BROWS>
 __global__ void __launch_bounds__(THREADS, 1)
 ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_qhi,
                   const __grid_constant__ CUtensorMap tmap_qlo, Params p) {
+    static_assert(BROWS == 32 || BROWS == 128, "wgmma N of the IVF_FLAT engine");
     using C = FlCfg<BROWS>;
     constexpr int STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, B_TILE_BYTES = C::B_TILE_BYTES, OFF_META = C::OFF_META,
                   OFF_BAR = C::OFF_BAR;
@@ -148,22 +153,17 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     const uint32_t base = (raw + 1023u) & ~1023u;
     unsigned char* sm = smem_dyn + (base - raw);
     const uint32_t bars = base + OFF_BAR;
-    // barriers: full_raw[S] full_conv[S] empty[S] acc_full[2] acc_empty[2] | tmem slot
-    auto bar_full_raw = [&](int s) { return bars + 8u * s; };
-    auto bar_full_conv = [&](int s) { return bars + 8u * (STAGES + s); };
-    auto bar_empty = [&](int s) { return bars + 8u * (2 * STAGES + s); };
-    auto bar_acc_full = [&](int i) { return bars + 8u * (3 * STAGES + i); };
-    auto bar_acc_empty = [&](int i) { return bars + 8u * (3 * STAGES + 2 + i); };
-    const uint32_t tmem_slot = bars + 8u * (3 * STAGES + 4);
-    volatile uint32_t* tmem_slot_ptr = (volatile uint32_t*)(sm + OFF_BAR + 8 * (3 * STAGES + 4));
-    uint32_t* log_cursor = (uint32_t*)(sm + OFF_BAR + 8 * (3 * STAGES + 5));
+    // barriers: full[S] empty[S] | log cursor
+    auto bar_full = [&](int s) { return bars + 8u * s; };
+    auto bar_empty = [&](int s) { return bars + 8u * (STAGES + s); };
+    uint32_t* log_cursor = (uint32_t*)(sm + OFF_BAR + 8 * (2 * STAGES));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_items = *p.n_items;
     const int nkb = p.d / BK;
 
-    // item sequence of this CTA, drawn from a global counter and shared by the four roles (same scheme as the IVF_PQ filter
-    // kernel; the roles are < 16 items apart: the producer leads by at most STAGES k-blocks, the epilogue trails by 2 tiles)
+    // item sequence of this CTA, drawn from a global counter and shared by the two roles (same scheme as the IVF_PQ filter
+    // kernel; the roles are < 16 items apart: the producer leads by at most STAGES k-blocks)
     constexpr int SCHED_R = 32;
     int* sch_claim = (int*)(sm + OFF_BAR + 256);
     int* sch_item = sch_claim + SCHED_R;
@@ -196,27 +196,15 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; s++) {
-            tc::mbar_init(bar_full_raw(s), 1);
-            tc::mbar_init(bar_full_conv(s), 128);
-            tc::mbar_init(bar_empty(s), 1);
-        }
-        for (int i = 0; i < 2; i++) {
-            tc::mbar_init(bar_acc_full(i), 1);
-            tc::mbar_init(bar_acc_empty(i), 128);
+            tc::mbar_init(bar_full(s), 1);
+            tc::mbar_init(bar_empty(s), 256);
         }
         *log_cursor = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(256) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         // ================= TMA producer: per (item, tile, k-block) one stage = raw A tile + B_hi + B_lo =================
         if (lane == 0) {
             uint32_t it = 0;
@@ -231,178 +219,145 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                         const int s = it % STAGES;
                         pqtc::mbar_wait_g(bar_empty(s), ((it / STAGES) & 1u) ^ 1u);
                         const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
-                        tc::mbar_expect_tx(bar_full_raw(s), TILE_BYTES + 2 * B_TILE_BYTES);
-                        tc::tma_load_2d(st, &tmap_x, kb * BK, (int)(off + (int64_t)t * TM), bar_full_raw(s));
-                        tc::tma_load_2d(st + 2 * TILE_BYTES, &tmap_qhi, kb * BK, q0, bar_full_raw(s));
-                        tc::tma_load_2d(st + 2 * TILE_BYTES + B_TILE_BYTES, &tmap_qlo, kb * BK, q0, bar_full_raw(s));
+                        tc::mbar_expect_tx(bar_full(s), TILE_BYTES + 2 * B_TILE_BYTES);
+                        tc::tma_load_2d(st, &tmap_x, kb * BK, (int)(off + (int64_t)t * TM), bar_full(s));
+                        tc::tma_load_2d(st + 2 * TILE_BYTES, &tmap_qhi, kb * BK, q0, bar_full(s));
+                        tc::tma_load_2d(st + 2 * TILE_BYTES + B_TILE_BYTES, &tmap_qlo, kb * BK, q0, bar_full(s));
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        uint32_t it = 0, g = 0;
-        int seq = 0;
-        for (int item = item_at(0); item < n_items; item = item_at(++seq)) {
-            const int l = p.item_list[item];
-            const int nmma = (p.item_nq[item] + 15) & ~15;
-            const int ntiles = (p.list_len[l] + TM - 1) / TM;
-            const uint32_t idesc = make_idesc_tf32(nmma);
-            for (int t = 0; t < ntiles; t++, g++) {
-                const int buf = g & 1;
-                pqtc::mbar_wait_g(bar_acc_empty(buf), ((g >> 1) & 1u) ^ 1u);
-                for (int kb = 0; kb < nkb; kb++, it++) {
-                    const int s = it % STAGES;
-                    pqtc::mbar_wait_g(bar_full_conv(s), (it / STAGES) & 1u);
-                    tc::tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
-                        const uint32_t d_t = tmem_base + (uint32_t)buf * 128u;
+        return;
+    }
+    // ================= consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile; columns = the item's queries
+    const int ct = threadIdx.x;          // 0..255
+    const int wg = ct >> 7;
+    const int w128 = ct & 127;
+    float* m_thr = (float*)(sm + OFF_META);
+    float* m_base = m_thr + NQ_ITEM;
+    int* m_q = (int*)(m_base + NQ_ITEM);
+    uint4* my_log = p.log + (size_t)blockIdx.x * p.log_cap;
+    bool log_over = false;
+    unsigned long long n_rows = 0;
+    float acc[BROWS / 2];
 #pragma unroll
-                        for (int kk = 0; kk < BK / 8; kk++) {
-                            const uint32_t ko = (uint32_t)kk * 32u;
-                            const uint64_t a_hi = tc::make_desc(st + ko);
-                            const uint64_t a_lo = tc::make_desc(st + TILE_BYTES + ko);
-                            const uint64_t b_hi = tc::make_desc(st + 2 * TILE_BYTES + ko);
-                            const uint64_t b_lo = tc::make_desc(st + 2 * TILE_BYTES + B_TILE_BYTES + ko);
-                            tc::tc_mma_tf32(d_t, a_hi, b_hi, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-                            tc::tc_mma_tf32(d_t, a_hi, b_lo, idesc, 1u);
-                            tc::tc_mma_tf32(d_t, a_lo, b_hi, idesc, 1u);
-                        }
-                        tc::tc_commit(bar_empty(s));
-                        if (kb == nkb - 1) tc::tc_commit(bar_acc_full(buf));
-                    }
-                    __syncwarp();
-                }
+    for (int i = 0; i < BROWS / 2; i++) acc[i] = 0.f;
+    uint32_t it = 0;
+    int seq = 0;
+    for (int item = item_at(0); item < n_items; item = item_at(++seq)) {
+        const int l = p.item_list[item];
+        const int q0 = p.item_q0[item];
+        const int nqi = p.item_nq[item];
+        const int len = p.list_len[l];
+        const int64_t off = p.list_off[l];
+        const int ntiles = (len + TM - 1) / TM;
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // every consumer thread is done with the previous item's meta
+        if (ct < NQ_ITEM) {
+            // admit  <=>  key - slack * (|q|^2 + |x|^2) <= bound   (|q|^2 + |x|^2 >= 2 |q||x| bounds the 3xTF32 error scale)
+            float thr = -INFINITY, bs = 0.f;
+            int q = -1;
+            if (ct < nqi) {
+                q = p.pair_q[q0 + ct];
+                bs = p.qnorm2[q];
+                const float bnd = p.bound[q];
+                thr = (bnd < INFINITY) ? bnd + kSlack * bs + 1e-30f : INFINITY;
             }
+            m_thr[ct] = thr;
+            m_base[ct] = bs;
+            m_q[ct] = q;
         }
-    } else if (warp < 6) {
-        // ================= converters: split the raw A tile into hi (in place) and lo =================
-        const int t128 = threadIdx.x - 64;   // 0..127
-        uint32_t it = 0;
-        int seq = 0;
-        for (int item = item_at(0); item < n_items; item = item_at(++seq)) {
-            const int l = p.item_list[item];
-            const int ntiles = (p.list_len[l] + TM - 1) / TM;
-            for (int t = 0; t < ntiles; t++) {
-                for (int kb = 0; kb < nkb; kb++, it++) {
-                    const int s = it % STAGES;
-                    pqtc::mbar_wait_g(bar_full_raw(s), (it / STAGES) & 1u);
-                    float4* hi = reinterpret_cast<float4*>(sm + (size_t)s * STAGE_BYTES);
-                    float4* lo = reinterpret_cast<float4*>(sm + (size_t)s * STAGE_BYTES + TILE_BYTES);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (ct == 0) n_rows += (unsigned long long)len * (unsigned long long)nqi;
+        for (int t = 0; t < ntiles; t++) {
+            int pending = -1;   // stage whose wgmmas may still be in flight
+            for (int kb = 0; kb < nkb; kb++, it++) {
+                const int s = it % STAGES;
+                pqtc::mbar_wait_g(bar_full(s), (it / STAGES) & 1u);
+                // split this warpgroup's 64 rows of the raw A tile into hi (in place) and lo
+                float4* hi = reinterpret_cast<float4*>(sm + (size_t)s * STAGE_BYTES + wg * (TILE_BYTES / 2));
+                float4* lo = reinterpret_cast<float4*>(sm + (size_t)s * STAGE_BYTES + TILE_BYTES + wg * (TILE_BYTES / 2));
 #pragma unroll 4
-                    for (int i = t128; i < TILE_BYTES / 16; i += 128) {
-                        const float4 v = hi[i];
-                        float4 h, w;
-                        h.x = tc::tf32_rn(v.x); w.x = tc::tf32_rn(v.x - h.x);
-                        h.y = tc::tf32_rn(v.y); w.y = tc::tf32_rn(v.y - h.y);
-                        h.z = tc::tf32_rn(v.z); w.z = tc::tf32_rn(v.z - h.z);
-                        h.w = tc::tf32_rn(v.w); w.w = tc::tf32_rn(v.w - h.w);
-                        hi[i] = h;
-                        lo[i] = w;
-                    }
-                    tc::fence_proxy_async();
-                    tc::mbar_arrive(bar_full_conv(s));
+                for (int i = w128; i < TILE_BYTES / 32; i += 128) {
+                    const float4 v = hi[i];
+                    float4 h, w;
+                    h.x = tc::tf32_rn(v.x); w.x = tc::tf32_rn(v.x - h.x);
+                    h.y = tc::tf32_rn(v.y); w.y = tc::tf32_rn(v.y - h.y);
+                    h.z = tc::tf32_rn(v.z); w.z = tc::tf32_rn(v.z - h.z);
+                    h.w = tc::tf32_rn(v.w); w.w = tc::tf32_rn(v.w - h.w);
+                    hi[i] = h;
+                    lo[i] = w;
                 }
-            }
-        }
-    } else {
-        // ================= epilogue: thread = list row, columns = the item's queries =================
-        const int e = threadIdx.x - 192;     // 0..127
-        const int quarter = warp & 3;        // TMEM lane quarter this warp may access (warps 6..9 -> 2,3,0,1)
-        const int row = quarter * 32 + lane;
-        float* m_thr = (float*)(sm + OFF_META);
-        float* m_base = m_thr + NQ_ITEM;
-        int* m_q = (int*)(m_base + NQ_ITEM);
-        uint4* my_log = p.log + (size_t)blockIdx.x * p.log_cap;
-        bool log_over = false;
-        unsigned long long n_rows = 0;
-        uint32_t g = 0;
-        int seq = 0;
-        for (int item = item_at(0); item < n_items; item = item_at(++seq)) {
-            const int l = p.item_list[item];
-            const int q0 = p.item_q0[item];
-            const int nqi = p.item_nq[item];
-            const int nmma = (nqi + 15) & ~15;
-            const int nch = (nmma + 31) >> 5;
-            const int len = p.list_len[l];
-            const int64_t off = p.list_off[l];
-            const int ntiles = (len + TM - 1) / TM;
-            asm volatile("bar.sync 1, 128;" ::: "memory");   // every epilogue thread is done with the previous item's meta
-            {
-                // admit  <=>  key - slack * (|q|^2 + |x|^2) <= bound   (|q|^2 + |x|^2 >= 2 |q||x| bounds the 3xTF32 error scale)
-                float thr = -INFINITY, bs = 0.f;
-                int q = -1;
-                if (e < nqi) {
-                    q = p.pair_q[q0 + e];
-                    bs = p.qnorm2[q];
-                    const float bnd = p.bound[q];
-                    thr = (bnd < INFINITY) ? bnd + kSlack * bs + 1e-30f : INFINITY;
+                tc::fence_proxy_async();
+                if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+                else asm volatile("bar.sync 3, 128;" ::: "memory");
+                const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
+                const uint32_t a_off = (uint32_t)wg * (TILE_BYTES / 2);
+                tc::fence_operand(acc);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < BK / 8; kk++) {
+                    const uint32_t ko = (uint32_t)kk * 32u;
+                    const uint64_t a_hi = tc::make_desc(st + a_off + ko);
+                    const uint64_t a_lo = tc::make_desc(st + TILE_BYTES + a_off + ko);
+                    const uint64_t b_hi = tc::make_desc(st + 2 * TILE_BYTES + ko);
+                    const uint64_t b_lo = tc::make_desc(st + 2 * TILE_BYTES + B_TILE_BYTES + ko);
+                    wgmma_tf32<BROWS>(acc, a_hi, b_hi, (kb > 0 || kk > 0) ? 1u : 0u);
+                    wgmma_tf32<BROWS>(acc, a_hi, b_lo, 1u);
+                    wgmma_tf32<BROWS>(acc, a_lo, b_hi, 1u);
                 }
-                m_thr[e] = thr;
-                m_base[e] = bs;
-                m_q[e] = q;
+                tc::wgmma_commit();
+                tc::fence_operand(acc);
+                tc::wgmma_wait<1>();
+                if (pending >= 0) tc::mbar_arrive(bar_empty(pending));
+                pending = s;
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (e == 0) n_rows += (unsigned long long)len * (unsigned long long)nqi;
-            for (int t = 0; t < ntiles; t++, g++) {
-                const int buf = g & 1;
-                pqtc::mbar_wait_g(bar_acc_full(buf), (g >> 1) & 1u);
-                tc::tc_fence_after();
-                const int rel = t * TM + row;
+            tc::wgmma_wait<0>();
+            tc::fence_operand(acc);
+            if (pending >= 0) tc::mbar_arrive(bar_empty(pending));
+            // ---- epilogue: this thread holds rows r0, r0 + 8 and columns 8 j + 2 (lane % 4) + c of the tile
+            const int r0 = t * TM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                const int rel = r0 + 8 * i;
                 const bool row_ok = rel < len;
                 float xn = 0.f;
                 if (row_ok) xn = __ldg(p.xnorm2 + off + rel);
                 bool alive = row_ok;
                 if (alive && p.bitset) alive = !bit_is_set(p.bitset, p.rows[off + rel]);
                 const float xs = (METRIC == KB2_METRIC_L2) ? xn * (1.f - kSlack) : -kSlack * xn;   // (row part of the key) - slack * |x|^2
-                const uint32_t taddr0 = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 128);
-#pragma unroll 1
-                for (int ci = 0; ci < nch; ci++) {
-                    uint32_t v[32];
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]),
-                          "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]),
-                          "=r"(v[30]), "=r"(v[31])
-                        : "r"(taddr0 + (uint32_t)(ci * 32)));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (ci == nch - 1) {   // the accumulator is in registers: hand it back
-                        tc::tc_fence_before();
-                        tc::mbar_arrive(bar_acc_empty(buf));
-                    }
-                    uint32_t mask = 0;
-                    if (alive) {
+                uint32_t mask = 0;
+                if (alive) {
 #pragma unroll
-                        for (int u = 0; u < 32; u++) {
-                            const int col = ci * 32 + u;
-                            const float acc = __uint_as_float(v[u]);
-                            const float key = (METRIC == KB2_METRIC_L2) ? (m_base[col] + xs - 2.f * acc) : (xs - acc);
-                            mask |= (col < nqi && key <= m_thr[col]) ? (1u << u) : 0u;
+                    for (int j = 0; j < BROWS / 8; j++) {
+#pragma unroll
+                        for (int c = 0; c < 2; c++) {
+                            const int col = j * 8 + 2 * (lane & 3) + c;
+                            const float a = acc[4 * j + 2 * i + c];
+                            const float key = (METRIC == KB2_METRIC_L2) ? (m_base[col] + xs - 2.f * a) : (xs - a);
+                            mask |= (col < nqi && key <= m_thr[col]) ? (1u << (2 * j + c)) : 0u;
                         }
                     }
-                    const uint32_t cnt = __popc(mask);
-                    if (__any_sync(0xffffffffu, cnt != 0u)) {
-                        uint32_t incl = cnt;
+                }
+                const uint32_t cnt = __popc(mask);
+                if (__any_sync(0xffffffffu, cnt != 0u)) {
+                    uint32_t incl = cnt;
 #pragma unroll
-                        for (int o = 1; o < 32; o <<= 1) {
-                            const uint32_t tv = __shfl_up_sync(0xffffffffu, incl, o);
-                            if (lane >= o) incl += tv;
-                        }
-                        uint32_t wbase = 0;
-                        if (lane == 31) wbase = atomicAdd(log_cursor, incl);
-                        wbase = __shfl_sync(0xffffffffu, wbase, 31);
-                        uint32_t slot = wbase + incl - cnt;
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const uint32_t tv = __shfl_up_sync(0xffffffffu, incl, o);
+                        if (lane >= o) incl += tv;
+                    }
+                    uint32_t wbase = 0;
+                    if (lane == 31) wbase = atomicAdd(log_cursor, incl);
+                    wbase = __shfl_sync(0xffffffffu, wbase, 31);
+                    uint32_t slot = wbase + incl - cnt;
 #pragma unroll
-                        for (int u = 0; u < 32; u++) {   // static register indices (a data-dependent v[u] would spill the tile)
-                            if ((mask >> u) & 1u) {
-                                const int col = ci * 32 + u;
-                                const float acc = __uint_as_float(v[u]);
-                                const float key = (METRIC == KB2_METRIC_L2) ? (m_base[col] + xn - 2.f * acc) : -acc;
+                    for (int j = 0; j < BROWS / 8; j++) {   // static register indices (a data-dependent acc[u] would spill the tile)
+#pragma unroll
+                        for (int c = 0; c < 2; c++) {
+                            if ((mask >> (2 * j + c)) & 1u) {
+                                const int col = j * 8 + 2 * (lane & 3) + c;
+                                const float a = acc[4 * j + 2 * i + c];
+                                const float key = (METRIC == KB2_METRIC_L2) ? (m_base[col] + xn - 2.f * a) : -a;
                                 if (slot < p.log_cap) {
                                     uint4 o;
                                     o.x = (uint32_t)m_q[col];
@@ -420,18 +375,12 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                 }
             }
         }
-        if (log_over) p.log_cnt[gridDim.x] = 1u;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (e == 0) {
-            p.log_cnt[blockIdx.x] = min(*log_cursor, p.log_cap);
-            if (p.counters) atomicAdd(p.counters, n_rows);
-        }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
+    if (log_over) p.log_cnt[gridDim.x] = 1u;
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (ct == 0) {
+        p.log_cnt[blockIdx.x] = min(*log_cursor, p.log_cap);
+        if (p.counters) atomicAdd(p.counters, n_rows);
     }
 }
 

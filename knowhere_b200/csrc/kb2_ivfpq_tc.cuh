@@ -5,9 +5,9 @@
 // IndexIVF::search_preassigned (F/IndexIVF.cpp:401-768).
 //
 // Why a second engine.  The query-major LUT kernel (kb2_ivf.cuh) is bound by the shared-memory gather pipe:
-// 16 wavefronts per 32 codes *per query* (profiles/r1_final_scan_kernel.md).  But the ADC inner term is a dot
+// 16 wavefronts per 32 codes *per query*.  But the ADC inner term is a dot
 // product, <q, r^(code)>, and at batch 10^4 x nprobe 64 every list is probed by ~150 queries.  Decoding a
-// 128-code tile ONCE into bf16 and contracting it with all the queries of the list on tcgen05 replaces
+// 128-code tile ONCE into bf16 and contracting it with all the queries of the list on the tensor cores replaces
 // 16 gathers per (query, code) by 16 gathers per code + 128 x N x 128 MACs on the tensor pipe.
 //
 // Exactness.  The tensor-core value S' is only a FILTER.  With u = 2^-8 (bf16 round-to-nearest),
@@ -19,20 +19,20 @@
 // (tests/test_ivf_gpu.py::test_ivfpq_tc_engine_matches_lut_engine).  Queries whose bound is missing (fewer
 // than K codes in their nearest lists) or whose survivor buffer overflows are flagged and redone by the LUT kernel.
 //
-// sm_100a mapping (one persistent CTA per SM, 544 threads, all 512 TMEM columns, <= 219.5 KB of shared memory):
+// sm_90a mapping (one persistent CTA per SM, 512 threads, <= 219.5 KB of shared memory):
 //   warps 0-7  decoders : (two groups of 4 warps, one per A buffer, so two tiles are decoded concurrently)
-//                         code tile -> A operand [128 codes x K] bf16 in the no-swizzle K-major UMMA layout (16-byte
+//                         code tile -> A operand [128 codes x K] bf16 in the no-swizzle K-major wgmma layout (16-byte
 //                         sub-vector of sub-quantizer m = one core-matrix row), via a bf16 copy of the PQ codebooks in
 //                         shared memory, + the admission-test K-step [-r_hi, -r_mid, -r_lo, 1, 1, 1, 0, 0]; they also stage
 //                         the B operand (bf16 queries of the item, gathered by index, + [1, 1, 1, h_hi, h_mid, h_lo, 0, 0])
 //                         and the per-column meta data, one item ahead.
-//   warp  16   MMA      : K/16 + 1 x tcgen05.mma.kind::f16 (M=128, N=16..256, K=16) per tile into one of two 256-column
-//                         TMEM accumulators; tcgen05.commit releases the A buffer and publishes the accumulator.
-//   warps 8-15 epilogue : (two groups of 4 warps, one per accumulator) tcgen05.ld (32 lanes x 32 columns, double-buffered in
-//                         registers); the accumulator holds D = S' + h - r, so "survives" is a clear sign bit: an AND tree
-//                         over the 32 words decides "nothing passes" and only hits are expanded -> one shared-memory slot
-//                         reservation per warp and tile -> the group's private survivor log in global memory (plain
-//                         stores, nothing on the critical path waits for a global round trip).
+//   warps 8-15 consumers: two warpgroups, warpgroup e owns the tiles g % 2 == e (A buffer e).  A tile is contracted in
+//                         blocks of 64 codes x 64 queries (K/16 + 1 x wgmma m64n64k16 bf16 into 32 registers per thread), the
+//                         next block of the same 64-code half is issued before the current one is tested; the accumulator
+//                         holds D = S' + h - r, so "survives" is a clear sign bit, collected branch-free into per-row masks
+//                         while the next block is in flight.  Once the tile is in registers the hits are expanded -> one
+//                         shared-memory slot reservation per warp and half tile -> the group's private survivor log in global
+//                         memory (plain stores, nothing on the critical path waits for a global round trip).
 //   Items are drawn from a global ticket counter in descending-cost order (DESIGN.md 4.5).
 // Then: scatter_survivors_kernel groups the log by query, exact_eval_kernel recomputes the survivors' keys in fp32.
 // Work item = (list, chunk of <= 256 of the queries probing it); items are laid out by a single-CTA plan kernel
@@ -48,11 +48,10 @@
 namespace kb2 {
 namespace pqtc {
 
-constexpr int TM = 128;        // codes per tile (UMMA M)
-constexpr int NQT = 256;       // queries per item (UMMA N max)
-constexpr int THREADS = 544;          // warps 0-7 decoders (2 groups), 8-15 epilogue (2 groups), 16 MMA
+constexpr int TM = 128;        // codes per tile (two wgmma M=64 halves)
+constexpr int NQT = 256;       // queries per item
+constexpr int THREADS = 512;          // warps 0-7 decoders (2 groups), 8-15 consumers (2 warpgroups)
 constexpr int GROUP_THREADS = 128;
-constexpr int MMA_WARP = 16;
 constexpr int META_BYTES = 3 * NQT * 4;   // h | base | qidx
 // geometry of one engine instance: G groups of 16 sub-quantizers of DSUB dimensions (K = 16 G DSUB).
 // Instances: <1, 8> (m = 16, d = 128: BASELINE C3) and <3, 2> (m = 48, d = 96: BASELINE C5).
@@ -64,7 +63,7 @@ struct TcCfg {
     static constexpr int XCHUNK = KD / 8;             // 16-byte chunk that carries the admission test (row term / column threshold)
     static constexpr int KSTEPS = KD / 16 + 1;        // the last K-step holds the test chunk + a zero chunk
     static constexpr int CHUNKS = 2 * KSTEPS;         // 16-byte chunks per operand row
-    static constexpr int GRP_BYTES = CHUNKS * 128;    // one 8-row group of an operand: core matrices of 128 B (UMMA SBO)
+    static constexpr int GRP_BYTES = CHUNKS * 128;    // one 8-row group of an operand: core matrices of 128 B (wgmma SBO)
     static constexpr int TAB_BYTES = M * 256 * DSUB * 2;   // bf16 codebooks
     static constexpr int A_BYTES = (TM / 8) * GRP_BYTES, B_BYTES = (NQT / 8) * GRP_BYTES;
     static constexpr int OFF_TAB = 0;
@@ -148,7 +147,7 @@ __device__ __forceinline__ void
 bar_sync_epi() {
     asm volatile("bar.sync 1, 256;" ::: "memory");
 }
-// UMMA shared-memory descriptor, K-major, no swizzle: core matrix = 8 rows x 16 B (128 B contiguous);
+// wgmma shared-memory descriptor, K-major, no swizzle: core matrix = 8 rows x 16 B (128 B contiguous);
 // LBO = distance between the two core matrices of one K=16 step (128 B), SBO = distance between 8-row groups (GRP_BYTES)
 __device__ __forceinline__ uint64_t
 make_desc_ns(uint32_t smem_addr, uint32_t grp_bytes) {
@@ -156,24 +155,7 @@ make_desc_ns(uint32_t smem_addr, uint32_t grp_bytes) {
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)(128 >> 4) << 16;
     d |= (uint64_t)(grp_bytes >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-// instruction descriptor: D=f32, A=B=bf16, K-major, M=128, N=n
-__device__ __forceinline__ uint32_t
-make_idesc_bf16(int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-}
-__device__ __forceinline__ void
-mma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+    return d;   // layout type 0 (no swizzle), base offset 0
 }
 
 // x = hi + mid + lo with three bf16 terms (24 significant bits: exact for finite fp32 up to 2^-27 |x|); +-inf -> (+-inf, 0, 0)
@@ -201,19 +183,15 @@ ivfpq_tc_filter_kernel(Params p) {
     const uint32_t base = (raw + 127u) & ~127u;
     unsigned char* sm = smem_dyn + (base - raw);
     const uint32_t bars = base + OFF_BAR;
-    // barriers: a_full[2] a_empty[2] acc_full[2] acc_empty[2] b_full b_free meta_full[2] meta_free[2]
+    // barriers: a_full[2] a_empty[2] (4..7 unused) b_full b_free meta_full[2] meta_free[2]
     auto bar_a_full = [&](int i) { return bars + 8u * i; };
     auto bar_a_empty = [&](int i) { return bars + 8u * (2 + i); };
-    auto bar_acc_full = [&](int i) { return bars + 8u * (4 + i); };
-    auto bar_acc_empty = [&](int i) { return bars + 8u * (6 + i); };
     const uint32_t bar_b_full = bars + 8u * 8, bar_b_free = bars + 8u * 9;
     auto bar_meta_full = [&](int i) { return bars + 8u * (10 + i); };
     auto bar_meta_free = [&](int i) { return bars + 8u * (12 + i); };
-    const uint32_t tmem_slot = bars + 8u * 14;
-    volatile uint32_t* tmem_slot_ptr = (volatile uint32_t*)(sm + OFF_BAR + 8 * 14);
     uint32_t* qcnt = (uint32_t*)(sm + OFF_BAR + 8 * 15);   // survivor counters: [epilogue group][own tile parity]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // role index, provably warp-uniform
     const int n_items = *p.n_items;
 
     // ---- item sequence of this CTA.  The three roles walk the same sequence independently (at most ~3 items apart), so the
@@ -251,30 +229,21 @@ ivfpq_tc_filter_kernel(Params p) {
     if (threadIdx.x == 0) {
         for (int i = 0; i < 2; i++) {
             tc::mbar_init(bar_a_full(i), GROUP_THREADS);
-            tc::mbar_init(bar_a_empty(i), 1);
-            tc::mbar_init(bar_acc_full(i), 1);
-            tc::mbar_init(bar_acc_empty(i), GROUP_THREADS);
+            tc::mbar_init(bar_a_empty(i), GROUP_THREADS);
             tc::mbar_init(bar_meta_full(i), 2 * GROUP_THREADS);
             tc::mbar_init(bar_meta_free(i), 2 * GROUP_THREADS);
         }
         tc::mbar_init(bar_b_full, 2 * GROUP_THREADS);
-        tc::mbar_init(bar_b_free, 1);
+        tc::mbar_init(bar_b_free, 2 * GROUP_THREADS);
         qcnt[0] = qcnt[1] = qcnt[2] = qcnt[3] = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     // bf16 codebooks -> shared memory
     {
         uint4* tab = (uint4*)(sm + OFF_TAB);
         for (int i = threadIdx.x; i < TAB_BYTES / 16; i += THREADS) tab[i] = __ldg(p.pqc16 + i);
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
     const float inv_alpha = (METRIC == KB2_METRIC_L2) ? 0.5f : 1.f;
 
     if (warp < 8) {
@@ -456,48 +425,16 @@ ivfpq_tc_filter_kernel(Params p) {
             g0 += (uint32_t)ntiles;
             item = item_next;
         }
-    } else if (warp == MMA_WARP) {
-        // =========================== MMA issuer ===========================
-        uint32_t g = 0;
-        int it = 0;
-        for (int item = item_at(0); item < n_items; item = item_at(++it)) {
-            const int l = p.item_list[item];
-            const int nqi = p.item_nq[item];
-            const int nmma = (nqi + 15) & ~15;
-            const int ntiles = (p.list_len[l] + TM - 1) / TM;
-            const uint32_t idesc = make_idesc_bf16(nmma);
-            mbar_wait_g(bar_b_full, (uint32_t)it & 1u);
-            for (int t = 0; t < ntiles; t++, g++) {
-                const int buf = g & 1;
-                mbar_wait_g(bar_a_full(buf), (g >> 1) & 1u);
-                mbar_wait_g(bar_acc_empty(buf), ((g >> 1) & 1u) ^ 1u);
-                tc::tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t a0 = base + OFF_A + buf * A_BYTES;
-                    const uint32_t b0 = base + OFF_B;
-                    const uint32_t d = tmem_base + (uint32_t)buf * 256u;
-#pragma unroll
-                    for (int ks = 0; ks < KSTEPS; ks++)
-                        mma_bf16(d, make_desc_ns(a0 + ks * 256, GRP_BYTES), make_desc_ns(b0 + ks * 256, GRP_BYTES), idesc, ks > 0 ? 1u : 0u);
-                    tc::tc_commit(bar_a_empty(buf));
-                    tc::tc_commit(bar_acc_full(buf));
-                }
-                __syncwarp();
-            }
-            if (lane == 0) tc::tc_commit(bar_b_free);
-            __syncwarp();
-        }
     } else {
-        // =========================== epilogue: two groups of 4 warps, group e owns accumulator e (tiles g % 2 == e) ======
+        // =========================== consumers: two warpgroups, warpgroup e owns A buffer e (tiles g % 2 == e) ==========
         // The accumulator holds D = S' + h_col - r_row: a (code, query) pair survives iff D >= 0, i.e. iff its sign bit is
-        // clear.  "No survivor in these 32 columns" is an AND over the 32 words (LOP3 tree); survivors are rare (~0.1 %), so
-        // the exact mask is built only on a hit and the entries go straight to the group's survivor log in global memory
-        // (slot range reserved with one shared-memory atomic per warp and tile; plain stores, nothing waits for them).
+        // clear.  "No survivor in this 64 x 64 block" is an AND over the thread's 32 words (LOP3 tree); survivors are rare
+        // (~0.1 %), so the exact mask is built only on a hit and the entries go straight to the group's survivor log in global
+        // memory (slot range reserved with one shared-memory atomic per warp and half tile; plain stores, nothing waits for them).
         const int et = threadIdx.x - 256;        // 0..255
         const int eg = et >> 7;                  // group
         const int e = et & 127;                  // thread inside the group
-        const int we = warp & 3;                 // TMEM lane quarter (== warp % 4)
-        const int row = we * 32 + lane;          // code row inside the tile
+        const int we = warp & 3;                 // warp inside the warpgroup: rows 16 we .. 16 we + 15 of a 64-row half
         const uint32_t n_logs = 2u * gridDim.x;  // private logs (log n_logs, the former shared one, stays empty)
         uint4* my_log = p.log + (size_t)(2 * blockIdx.x + eg) * p.log_cap;
         uint32_t* my_cursor = qcnt + eg;
@@ -505,21 +442,16 @@ ivfpq_tc_filter_kernel(Params p) {
         unsigned long long n_codes = 0;
         uint32_t g0 = 0;
         int it = 0;
-#define KB2_TMEM_LD32(V, TADDR)                                                                                          \
-    asm volatile(                                                                                                        \
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                        \
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                                                        \
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"                                       \
-        : "=r"(V[0]), "=r"(V[1]), "=r"(V[2]), "=r"(V[3]), "=r"(V[4]), "=r"(V[5]), "=r"(V[6]), "=r"(V[7]), "=r"(V[8]),    \
-          "=r"(V[9]), "=r"(V[10]), "=r"(V[11]), "=r"(V[12]), "=r"(V[13]), "=r"(V[14]), "=r"(V[15]), "=r"(V[16]),         \
-          "=r"(V[17]), "=r"(V[18]), "=r"(V[19]), "=r"(V[20]), "=r"(V[21]), "=r"(V[22]), "=r"(V[23]), "=r"(V[24]),        \
-          "=r"(V[25]), "=r"(V[26]), "=r"(V[27]), "=r"(V[28]), "=r"(V[29]), "=r"(V[30]), "=r"(V[31])                      \
-        : "r"(TADDR))
+        float va[32], vb[32];
+#pragma unroll
+        for (int i = 0; i < 32; i++) va[i] = vb[i] = 0.f;
         for (int item = item_at(0); item < n_items; item = item_at(++it)) {
             const int l = p.item_list[item];
             const int nqi = p.item_nq[item];
             const int nmma = (nqi + 15) & ~15;
-            const int nch = (nmma + 31) >> 5;    // 32-column chunks; a 16-column tail reads 16 stale columns (masked below)
+            const int nblk = __shfl_sync(0xffffffffu, (nmma + 63) >> 6, 0);   // 64-query blocks; columns >= nmma of the last one are masked.
+            // The broadcast makes the block loop provably warp-uniform: with a loop bound ptxas must treat as divergent it
+            // serializes the wgmmas (C7518).
             const int len = p.list_len[l];
             const int64_t off = p.list_off[l];
             const int ntiles = (len + TM - 1) / TM;
@@ -529,95 +461,112 @@ ivfpq_tc_filter_kernel(Params p) {
             const int* m_q = (const int*)(m_base + NQT);
             if (et == 0) n_codes += (unsigned long long)len * (unsigned long long)nqi;
             const int t_first = (int)((eg - (int)(g0 & 1u)) & 1);
-            const uint32_t tail_mask = (nmma & 31) ? 0x0000ffffu : 0xffffffffu;   // valid columns of the last chunk
+            mbar_wait_g(bar_b_full, (uint32_t)it & 1u);
+            const uint32_t a0 = base + OFF_A + eg * A_BYTES;
+            const uint32_t b0 = base + OFF_B;
             for (int t = t_first; t < ntiles; t += 2) {
                 const uint32_t g = g0 + (uint32_t)t;   // g & 1 == eg
-                mbar_wait_g(bar_acc_full(eg), (g >> 1) & 1u);
-                tc::tc_fence_after();
-                const int rel = t * TM + row;
-                const uint32_t taddr0 = tmem_base + ((uint32_t)(we * 32) << 16) + (uint32_t)(eg * 256);
-                uint32_t masks[8];
-                uint32_t va[32], vb[32];
-                // D >= 0  <=>  sign bit clear.  Two-level test with short dependency chains (the serial OR-chain of a naive
-                // mask build was the epilogue's critical path): 8 independent 4-way ANDs, a 3-deep AND tree over them for the
-                // common "nothing passes" exit, and on a hit only the groups whose AND has a clear sign bit are expanded.
-                auto scan_chunk = [&](const uint32_t (&v)[32]) -> uint32_t {
-                    uint32_t g[8];
+                mbar_wait_g(bar_a_full(eg), (g >> 1) & 1u);
+                auto issue = [&](float (&acc)[32], int h, int c) {
+                    const uint32_t a = a0 + (uint32_t)(h * 8 * GRP_BYTES), b = b0 + (uint32_t)(c * 8 * GRP_BYTES);
+                    tc::fence_operand(acc);
+                    tc::wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 8; i++) g[i] = (v[4 * i] & v[4 * i + 1]) & (v[4 * i + 2] & v[4 * i + 3]);
-                    const uint32_t all = ((g[0] & g[1]) & (g[2] & g[3])) & ((g[4] & g[5]) & (g[6] & g[7]));
-                    if ((int32_t)all < 0) return 0u;   // all 32 sign bits set: nothing passes
-                    uint32_t m = 0;
-#pragma unroll
-                    for (int i = 0; i < 8; i++) {
-                        if ((int32_t)g[i] >= 0) {
-                            const uint32_t b0 = (~v[4 * i]) >> 31, b1 = (~v[4 * i + 1]) >> 31;
-                            const uint32_t b2 = (~v[4 * i + 2]) >> 31, b3 = (~v[4 * i + 3]) >> 31;
-                            m |= ((b0 | (b1 << 1)) | ((b2 << 2) | (b3 << 3))) << (4 * i);
-                        }
-                    }
-                    return m;
+                    for (int ks = 0; ks < KSTEPS; ks++)
+                        tc::wgmma_bf16_n64(acc, make_desc_ns(a + ks * 256, GRP_BYTES), make_desc_ns(b + ks * 256, GRP_BYTES), ks > 0 ? 1u : 0u);
+                    tc::wgmma_commit();
+                    tc::fence_operand(acc);
                 };
-                // software pipeline over the chunks: the TMEM load of chunk ci+1 is in flight while chunk ci is tested
-                KB2_TMEM_LD32(va, taddr0);
+                // sign test of one block -> bits (c * 16 + 2 j + cc) of the masks of the thread's two rows of half h.  Branch-free:
+                // it runs between the issue and the wait of the next block, where divergent code would make ptxas serialize
+                // the wgmmas.
+                uint64_t mh[2][2] = {{0ull, 0ull}, {0ull, 0ull}};
+                auto test = [&](const float (&v)[32], int h, int c) {
+                    const int lim = nmma - c * 64 - 2 * (lane & 3);   // column 8 j + cc of the block is valid iff 8 j + cc < lim
+                    uint32_t m0 = 0u, m1 = 0u;
 #pragma unroll
-                for (int ci = 0; ci < 8; ci++) {
-                    masks[ci] = 0;
-                    if (ci < nch) {   // (the other epilogue group works on the other accumulator meanwhile)
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                        if (ci + 1 < nch) {
-                            if (ci & 1) { KB2_TMEM_LD32(va, taddr0 + (uint32_t)((ci + 1) * 32)); }
-                            else { KB2_TMEM_LD32(vb, taddr0 + (uint32_t)((ci + 1) * 32)); }
-                        } else {
-                            // everything of this tile is in registers: hand the accumulator back before the last test
-                            tc::tc_fence_before();
-                            tc::mbar_arrive(bar_acc_empty(eg));
+                    for (int j = 0; j < 8; j++) {
+#pragma unroll
+                        for (int cc = 0; cc < 2; cc++) {
+                            const uint32_t ok = (uint32_t)(8 * j + cc < lim);
+                            m0 |= ((~__float_as_uint(v[4 * j + cc]) >> 31) & ok) << (2 * j + cc);
+                            m1 |= ((~__float_as_uint(v[4 * j + 2 + cc]) >> 31) & ok) << (2 * j + cc);
                         }
-                        masks[ci] = (ci & 1) ? scan_chunk(vb) : scan_chunk(va);
-                        if (ci == nch - 1) masks[ci] &= tail_mask;
                     }
-                }
-                // ---- survivors of this thread's row -> the group's log
-                uint32_t total = 0;
+                    mh[h][0] |= (uint64_t)m0 << (c * 16);   // h is a compile-time index (the half loop is unrolled)
+                    mh[h][1] |= (uint64_t)m1 << (c * 16);
+                };
+                // survivors of the thread's two rows of half h -> the group's log
+                auto flush = [&](int h) {
+                    const uint32_t total = (uint32_t)(__popcll(mh[h][0]) + __popcll(mh[h][1]));
+                    if (__any_sync(0xffffffffu, total != 0u)) {
+                        uint32_t incl = total;
 #pragma unroll
-                for (int ci = 0; ci < 8; ci++) total += __popc(masks[ci]);
-                if (__any_sync(0xffffffffu, total != 0u)) {
-                    uint32_t incl = total;
+                        for (int o = 1; o < 32; o <<= 1) {
+                            const uint32_t tv = __shfl_up_sync(0xffffffffu, incl, o);
+                            if (lane >= o) incl += tv;
+                        }
+                        uint32_t wbase = 0;
+                        if (lane == 31) wbase = atomicAdd(my_cursor, incl);
+                        wbase = __shfl_sync(0xffffffffu, wbase, 31);
+                        uint32_t slot = wbase + incl - total;
 #pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) {
-                        const uint32_t tv = __shfl_up_sync(0xffffffffu, incl, o);
-                        if (lane >= o) incl += tv;
-                    }
-                    uint32_t wbase = 0;
-                    if (lane == 31) wbase = atomicAdd(my_cursor, incl);
-                    wbase = __shfl_sync(0xffffffffu, wbase, 31);
-                    uint32_t slot = wbase + incl - total;
-#pragma unroll
-                    for (int ci = 0; ci < 8; ci++) {
-                        uint32_t m = masks[ci];
-                        while (m) {
-                            const int u = __ffs(m) - 1;
-                            m &= m - 1;
-                            const int col = ci * 32 + u;
-                            if (slot < p.log_cap) {
-                                uint4 o;
-                                o.x = (uint32_t)m_q[col];
-                                o.y = (uint32_t)(off + rel);
-                                o.z = __float_as_uint(m_base[col]);
-                                o.w = 0u;
-                                my_log[slot] = o;
-                            } else {
-                                log_over = true;
+                        for (int i = 0; i < 2; i++) {
+                            const int rel = t * TM + h * 64 + we * 16 + (lane >> 2) + 8 * i;
+                            uint64_t m = mh[h][i];
+                            while (m) {
+                                const int bit = __ffsll((long long)m) - 1;
+                                m &= m - 1;
+                                const int col = (bit >> 4) * 64 + 8 * ((bit & 15) >> 1) + 2 * (lane & 3) + (bit & 1);
+                                if (slot < p.log_cap) {
+                                    uint4 o;
+                                    o.x = (uint32_t)m_q[col];
+                                    o.y = (uint32_t)(off + rel);
+                                    o.z = __float_as_uint(m_base[col]);
+                                    o.w = 0u;
+                                    my_log[slot] = o;
+                                } else {
+                                    log_over = true;
+                                }
+                                slot++;
                             }
-                            slot++;
+                        }
+                    }
+                };
+                // software pipeline over the blocks of each half: the wgmmas of block c+1 run while block c is tested; the
+                // survivors are expanded once the whole tile is in registers
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    issue(va, h, 0);
+                    for (int c = 0; c < nblk; c += 2) {
+                        if (c + 1 < nblk) {
+                            issue(vb, h, c + 1);
+                            tc::wgmma_wait<1>();
+                        } else {
+                            tc::wgmma_wait<0>();
+                        }
+                        tc::fence_operand(va);
+                        test(va, h, c);
+                        if (c + 1 < nblk) {
+                            if (c + 2 < nblk) {
+                                issue(va, h, c + 2);
+                                tc::wgmma_wait<1>();
+                            } else {
+                                tc::wgmma_wait<0>();
+                            }
+                            tc::fence_operand(vb);
+                            test(vb, h, c + 1);
                         }
                     }
                 }
+                tc::mbar_arrive(bar_a_empty(eg));   // every wgmma of this tile has retired: hand the A buffer back
+                flush(0);
+                flush(1);
             }
+            tc::mbar_arrive(bar_b_free);            // this group's wgmmas of the item have all retired
             tc::mbar_arrive(bar_meta_free(par));
             g0 += (uint32_t)ntiles;
         }
-#undef KB2_TMEM_LD32
         if (log_over) p.log_cnt[n_logs + 1] = 1u;
         if (eg == 0) asm volatile("bar.sync 3, 128;" ::: "memory"); else asm volatile("bar.sync 4, 128;" ::: "memory");
         if (e == 0) {
@@ -626,12 +575,6 @@ ivfpq_tc_filter_kernel(Params p) {
             if (p.counters) atomicAdd(p.counters + 2, (unsigned long long)n);
         }
         if (et == 0 && p.counters) atomicAdd(p.counters, n_codes);
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        tc::tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
     }
 }
 

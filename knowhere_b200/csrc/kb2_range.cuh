@@ -197,7 +197,7 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
         sp.vecs = fi ? fi->base.p : hn->d_vecs.p;
         sp.rows = nullptr;
         rp.single_len = ix.count();
-        sp.nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * kNumSMs + nq - 1) / nq),
+        sp.nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nq - 1) / nq),
                                            std::max<int64_t>(1, ix.count() / 1024));
         smem += 64;
     } else if (iv) {
@@ -241,7 +241,7 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
         rp.kind = iv->is_pq ? (iv->G > 0 ? 1 : 2) : 0;
         rp.G = iv->G;
         rp.codes_b = iv->codes.p;
-        sp.nsplit = (nq < 2 * kNumSMs) ? (int)std::min<int64_t>(nprobe, (2 * kNumSMs + nq - 1) / nq) : 1;
+        sp.nsplit = (nq < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq) : 1;
         const int np_max = (nprobe + sp.nsplit - 1) / sp.nsplit;
         smem += (size_t)(np_max + 1) * 4 + (size_t)np_max * 12;
         if (iv->is_pq) smem += (size_t)iv->M * 1024;

@@ -7,7 +7,7 @@ sharded across the GPUs of one box (one process per GPU, NCCL communicator owned
 
 int8 data: the reference widens int8 to fp32 up front (src/index/index_node_data_mock_wrapper.cc:24-60); here the typed
 entry points widen each chunk on the device.  Every rank regenerates the same synthetic rows chunk by chunk (seeded), assigns
-all of them (tcgen05 contraction against the 65536 centroids) and keeps the codes of the lists it owns (l % world).
+all of them (wgmma contraction against the 65536 centroids) and keeps the codes of the lists it owns (l % world).
 Rank 0 trains (k-means on 256 x nlist sampled rows, PQ on 65536) and broadcasts the quantizers.
 Prints ONE JSON line (rank 0): queries/s (device-resident batch, collective search), e2e with host buffers, recall@10 vs
 exact brute force on a sample of the queries, roofline of the filter kernel, per-stage breakdown.

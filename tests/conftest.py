@@ -27,7 +27,7 @@ os.environ.setdefault("OMP_NUM_THREADS", str(_usable_cpus()))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -2,7 +2,7 @@
 // (include/knowhere_b200.hpp) the way the reference's Catch2 tests drive Knowhere:
 //   tests/ut/test_search.cc:57-268  (IndexFactory::Create -> Build -> Search, recall vs BruteForce)
 //   tests/ut/test_bruteforce.cc:57-77 (self-query KAT)
-// Plain asserts instead of Catch2 (not in this image).  Exit code 0 = pass.  Needs a B200.
+// Plain asserts instead of Catch2 (not in this image).  Exit code 0 = pass.  Needs an H100.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol(kb):
         assert hasattr(L, s), f"{s} declared in include/knowhere_b200.h but not exported"
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
@@ -32,7 +32,7 @@ def test_sass_is_sm100a_only():
     from knowhere_b200 import LIB
     out = subprocess.run(["cuobjdump", "-lelf", LIB], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_no_cpu_fallback_without_gpu(kb):

@@ -28,7 +28,7 @@ def test_c2_shape_ivfflat_1m(kb, ref):
     ix.build(xb)
     ix.enable_kernel_timing(True)
     ids, dist = ix.search(xq, k, {"nprobe": nprobe})
-    assert ix.last_stage_info()["engine"] == "tc"      # the list-major tcgen05 engine serves this shape
+    assert ix.last_stage_info()["engine"] == "tc"      # the list-major tensor-core engine serves this shape
     r = _export(ref, ix, "IVF_FLAT", d, nlist, 0, xb, False)
     I0, D0 = r.search(xq, k, nprobe)
     assert_topk_parity(ids, dist, I0, D0, rtol=1e-4, atol=1e-4, what="C2 IVF_FLAT 1M", max_tie_rows=nq // 100)

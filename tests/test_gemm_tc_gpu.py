@@ -1,4 +1,4 @@
-"""The tcgen05 (3xTF32, TMA-fed) contraction must reproduce the fp32 CUDA-core contraction, which in turn
+"""The wgmma (3xTF32, TMA-fed) contraction must reproduce the fp32 CUDA-core contraction, which in turn
 is what the reference computes with src/simd fvec_L2sqr_ny / fvec_inner_products_ny (distances_ref.cc:22-38)."""
 import ctypes
 

@@ -336,7 +336,7 @@ def _with_env(name, value, fn):
 @pytest.mark.parametrize("metric", [0, 1])
 @pytest.mark.parametrize("d", [128, 96])
 def test_ivfflat_tc_engine_matches_scan_and_reference(kb, ref, metric, d):
-    """IVF_FLAT list-major tcgen05 engine (kb2_ivfflat_tc.cuh: 3xTF32 filter + exact fp32 re-rank) against the query-major
+    """IVF_FLAT list-major tensor-core engine (kb2_ivfflat_tc.cuh: 3xTF32 filter + exact fp32 re-rank) against the query-major
     exact scan of the same index and against the reference's IndexIVFFlat: identical ids, distances to fp32 rounding."""
     nb, nlist, nprobe, nq, k = 60000, 64, 16, 2000, 10
     xb = datagen.clustered(nb, d, 42)
@@ -426,7 +426,7 @@ def test_ivfpq_low_precision_refine_store(kb, rtype):
 
 
 def test_coarse_stage_on_tensor_core_kernel_matches_dense_path(kb):
-    """The coarse quantizer served by the list-major tcgen05 kernel (sampled admission bound + check, kb2_index.cuh
+    """The coarse quantizer served by the list-major tensor-core kernel (sampled admission bound + check, kb2_index.cuh
     coarse_probes_tc) must give the probe lists of the dense path (key matrix + selection): same final answers."""
     nb, d, nlist, nq, k = 150000, 64, 2048, 3000, 10
     xb = datagen.clustered(nb, d, 42)
