@@ -28,7 +28,7 @@
 //                         and the per-column meta data, one item ahead.
 //   warps 8-15 consumers: two warpgroups, warpgroup e owns the tiles g % 2 == e (A buffer e).  A tile is contracted in
 //                         blocks of 64 codes x 64 queries (K/16 + 1 x wgmma m64n64k16 bf16 into 32 registers per thread), the
-//                         next block of the same 64-code half is issued before the current one is tested; the accumulator
+//                         next block of the tile (of either 64-code half) is issued before the current one is tested; the accumulator
 //                         holds D = S' + h - r, so "survives" is a clear sign bit, collected branch-free into per-row masks
 //                         while the next block is in flight.  Once the tile is in registers the hits are expanded -> one
 //                         shared-memory slot reservation per warp and half tile -> the group's private survivor log in global
@@ -41,6 +41,8 @@
 #include <cuda_bf16.h>
 
 #include <cub/block/block_scan.cuh>
+#include <type_traits>
+#include <utility>
 
 #include "kb2_gemm_tc.cuh"
 #include "kb2_ivf.cuh"
@@ -119,6 +121,26 @@ struct Params {
     uint32_t* qflag;               // [nq] 1: redo this query with the LUT kernel
     unsigned long long* counters;  // [0] codes scanned (pairs x codes), [2] survivors re-evaluated, [3] flagged
 };
+
+// f(std::integral_constant<int, I>{}) for I = 0 .. N-1, in order
+template <typename F, int... I>
+__device__ __forceinline__ void
+static_for_impl(F&& f, std::integer_sequence<int, I...>) {
+    (f(std::integral_constant<int, I>{}), ...);
+}
+template <int N, typename F>
+__device__ __forceinline__ void
+static_for(F&& f) {
+    static_for_impl(f, std::make_integer_sequence<int, N>{});
+}
+// f(std::integral_constant<int, n>{}) for the run-time block count n = 1 .. NQT / 64 (warp-uniform)
+template <typename F>
+__device__ __forceinline__ void
+for_each_block_count(int n, F&& f) {
+    static_for<NQT / 64>([&](auto i) {
+        if (n == decltype(i)::value + 1) f(std::integral_constant<int, decltype(i)::value + 1>{});
+    });
+}
 
 __device__ __forceinline__ bool
 mbar_try(uint32_t bar, uint32_t parity) {
@@ -450,7 +472,7 @@ ivfpq_tc_filter_kernel(Params p) {
             const int nqi = p.item_nq[item];
             const int nmma = (nqi + 15) & ~15;
             const int nblk = __shfl_sync(0xffffffffu, (nmma + 63) >> 6, 0);   // 64-query blocks; columns >= nmma of the last one are masked.
-            // The broadcast makes the block loop provably warp-uniform: with a loop bound ptxas must treat as divergent it
+            // The broadcast makes the block-count dispatch provably warp-uniform: with a bound ptxas must treat as divergent it
             // serializes the wgmmas (C7518).
             const int len = p.list_len[l];
             const int64_t off = p.list_off[l];
@@ -482,19 +504,20 @@ ivfpq_tc_filter_kernel(Params p) {
                 // the wgmmas.
                 uint64_t mh[2][2] = {{0ull, 0ull}, {0ull, 0ull}};
                 auto test = [&](const float (&v)[32], int h, int c) {
-                    const int lim = nmma - c * 64 - 2 * (lane & 3);   // column 8 j + cc of the block is valid iff 8 j + cc < lim
+                    // column 8 j + cc of the block is valid iff 8 j + cc < lim; lim is even, so iff j < ceil(lim / 8)
+                    const int lim = nmma - c * 64 - 2 * (lane & 3);
+                    const uint32_t valid = (1u << (2 * min(8, max(0, (lim + 7) >> 3)))) - 1u;
                     uint32_t m0 = 0u, m1 = 0u;
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
 #pragma unroll
                         for (int cc = 0; cc < 2; cc++) {
-                            const uint32_t ok = (uint32_t)(8 * j + cc < lim);
-                            m0 |= ((~__float_as_uint(v[4 * j + cc]) >> 31) & ok) << (2 * j + cc);
-                            m1 |= ((~__float_as_uint(v[4 * j + 2 + cc]) >> 31) & ok) << (2 * j + cc);
+                            m0 |= (~__float_as_uint(v[4 * j + cc]) >> 31) << (2 * j + cc);
+                            m1 |= (~__float_as_uint(v[4 * j + 2 + cc]) >> 31) << (2 * j + cc);
                         }
                     }
-                    mh[h][0] |= (uint64_t)m0 << (c * 16);   // h is a compile-time index (the half loop is unrolled)
-                    mh[h][1] |= (uint64_t)m1 << (c * 16);
+                    mh[h][0] |= (uint64_t)(m0 & valid) << (c * 16);   // h and c are compile-time indices (unrolled pipeline)
+                    mh[h][1] |= (uint64_t)(m1 & valid) << (c * 16);
                 };
                 // survivors of the thread's two rows of half h -> the group's log
                 auto flush = [&](int h) {
@@ -533,32 +556,32 @@ ivfpq_tc_filter_kernel(Params p) {
                         }
                     }
                 };
-                // software pipeline over the blocks of each half: the wgmmas of block c+1 run while block c is tested; the
-                // survivors are expanded once the whole tile is in registers
-#pragma unroll
-                for (int h = 0; h < 2; h++) {
-                    issue(va, h, 0);
-                    for (int c = 0; c < nblk; c += 2) {
-                        if (c + 1 < nblk) {
-                            issue(vb, h, c + 1);
+                // software pipeline over the 2 nblk blocks of the tile (half-major, va / vb alternating): the wgmmas of block
+                // b+1 run while block b is tested, across the boundary between the halves too; the survivors are expanded
+                // once the whole tile is in registers.  The sequence is unrolled for each block count, so every issue, wait
+                // and test sits in straight-line code: with the wait inside a run-time loop ptxas cannot prove that the
+                // tested buffer has retired, and serializes every wgmma of the kernel (C7514).
+                for_each_block_count(nblk, [&](auto nb) {
+                    constexpr int NB = decltype(nb)::value, NBT = 2 * NB;
+                    issue(va, 0, 0);
+                    static_for<NBT>([&](auto bc) {
+                        constexpr int b = decltype(bc)::value;
+                        if constexpr (b + 1 < NBT) {
+                            if constexpr ((b + 1) & 1) issue(vb, (b + 1) / NB, (b + 1) % NB);
+                            else issue(va, (b + 1) / NB, (b + 1) % NB);
                             tc::wgmma_wait<1>();
                         } else {
                             tc::wgmma_wait<0>();
                         }
-                        tc::fence_operand(va);
-                        test(va, h, c);
-                        if (c + 1 < nblk) {
-                            if (c + 2 < nblk) {
-                                issue(va, h, c + 2);
-                                tc::wgmma_wait<1>();
-                            } else {
-                                tc::wgmma_wait<0>();
-                            }
+                        if constexpr (b & 1) {
                             tc::fence_operand(vb);
-                            test(vb, h, c + 1);
+                            test(vb, b / NB, b % NB);
+                        } else {
+                            tc::fence_operand(va);
+                            test(va, b / NB, b % NB);
                         }
-                    }
-                }
+                    });
+                });
                 tc::mbar_arrive(bar_a_empty(eg));   // every wgmma of this tile has retired: hand the A buffer back
                 flush(0);
                 flush(1);

@@ -1,0 +1,45 @@
+"""Block counts of the IVF_PQ filter kernel (kb2_ivfpq_tc.cuh) against the query-major LUT engine.
+
+The consumer warpgroups run one unrolled wgmma pipeline per number of 64-query blocks of an item (1 to 4).  With
+nprobe == nlist every list is probed by every query of the batch, so the batch size sets the width of every item:
+5 queries -> 1 block, 70 -> 2, 140 -> 3, 250 -> 4, 600 -> chunks of 208 + 184 queries (4 and 3 blocks).  Each width
+must return the LUT engine's rows bit for bit, for both metrics and both geometries of the engine."""
+import os
+
+import numpy as np
+import pytest
+
+from knowhere_b200 import datagen
+
+pytestmark = pytest.mark.gpu
+
+
+def _search(ix, xq, k, cfg, engine):
+    old = os.environ.get("KB2_PQ_ENGINE")
+    os.environ["KB2_PQ_ENGINE"] = engine
+    try:
+        return ix.search(xq, k, cfg)
+    finally:
+        if old is None:
+            os.environ.pop("KB2_PQ_ENGINE", None)
+        else:
+            os.environ["KB2_PQ_ENGINE"] = old
+
+
+@pytest.mark.parametrize("metric", ["L2", "IP"])
+@pytest.mark.parametrize("d,m", [(128, 16), (96, 48)])
+def test_ivfpq_tc_engine_every_block_count(kb, metric, d, m):
+    nb, nlist, k = 20000, 16, 10
+    xb = datagen.clustered(nb, d, 11)
+    ix = kb.Index("IVF_PQ", metric, d, {"nlist": nlist, "m": m, "nbits": 8})
+    ix.train(xb)
+    ix.add(xb)
+    cfg = {"nprobe": nlist}
+    for nq in (5, 70, 140, 250, 600):
+        xq = datagen.clustered(nq, d, 12)
+        i0, d0 = _search(ix, xq, k, cfg, "lut")
+        i1, d1 = _search(ix, xq, k, cfg, "tc")
+        assert ix.last_stage_info()["engine"] == "tc", f"nq={nq}: tensor-core engine was not selected"
+        assert ix.last_counters()["codes"] >= nq * nb, f"nq={nq}: the filter pass did not scan every (query, code) pair"
+        assert np.array_equal(d0.view(np.uint32), d1.view(np.uint32)), f"nq={nq}: distances differ in {(d0 != d1).any(axis=1).sum()} rows"
+        assert np.array_equal(i0, i1), f"nq={nq}: ids differ in {(i0 != i1).any(axis=1).sum()} rows"
