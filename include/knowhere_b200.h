@@ -83,7 +83,7 @@ int kb2_index_set_stream(kb2_index_t h, void* cuda_stream);
 
 /* Multi-GPU list/row sharding (SURVEY §8e).  Must be called before train/add/import.
  * IVF_*: every inverted list lives on exactly one rank (greedy size-balanced packing over the global list sizes,
- * identical on all ranks; KB2_SHARD_POLICY=mod selects l % world).  FLAT: row i is kept by rank
+ * identical on all ranks).  FLAT: row i is kept by rank
  * floor(i * world / n) at add time.  HNSW: graph partitions — every rank builds an independent sub-graph over its
  * contiguous row slice of the (single) add() call and all of them are searched with the same ef (SURVEY §8e option 2;
  * recall >= the single graph's in practice, at world x the distance evaluations).

@@ -20,22 +20,8 @@
 
 namespace kb2 {
 
-#ifndef KB2_DEFAULT_GEMM_MODE
-#define KB2_DEFAULT_GEMM_MODE 1
-#endif
-// 0 = fp32 CUDA-core contraction, 1 = wgmma (3xTF32) contraction.  KB2_GEMM=fp32|tc overrides.
-inline int
-gemm_mode() {
-    static int mode = [] {
-        const char* e = getenv("KB2_GEMM");
-        if (e && strcmp(e, "fp32") == 0) return 0;
-        if (e && strcmp(e, "tc") == 0) return 1;
-        return KB2_DEFAULT_GEMM_MODE;
-    }();
-    return mode;
-}
-
-// keys[nq][ldk] <- contraction of Q[nq][d] with X[cols][d]; returns true if the tensor-core path ran
+// keys[nq][ldk] <- contraction of Q[nq][d] with X[cols][d]; returns true if the tensor-core path ran.
+// mode: 0 = fp32 CUDA-core contraction, 1 = wgmma (3xTF32) contraction where the shapes allow it.
 inline bool
 launch_gemm_keys(cudaStream_t st, int mode, int metric, const float* Q, const float* X, const float* qn,
                  const float* xn, int nq, int cols, int d, float* keys, int64_t ldk, const uint8_t* bitset,
@@ -55,11 +41,10 @@ launch_gemm_keys(cudaStream_t st, int mode, int metric, const float* Q, const fl
                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::smem_bytes(1));
             });
             dim3 g((unsigned)((cols + tc::BN - 1) / tc::BN), (unsigned)((nq + tc::BM - 1) / tc::BM));
-            static const int short_k = [] { const char* e = getenv("KB2_GEMM_SHORTK"); return e ? atoi(e) : 192; }();
 #define KB2_GEMM_LAUNCH(MM, NST)                                                                                                  \
     tc::gemm_keys_tc_kernel<MM, NST><<<g, tc::THREADS, tc::smem_bytes(NST), st>>>(tq, tx, qn, xn, nq, cols, d, keys, ldk, bitset, \
                                                                                   rows, row_base)
-            if (d <= short_k) {
+            if (d <= tc::SHORT_K) {
                 if (metric == KB2_METRIC_L2) KB2_GEMM_LAUNCH(KB2_METRIC_L2, 1); else KB2_GEMM_LAUNCH(KB2_METRIC_IP, 1);
             } else {
                 if (metric == KB2_METRIC_L2) KB2_GEMM_LAUNCH(KB2_METRIC_L2, 3); else KB2_GEMM_LAUNCH(KB2_METRIC_IP, 3);
@@ -369,7 +354,7 @@ assign_nearest(const float* x, int64_t n, int d, const float* cent, int k, int m
     // wide codebooks (IVF coarse quantizers): the wgmma 3xTF32 contraction (keys to ~5e-6 relative; the reference's own
     // add()/k-means assignment goes through BLAS sgemm, F/utils/distances.cpp:400-520).  Narrow ones (PQ sub-quantizers,
     // k = 256, d = 2..8) stay on the fp32 CUDA-core kernel.
-    const int mode = (k >= 512 && (d & 3) == 0 && n >= 1024) ? gemm_mode() : 0;
+    const int mode = (k >= 512 && (d & 3) == 0 && n >= 1024) ? 1 : 0;
     const int64_t ldk = (k + 3) & ~3;
     sc.keys.ensure((size_t)chunk * ldk);
     sc.xn.ensure((size_t)chunk);

@@ -182,8 +182,7 @@ select_keys_kernel(const float* __restrict__ keys, int64_t ldk, int ncols, int K
 // grid (nq, nsplit), block 256, dynamic smem: slice*4 + 4160 bytes.
 __global__ void __launch_bounds__(256)
 select_keys_hist_kernel(const float* __restrict__ keys, int64_t ldk, int ncols, int K_need, int K_cap,
-                        uint64_t* __restrict__ partial, int slots_per_query, int slot_base, uint32_t pos_base,
-                        int allow_fast = 1) {
+                        uint64_t* __restrict__ partial, int slots_per_query, int slot_base, uint32_t pos_base) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     uint32_t* hist = (uint32_t*)smem_raw;          // 1024 bins (+1)
     uint32_t* ctl = hist + 1032;                   // [0] min [1] max [2] out cursor [3] bstar+1 [4] cum(bstar) [5] shift
@@ -226,7 +225,7 @@ select_keys_hist_kernel(const float* __restrict__ keys, int64_t ldk, int ncols, 
     // histogram of the chunk minima (256 shared-memory atomics instead of one per key, 8 bins per lane to scan), then every
     // thread emits its keys <= T: about K_need * (1 + K_need / 256) entries.  If more than K_cap qualify (rare: K_cap is the
     // next power of two) the level-wise histogram below redoes the row, so the result is always a superset of the K_need best.
-    const bool fast = allow_fast && blockDim.x == 256 && n >= 512 && 2 * K_need <= 256 && K_need <= K_cap;
+    const bool fast = blockDim.x == 256 && n >= 512 && 2 * K_need <= 256 && K_need <= K_cap;
     const uint32_t cmin = lmin;   // this thread's chunk minimum (0xffffffff: no finite key)
     uint32_t cmax = (cmin != 0xffffffffu) ? cmin : 0u;
     for (int i = threadIdx.x; i < 1032; i += blockDim.x) hist[i] = 0;

@@ -37,6 +37,7 @@ constexpr size_t SMEM_BYTES = smem_bytes(STAGES);
 // Short contractions (d <= 192: the IVF coarse quantizer, k-means assignment) run a single-stage instantiation with two
 // CTAs per SM instead: a 128x128 tile is then a strictly serial TMA -> split -> MMA -> store chain, and a second resident
 // CTA overlaps its epilogue store with the other's loads.
+constexpr int SHORT_K = 192;                   // largest d served by the single-stage instantiation
 
 __device__ __forceinline__ uint32_t
 smem_u32(const void* p) {

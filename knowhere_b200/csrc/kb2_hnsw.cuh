@@ -1304,6 +1304,7 @@ struct HnswIndex : IndexBase {
     }
 
     // ------------------------------------------------------------ device-side construction (see hnsw_select_kernel)
+    static constexpr int64_t kBuildBatch = 16384;   // most nodes inserted per batch (also at most a quarter of those linked)
     static bool
     gpu_build_wanted(int64_t n_rows, int M_) {
         if (2 * M_ > 64) return false;   // the link kernel keeps a row in 64 slots
@@ -1336,9 +1337,7 @@ struct HnswIndex : IndexBase {
         KB2_CUDA_CHECK(cudaMemcpyAsync(d_order.p, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
         KB2_CUDA_CHECK(cudaMemcpyAsync(d_rank.p, rank.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
         KB2_CUDA_CHECK(cudaMemsetAsync(d_locks.p, 0, (size_t)n * 4, st));
-        int64_t maxb = 16384;
-        if (const char* e = getenv("KB2_HNSW_BUILD_BATCH")) maxb = std::max<int64_t>(1, atoll(e));
-        maxb = std::min<int64_t>(maxb, n);
+        const int64_t maxb = std::min<int64_t>(kBuildBatch, n);
         d_cand_ids.alloc_exact((size_t)maxb * ef);
         d_cand_dist.alloc_exact((size_t)maxb * ef);
         d_sel.alloc_exact((size_t)maxb * 64);

@@ -21,12 +21,6 @@ namespace kb2 {
 constexpr int kMaxK = 1024;            // largest k' any selection kernel keeps
 constexpr int kMaxSortEntries = 8192;  // finalize sorts at most this many candidates per query
 constexpr int kMaxDynSmem = 227 * 1024;
-#ifndef KB2_DEFAULT_SCAN_PREFETCH
-#define KB2_DEFAULT_SCAN_PREFETCH 1
-#endif
-#ifndef KB2_DEFAULT_SCAN_NT
-#define KB2_DEFAULT_SCAN_NT 256
-#endif
 
 inline void
 init_kernel_attributes() {
@@ -39,30 +33,18 @@ init_kernel_attributes() {
         set((const void*)reduce_partials_kernel);
         set((const void*)select_keys_kernel);
         set((const void*)select_keys_hist_kernel);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, false, 256>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, true, 256>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, false, 256>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, true, 256>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, false, 256>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, true, 256>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, false, 256>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, true, 256>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, false, 256>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, true, 256>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, false, 256>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, true, 256>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, false, 512>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, true, 512>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, false, 512>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, true, 512>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, false, 512>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, true, 512>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, false, 512>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, true, 512>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, false, 512>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, true, 512>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, false, 512>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, true, 512>);
+        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, false>);
+        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, true>);
+        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, false>);
+        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, true>);
+        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, false>);
+        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, true>);
+        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, false>);
+        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, true>);
+        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, false>);
+        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, true>);
+        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, false>);
+        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, true>);
         set((const void*)ivfpq_scan_generic_kernel<KB2_METRIC_L2>);
         set((const void*)ivfpq_scan_generic_kernel<KB2_METRIC_IP>);
         set((const void*)ivfflat_scan_kernel<KB2_METRIC_L2>);
@@ -71,14 +53,10 @@ init_kernel_attributes() {
         set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, 1, 8>);
         set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_L2, 3, 2>);
         set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, 3, 2>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 32>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 32>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 64>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 64>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 32, 1, 8, 256>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 32, 1, 8, 256>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 32, 3, 2>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 32, 3, 2>);
+        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 1, 8, 256>);
+        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 1, 8, 256>);
+        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 3, 2, 128>);
+        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 3, 2, 128>);
         set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_L2, 32>);
         set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_IP, 32>);
         set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_L2, 128>);
@@ -290,8 +268,6 @@ dense_candidates(IndexBase& ix, const float* Q, int64_t nq, const float* X, cons
         KB2_CUDA_CHECK(cudaMemset2DAsync(ix.s_partial.p, (size_t)pl.stride() * 8, 0xFF, (size_t)slots * pl.Ksel * 8, (size_t)nq, st));
     }
     const size_t sel_smem = (size_t)kScanWarps * 2 * pl.Ksel * 8;
-    // chunk-minimum fast path of the wide select (KB2_SELECT_FAST=0: level-wise histogram only)
-    static const bool select_fast = [] { const char* e = getenv("KB2_SELECT_FAST"); return !(e && atoi(e) == 0); }();
     for (int64_t c0 = 0; c0 < n; c0 += chunk) {
         const int64_t cols = std::min(chunk, n - c0);
         if (pl.used + nsplit > pl.S) {
@@ -302,14 +278,13 @@ dense_candidates(IndexBase& ix, const float* Q, int64_t nq, const float* X, cons
             ix.last.launches++;
             pl.used = 1;
         }
-        launch_gemm_keys(st, gemm_mode(), metric, Q, X + c0 * d, ix.s_qn.p, xn + c0, (int)nq, (int)cols, d, ix.s_keys.p, ldk,
+        launch_gemm_keys(st, 1, metric, Q, X + c0 * d, ix.s_qn.p, xn + c0, (int)nq, (int)cols, d, ix.s_keys.p, ldk,
                          bitset, rows, c0 + bit_offset);
         const int per_slice = (int)(((cols + nsplit - 1) / nsplit + 31) / 32 * 32);
         const size_t hist_smem = (size_t)per_slice * 4 + 4160;
         if (pl.Ksel >= 64 && hist_smem <= (size_t)kMaxDynSmem) {
             select_keys_hist_kernel<<<dim3((unsigned)nq, nsplit), 256, hist_smem, st>>>(
-                ix.s_keys.p, ldk, (int)cols, std::min(k_need, pl.Ksel), pl.Ksel, ix.s_partial.p, pl.S, pl.used, (uint32_t)c0,
-                select_fast ? 1 : 0);
+                ix.s_keys.p, ldk, (int)cols, std::min(k_need, pl.Ksel), pl.Ksel, ix.s_partial.p, pl.S, pl.used, (uint32_t)c0);
         } else {
             select_keys_kernel<<<dim3((unsigned)nq, nsplit), kScanThreads, sel_smem, st>>>(
                 ix.s_keys.p, ldk, (int)cols, pl.Ksel, pl.Ksel, ix.s_partial.p, pl.S, pl.used, (uint32_t)c0);
@@ -326,8 +301,7 @@ launch_finalize(IndexBase& ix, FinalizeParams fp, int64_t nq) {
     fp.n_sort = next_pow2(std::max(fp.n_partial, 2));
     KB2_REQUIRE(fp.n_sort <= kMaxSortEntries, KB2_INTERNAL_ERROR, "finalize: too many partial candidates");
     KB2_REQUIRE(fp.k_sel <= kMaxK && fp.k_out <= fp.k_sel, KB2_INVALID_ARGS, "k too large");
-    static const bool warp_path = [] { const char* e = getenv("KB2_FINALIZE"); return !(e && !strcmp(e, "cta")); }();
-    if (warp_path && fp.k_sel <= 128 && fp.d <= 1024 && (fp.n_partial <= 256 || fp.counts)) {
+    if (fp.k_sel <= 128 && fp.d <= 1024 && (fp.n_partial <= 256 || fp.counts)) {
         // one warp per query (see finalize_warp_kernel); variable-length rows longer than 256 entries fall through to the
         // CTA kernel below, which then skips the short ones (measured at C3: a 512-entry register sort for the tail costs
         // more than that second launch)
@@ -673,23 +647,18 @@ struct IvfIndex : IndexBase {
         std::vector<int64_t> first_rank(nlist, 0);
         int64_t cur = 0, rank = 0;
         // list -> shard: greedy size-balanced packing (longest list first onto the lightest shard; SURVEY 8e), computed from
-        // the global list sizes, which every rank holds, so all ranks derive the same table.  KB2_SHARD_POLICY=mod: l % world.
+        // the global list sizes, which every rank holds, so all ranks derive the same table.
         h_list_owner.assign(nlist, 0);
         if (shard_world > 1) {
-            const char* pol = getenv("KB2_SHARD_POLICY");
-            if (pol && !strcmp(pol, "mod")) {
-                for (int64_t l = 0; l < nlist; l++) h_list_owner[l] = (int32_t)(l % shard_world);
-            } else {
-                std::vector<int64_t> order(nlist), load(shard_world, 0);
-                for (int64_t l = 0; l < nlist; l++) order[l] = l;
-                std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return h_list_cnt_all[a] > h_list_cnt_all[b]; });
-                for (int64_t l : order) {
-                    int best = 0;
-                    for (int r = 1; r < shard_world; r++)
-                        if (load[r] < load[best]) best = r;
-                    h_list_owner[l] = best;
-                    load[best] += h_list_cnt_all[l];
-                }
+            std::vector<int64_t> order(nlist), load(shard_world, 0);
+            for (int64_t l = 0; l < nlist; l++) order[l] = l;
+            std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return h_list_cnt_all[a] > h_list_cnt_all[b]; });
+            for (int64_t l : order) {
+                int best = 0;
+                for (int r = 1; r < shard_world; r++)
+                    if (load[r] < load[best]) best = r;
+                h_list_owner[l] = best;
+                load[best] += h_list_cnt_all[l];
             }
         }
         list_owner.alloc_exact(nlist);
@@ -811,30 +780,18 @@ struct IvfIndex : IndexBase {
                                    (size_t)dim * 4 + 64 + 8 * (2 * kScanWarps + 4) + (size_t)4 * Ksel * 8;   // + CTA bound block + merge buffer
         if (is_pq) {
             if (G > 0) {
-                const int scan_nt_env = [] { const char* e = getenv("KB2_SCAN_NT"); return e ? atoi(e) : 0; }();
-                int scan_nt = (scan_nt_env == 256 || scan_nt_env == 512) ? scan_nt_env : KB2_DEFAULT_SCAN_NT;
-                size_t smem = (size_t)G * 65536 + common_smem;
-                if (scan_nt == 512) {
-                    const size_t smem512 = smem + (size_t)kScanWarps * 2 * Ksel * 8 + 8 * kScanWarps;  // 16 warp buffers
-                    if (smem512 <= (size_t)kMaxDynSmem) smem = smem512; else scan_nt = 256;
-                }
+                const size_t smem = (size_t)G * 65536 + common_smem;
                 KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "IVF_PQ: k too large for shared memory");
-#define KB2_LAUNCH_PQ_NT(GG, NTT)                                                                              \
+#define KB2_LAUNCH_PQ(GG)                                                                                      \
     if (metric == KB2_METRIC_L2) {                                                                             \
-        if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_L2, true, NTT><<<grid, NTT, smem, st>>>(sp);               \
-        else ivfpq_scan_kernel<GG, KB2_METRIC_L2, false, NTT><<<grid, NTT, smem, st>>>(sp);                    \
+        if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_L2, true><<<grid, kScanThreads, smem, st>>>(sp);           \
+        else ivfpq_scan_kernel<GG, KB2_METRIC_L2, false><<<grid, kScanThreads, smem, st>>>(sp);                \
     } else {                                                                                                   \
-        if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_IP, true, NTT><<<grid, NTT, smem, st>>>(sp);               \
-        else ivfpq_scan_kernel<GG, KB2_METRIC_IP, false, NTT><<<grid, NTT, smem, st>>>(sp);                    \
+        if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_IP, true><<<grid, kScanThreads, smem, st>>>(sp);           \
+        else ivfpq_scan_kernel<GG, KB2_METRIC_IP, false><<<grid, kScanThreads, smem, st>>>(sp);                \
     }
-#define KB2_LAUNCH_PQ(GG)                                     \
-    if (scan_nt == 512) { KB2_LAUNCH_PQ_NT(GG, 512) } else { KB2_LAUNCH_PQ_NT(GG, 256) }
-                const char* e_pf = getenv("KB2_SCAN_PREFETCH");
-                sp.flags = (e_pf ? atoi(e_pf) : KB2_DEFAULT_SCAN_PREFETCH) ? 2 : 0;
-                if (const char* e_fm = getenv("KB2_SCAN_FULLMERGE")) sp.flags |= atoi(e_fm) ? 4 : 0;
                 if (G == 1) { KB2_LAUNCH_PQ(1) } else if (G == 2) { KB2_LAUNCH_PQ(2) } else { KB2_LAUNCH_PQ(3) }
 #undef KB2_LAUNCH_PQ
-#undef KB2_LAUNCH_PQ_NT
             } else {
                 const size_t smem = (size_t)M * 1024 + common_smem;
                 KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "IVF_PQ: m too large for the generic kernel");
@@ -856,6 +813,8 @@ struct IvfIndex : IndexBase {
 
     // ---------------------------------------------------------------- list-major tensor-core engine (kb2_ivfpq_tc.cuh)
     static constexpr int kTcCandCap = 2048;     // survivor slots per query (overflow -> LUT kernel redoes the query)
+    static constexpr double kTcMinQpl = 8.0;    // queries per list from which the list-major engine is taken (use_tc_engine)
+    static constexpr int kTcACodes = 3000;      // phase A: codes per query its bound is taken from
     DevBuf<uint16_t> tc_pqc16, s_qb16;
     DevBuf<float> tc_pqc_t;   // codebook transposed for the in-kernel tables of bound_kernel<..., 3, 2>
     DevBuf<float> tc_maxn2, s_qnorm, s_pair_base, s_lut, s_bound;
@@ -874,14 +833,14 @@ struct IvfIndex : IndexBase {
     DevBuf<uint32_t> s_bal_key, s_bal_key2;
     // Side stream of the list-major engine: the plan (pairs grouped by list, item table, cost sort: seven small, latency-bound
     // launches that depend on the coarse result only) runs beside phase A (which fills the SMs with 3 x 128 threads each) and
-    // joins before the filter kernel.  KB2_TC_OVERLAP=0 keeps everything on the handle's stream.
+    // joins before the filter kernel.  With KB2_TC_VERBOSE set everything stays on the handle's stream, so that the stage
+    // timings do not overlap.
     cudaStream_t side_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     bool side_pending = false;   // forked, not yet joined (only ever observed true after an exception)
     bool
     plan_overlap() {
-        static const bool on = [] { const char* e = getenv("KB2_TC_OVERLAP"); return !(e && atoi(e) == 0); }();
-        if (!on || getenv("KB2_TC_VERBOSE")) return false;
+        if (getenv("KB2_TC_VERBOSE")) return false;
         if (!side_stream) {
             KB2_CUDA_CHECK(cudaStreamCreateWithFlags(&side_stream, cudaStreamNonBlocking));
             KB2_CUDA_CHECK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
@@ -894,12 +853,10 @@ struct IvfIndex : IndexBase {
         if (ev_join) cudaEventDestroy(ev_join);
         if (side_stream) cudaStreamDestroy(side_stream);
     }
-    // sort the items by descending cost and deal them to the G persistent CTAs in snake order; returns the new item arrays
+    // sort the items by descending cost (the persistent kernels draw them in this order); returns the new item arrays
     int32_t*
-    balance_items(int32_t* items, int64_t max_items, int G_ctas, int tile_cost, int col_cost, cudaStream_t st = nullptr) {
+    balance_items(int32_t* items, int64_t max_items, int tile_cost, int col_cost, cudaStream_t st = nullptr) {
         if (!st) st = stream;
-        const char* e = getenv("KB2_TC_BALANCE");
-        if (e && atoi(e) == 0) return items;
         s_items2.ensure((size_t)3 * max_items);
         s_bal_key.ensure((size_t)max_items); s_bal_key2.ensure((size_t)max_items);
         s_bal_idx.ensure((size_t)max_items); s_bal_idx2.ensure((size_t)max_items);
@@ -909,18 +866,13 @@ struct IvfIndex : IndexBase {
         cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, s_bal_key.p, s_bal_key2.p, s_bal_idx.p, s_bal_idx2.p, (int)max_items, 0, 16, st);
         s_sort_tmp.ensure(tmp_bytes);
         cub::DeviceRadixSort::SortPairs(s_sort_tmp.p, tmp_bytes, s_bal_key.p, s_bal_key2.p, s_bal_idx.p, s_bal_idx2.p, (int)max_items, 0, 16, st);
-        pqtc::deal_items_kernel<<<grid1d(max_items, 256), 256, 0, st>>>(s_plan_out.p, s_bal_idx2.p, G_ctas, items, items + max_items,
+        pqtc::deal_items_kernel<<<grid1d(max_items, 256), 256, 0, st>>>(s_plan_out.p, s_bal_idx2.p, items, items + max_items,
                                                                       items + 2 * max_items, s_items2.p, s_items2.p + max_items,
                                                                       s_items2.p + 2 * max_items);
         last.launches += 4;
         return s_items2.p;
     }
 
-    static bool
-    tc_dynamic_sched() {
-        static const bool dyn = [] { const char* e = getenv("KB2_TC_SCHED"); return !(e && !strcmp(e, "static")); }();
-        return dyn;
-    }
     bool
     use_tc_engine(int64_t nq, int nprobe, int Ksel) const {
         if (!is_pq || !(tc_geom_18() || tc_geom_32())) return false;
@@ -930,9 +882,8 @@ struct IvfIndex : IndexBase {
         if (e && !strcmp(e, "tc")) return true;
         // the decode of a list is amortised over the queries that probe it.  Measured at C5 (100M x 96, nlist 65536, 19.5
         // queries per list on average): the query-major LUT engine needs 34.5 ms per 10000-query batch on two GPUs, so the
-        // list-major engine is taken from 8 queries per list on (KB2_TC_MIN_QPL overrides)
-        static const double min_qpl = [] { const char* t = getenv("KB2_TC_MIN_QPL"); return t ? atof(t) : 8.0; }();
-        return (double)nq * nprobe >= min_qpl * (double)nlist;
+        // list-major engine is taken from kTcMinQpl queries per list on
+        return (double)nq * nprobe >= kTcMinQpl * (double)nlist;
     }
 
     void
@@ -994,12 +945,8 @@ struct IvfIndex : IndexBase {
         //      subset of the codes is valid on every rank, so with a communicator the query is handled by the rank that owns
         //      its nearest list (1/world of the batch each; tables only for those) and the bounds are min-reduced.
         const char* e_p0 = getenv("KB2_TC_P0");
-        const char* e_ac = getenv("KB2_TC_A_CODES");
         const int p0 = std::max(1, std::min((e_p0 ? atoi(e_p0) : 8) * std::max(1, shard_world), nprobe));   // at most this many lists
-        const int a_codes = e_ac ? atoi(e_ac) : 3000;                                                        // ... until this many codes
         s_bound.ensure((size_t)nq);
-        static const bool generic_a = [] { const char* e = getenv("KB2_TC_PHASE_A"); return e && !strcmp(e, "scan"); }();
-        if (tc_geom_18() || (tc_geom_32() && !generic_a)) {
         if (tc_geom_18()) s_lut.ensure((size_t)nq * 4096);
         const int32_t* qlist = nullptr;
         const uint32_t* qcount = nullptr;
@@ -1015,60 +962,29 @@ struct IvfIndex : IndexBase {
             last.launches += 2;
         }
         {
-            const char* e_rw = getenv("KB2_BOUND_ROWW");
-            const int roww = (e_rw && atoi(e_rw) == 64) ? 64 : 32;   // 32 rows: 3 CTAs/SM, 64 rows: 2 CTAs/SM
-            const size_t smem = pqtc::bound_smem(roww, pqtc::bound_kmax(a_codes, k_base));
-            static const int bound_nt = [] { const char* e = getenv("KB2_BOUND_NT"); return e ? atoi(e) : 256; }();
-#define KB2_BOUND_LAUNCH(MM, RW)                                                                                                    \
-    pqtc::lut_build_kernel<MM><<<num_sms(), 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
-    mark("lut");                                                                                                                    \
-    pqtc::bound_kernel<MM, RW><<<bound_grid, 128, smem, st>>>(s_lut.p, qlist, qcount, nq, sp.probe_ids, sp.probe_dis, nprobe, p0,   \
-                                                             a_codes, k_base, list_off.p, list_len.p, (const uint4*)codes.p, t1.p, \
-                                                             sp.bitset, rows.p, s_bound.p, d_counter.p + 4);
+            const size_t smem = pqtc::bound_smem(pqtc::bound_kmax(kTcACodes, k_base));
             if (tc_geom_32()) {
                 // m48 x dsub2: three groups through one in-kernel table each (no [nq][m][256] table in global memory)
 #define KB2_BOUND_LAUNCH3(MM)                                                                                                       \
-    pqtc::bound_kernel<MM, 32, 3, 2><<<bound_grid, 128, pqtc::bound_smem(32, pqtc::bound_kmax(a_codes, k_base)), st>>>(             \
-        nullptr, qlist, qcount, nq, sp.probe_ids, sp.probe_dis, nprobe, p0, a_codes, k_base, list_off.p, list_len.p,                \
+    pqtc::bound_kernel<MM, 3, 2, 128><<<bound_grid, 128, smem, st>>>(                                                               \
+        nullptr, qlist, qcount, nq, sp.probe_ids, sp.probe_dis, nprobe, p0, kTcACodes, k_base, list_off.p, list_len.p,              \
         (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p, d_counter.p + 4, npad, sp.queries, tc_pqc_t.p);
                 if (metric == KB2_METRIC_L2) { KB2_BOUND_LAUNCH3(KB2_METRIC_L2) } else { KB2_BOUND_LAUNCH3(KB2_METRIC_IP) }
 #undef KB2_BOUND_LAUNCH3
-            } else if (bound_nt == 256 && roww == 32) {
-                // 8 warps per CTA over the same tables (default; KB2_BOUND_NT=128 for the 4-warp instance)
-#define KB2_BOUND_LAUNCH256(MM)                                                                                                     \
+            } else {
+                // m16 x dsub8: the batch's tables from lut_build_kernel, 8 warps per CTA over them
+#define KB2_BOUND_LAUNCH(MM)                                                                                                        \
     pqtc::lut_build_kernel<MM><<<num_sms(), 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
     mark("lut");                                                                                                                    \
-    pqtc::bound_kernel<MM, 32, 1, 8, 256><<<bound_grid, 256, smem, st>>>(s_lut.p, qlist, qcount, nq, sp.probe_ids, sp.probe_dis,     \
-                                                                         nprobe, p0, a_codes, k_base, list_off.p, list_len.p,       \
-                                                                         (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p, \
-                                                                         d_counter.p + 4);
-                if (metric == KB2_METRIC_L2) { KB2_BOUND_LAUNCH256(KB2_METRIC_L2) } else { KB2_BOUND_LAUNCH256(KB2_METRIC_IP) }
-#undef KB2_BOUND_LAUNCH256
-            } else if (metric == KB2_METRIC_L2) {
-                if (roww == 32) { KB2_BOUND_LAUNCH(KB2_METRIC_L2, 32) } else { KB2_BOUND_LAUNCH(KB2_METRIC_L2, 64) }
-            } else {
-                if (roww == 32) { KB2_BOUND_LAUNCH(KB2_METRIC_IP, 32) } else { KB2_BOUND_LAUNCH(KB2_METRIC_IP, 64) }
-            }
+    pqtc::bound_kernel<MM, 1, 8, 256><<<bound_grid, 256, smem, st>>>(s_lut.p, qlist, qcount, nq, sp.probe_ids, sp.probe_dis,         \
+                                                                     nprobe, p0, kTcACodes, k_base, list_off.p, list_len.p,         \
+                                                                     (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p,     \
+                                                                     d_counter.p + 4);
+                if (metric == KB2_METRIC_L2) { KB2_BOUND_LAUNCH(KB2_METRIC_L2) } else { KB2_BOUND_LAUNCH(KB2_METRIC_IP) }
 #undef KB2_BOUND_LAUNCH
+            }
             KB2_CUDA_CHECK(cudaGetLastError());
             last.launches += 2;
-        }
-        } else {
-            // other geometries: the query-major LUT kernel over the first probes gives the exact k_base-th best key of those
-            // lists (any subset of the codes yields a valid bound)
-            int64_t avg_len = std::max<int64_t>(1, n_total / std::max<int64_t>(1, nlist));
-            const int pA = (int)std::min<int64_t>(nprobe, std::max<int64_t>(2, (a_codes + avg_len - 1) / avg_len + 1) * std::max(1, shard_world));
-            IvfScanParams a = sp;
-            a.nprobe = pA;
-            a.probe_stride = nprobe;
-            a.nsplit = 1;
-            a.partial = s_partial2.p;
-            a.partial_stride = 0;
-            a.counters = d_counter.p + 4;
-            a.qperm = nullptr;
-            launch_scan(a, (unsigned)nq, Ksel, pA, has_bits);
-            fltc::extract_bound_kernel<<<grid1d(nq, 256), 256, 0, st>>>(s_partial2.p, Ksel, k_base, nq, s_bound.p);
-            last.launches += 1;
         }
         if (dist) comm->all_reduce_min_f32(s_bound.p, s_bound.p, (size_t)nq, st);
         mark("phaseA");
@@ -1093,9 +1009,8 @@ struct IvfIndex : IndexBase {
         pqtc::plan_kernel<<<1, 1024, 0, ps>>>(s_lcount.p, (int)nlist, s_lstart.p, item_list, item_q0, item_nq, s_plan_out.p);
         {
             // per tile: decode ~ constant, contraction ~ columns (+ the test K-step)
-            // dynamic draw (default): items in descending cost order, CTAs take the next one when free; KB2_TC_SCHED=static
-            // keeps the fixed round-robin assignment with the snake deal
-            int32_t* bal = balance_items(s_items.p, max_items, tc_dynamic_sched() ? 0 : num_sms(), 600, 5, ps);
+            // items in descending cost order, CTAs take the next one when free
+            int32_t* bal = balance_items(s_items.p, max_items, 600, 5, ps);
             item_list = bal;
             item_q0 = bal + max_items;
             item_nq = bal + 2 * max_items;
@@ -1119,10 +1034,8 @@ struct IvfIndex : IndexBase {
         tp.qb16 = (const __nv_bfloat16*)s_qb16.p;
         tp.qnorm = s_qnorm.p;
         tp.n_items = s_plan_out.p;
-        if (tc_dynamic_sched()) {
-            tp.ticket = s_plan_out.p + 4;
-            KB2_CUDA_CHECK(cudaMemsetAsync(tp.ticket, 0, 4, st));
-        }
+        tp.ticket = s_plan_out.p + 4;
+        KB2_CUDA_CHECK(cudaMemsetAsync(tp.ticket, 0, 4, st));
         tp.item_list = item_list;
         tp.item_q0 = item_q0;
         tp.item_nq = item_nq;
@@ -1142,15 +1055,14 @@ struct IvfIndex : IndexBase {
         tp.pqc16 = (const uint4*)tc_pqc16.p;
         tp.bitset = sp.bitset;
         tp.rows = rows.p;
-        const int n_logs = 2 * num_sms();   // one per epilogue group (+ 1 legacy slot that stays empty)
+        const int n_logs = 2 * num_sms();   // one per epilogue group
         const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(nq * 1024 / n_logs, 16384), 1 << 19);
-        s_log.ensure((size_t)(n_logs + 1) * log_cap);
+        s_log.ensure((size_t)n_logs * log_cap);
         s_logcnt.ensure(n_logs + 8);
         KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (n_logs + 8) * 4, st));
         tp.log = s_log.p;
         tp.log_cnt = s_logcnt.p;
         tp.log_cap = log_cap;
-        tp.shared_cap = log_cap;
         tp.qflag = s_cand_cnt.p + nq;
         tp.counters = d_counter.p;
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
@@ -1165,14 +1077,13 @@ struct IvfIndex : IndexBase {
         KB2_CUDA_CHECK(cudaGetLastError());
         mark("tc_filter");
         // ---- survivors: group by query, exact fp32 keys (bit-identical to the LUT engine's)
-        pqtc::scatter_survivors_kernel<<<dim3(16, n_logs + 1), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, log_cap, s_cand.p, s_cand_cnt.p,
-                                                                         kTcCandCap, tp.qflag, d_counter.p);
+        pqtc::scatter_survivors_kernel<<<dim3(16, n_logs), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p,
+                                                                     kTcCandCap, tp.qflag, d_counter.p);
+        // exact_eval trims every survivor row to its k_base best.  Measured at C3: step 1.977 -> 1.957 ms
 #define KB2_TC_EVAL(MM, GG, DD)                                                                                                      \
     pqtc::exact_eval_kernel<MM, GG, DD><<<(unsigned)nq, 128, 0, st>>>(sp.queries, pqc.p, eval_lut, s_bound.p, (const uint4*)codes.p, npad, t1.p,  \
                                                                       sp.bitset, rows.p, s_cand.p, s_cand_cnt.p, kTcCandCap, tp.qflag,  \
-                                                                      s_logcnt.p + n_logs + 1, eval_trim ? k_base : 0);
-        // trim every survivor row to its k' best inside exact_eval (KB2_EVAL_TRIM=0: off).  Measured at C3: step 1.977 -> 1.957 ms
-        static const bool eval_trim = [] { const char* e = getenv("KB2_EVAL_TRIM"); return !(e && atoi(e) == 0); }();
+                                                                      s_logcnt.p + n_logs + 1, k_base);
         const float* eval_lut = (tc_geom_18() && !dist) ? s_lut.p : nullptr;   // tables of the whole batch exist only without a communicator
         if (tc_geom_18()) {
             if (metric == KB2_METRIC_L2) { KB2_TC_EVAL(KB2_METRIC_L2, 1, 8) } else { KB2_TC_EVAL(KB2_METRIC_IP, 1, 8) }
@@ -1279,7 +1190,7 @@ struct IvfIndex : IndexBase {
         int32_t* item_nq = s_items.p + 2 * max_items;
         fltc::plan_kernel<<<1, 1024, 0, st>>>(s_lcount.p, (int)nlist, item_cap, s_lstart.p, item_list, item_q0, item_nq, s_plan_out.p);
         {
-            int32_t* bal = balance_items(s_items.p, max_items, tc_dynamic_sched() ? 0 : num_sms(), 1000, 2);   // a tile is bound by its HBM stream
+            int32_t* bal = balance_items(s_items.p, max_items, 1000, 2);   // a tile is bound by its HBM stream
             item_list = bal;
             item_q0 = bal + max_items;
             item_nq = bal + 2 * max_items;
@@ -1298,10 +1209,8 @@ struct IvfIndex : IndexBase {
         fpar.metric = metric;
         fpar.d = dim;
         fpar.n_items = s_plan_out.p;
-        if (tc_dynamic_sched()) {
-            fpar.ticket = s_plan_out.p + 4;
-            KB2_CUDA_CHECK(cudaMemsetAsync(fpar.ticket, 0, 4, st));
-        }
+        fpar.ticket = s_plan_out.p + 4;
+        KB2_CUDA_CHECK(cudaMemsetAsync(fpar.ticket, 0, 4, st));
         fpar.item_list = item_list;
         fpar.item_q0 = item_q0;
         fpar.item_nq = item_nq;
@@ -1345,136 +1254,10 @@ struct IvfIndex : IndexBase {
 
     // coarse quantizer for queries [q_lo, q_hi): top-nprobe centroids with exact dis0 (F/IndexIVF.cpp:336-342) into rows
     // [q_lo, q_hi) of s_probe_ids / s_probe_dis
-    // Coarse stage on the list-major tensor-core kernel: the centroid table is ONE pseudo-list scanned by every query, i.e. an
-    // IVF_FLAT search with k = nprobe + 16.  The admission bound comes from a sample (the first nlist/8 centroids through the
-    // dense path: its k'-th best key, k' = 2x the expected share + 8), so the kernel logs ~2(nprobe+16) candidates per query
-    // instead of writing the [nq][nlist] key matrix that a separate selection kernel had to read back.  The bound is a
-    // heuristic, so it is CHECKED: a query with fewer than nprobe + 16 candidates raises a counter and the caller repeats
-    // the search with the dense path (counter slot 8; never observed on the benchmark shapes).
-    bool coarse_tc_disabled = false;
-    DevBuf<float> s_cbound;
-    DevBuf<int64_t> s_coff;
-    DevBuf<int32_t> s_clen;
-    bool
-    use_coarse_tc(int64_t m, int nprobe) const {
-        const char* e = getenv("KB2_COARSE");
-        if (coarse_tc_disabled || (e && !strcmp(e, "dense"))) return false;
-        if (dim % fltc::BK != 0 || nlist < 1024 || nprobe + 16 > 256 || nprobe + 16 > nlist / 8) return false;
-        // opt-in (KB2_COARSE=tc): at C3 (10000 x 4096 centroids) the list-major kernel + its sample bound cost more than the
-        // dense GEMM + select it would replace
-        return e && !strcmp(e, "tc") && m >= 296;
-    }
-    void
-    coarse_probes_tc(const float* Q, int64_t m, int nprobe, int64_t* out_ids, float* out_dis) {
-        cudaStream_t st = stream;
-        const int need = nprobe + 16;
-        // ---- sample bound
-        const int64_t ns = std::max<int64_t>(512, (nlist / 8 + 127) / 128 * 128);
-        const int k_sample = (int)std::min<int64_t>(ns, 2 * ((int64_t)need * ns + nlist - 1) / nlist + 8);
-        DensePlan pl = dense_candidates(*this, Q, m, centroids.p, cnorms.p, ns, dim, metric, std::max(k_sample, 17) - 16 + 16, nullptr, nullptr);
-        KB2_REQUIRE(k_sample <= pl.Ksel, KB2_INTERNAL_ERROR, "coarse sample selection too small");
-        s_cbound.ensure((size_t)m);
-        fltc::extract_bound_kernel<<<grid1d(m, 256), 256, 0, st>>>(s_partial.p, pl.stride(), k_sample, m, s_cbound.p);
-        // ---- items: chunks of consecutive queries over the single pseudo-list [0, nlist)
-        const int item_cap = (m / 128 < 2 * num_sms()) ? 32 : 128;
-        const int64_t n_it = (m + item_cap - 1) / item_cap;
-        const int64_t npairs_pad = m + fltc::NQ_ITEM;
-        s_items.ensure((size_t)3 * n_it);
-        s_plan_out.ensure(8);
-        s_pair_q.ensure((size_t)m);
-        s_qnorm.ensure((size_t)m);
-        s_cand.ensure((size_t)m * kTcCandCap);
-        s_cand_cnt.ensure((size_t)2 * m + 4);
-        s_qhi.ensure((size_t)npairs_pad * dim);
-        s_qlo.ensure((size_t)npairs_pad * dim);
-        if (s_coff.n < 1) {
-            s_coff.ensure(1);
-            s_clen.ensure(1);
-        }
-        const int64_t h_off = 0;
-        const int32_t h_len = (int32_t)nlist;
-        KB2_CUDA_CHECK(cudaMemcpyAsync(s_coff.p, &h_off, 8, cudaMemcpyHostToDevice, st));
-        KB2_CUDA_CHECK(cudaMemcpyAsync(s_clen.p, &h_len, 4, cudaMemcpyHostToDevice, st));
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_cand_cnt.p, 0, ((size_t)2 * m + 4) * 4, st));
-        int32_t* item_list = s_items.p;
-        int32_t* item_q0 = s_items.p + n_it;
-        int32_t* item_nq = s_items.p + 2 * n_it;
-        fltc::uniform_items_kernel<<<grid1d(std::max<int64_t>(m, n_it), 256), 256, 0, st>>>(m, item_cap, item_list, item_q0, item_nq,
-                                                                                         s_plan_out.p, s_pair_q.p);
-        fltc::gather_split_queries_kernel<<<grid1d(npairs_pad * 32, 256), 256, 0, st>>>(Q, s_pair_q.p, m, npairs_pad, dim, s_qhi.p, s_qlo.p);
-        row_norms_kernel<<<grid1d(m * 32, 256), 256, 0, st>>>(Q, m, dim, s_qnorm.p);
-        CUtensorMap tx, thi, tlo;
-        KB2_REQUIRE(tc::make_tmap(&tx, centroids.p, nlist, dim) && tc::make_tmap(&thi, s_qhi.p, npairs_pad, dim, item_cap) &&
-                        tc::make_tmap(&tlo, s_qlo.p, npairs_pad, dim, item_cap),
-                    KB2_INTERNAL_ERROR, "coarse tensor-core stage: tensor map encoding failed");
-        fltc::Params fpar{};
-        fpar.metric = metric;
-        fpar.d = dim;
-        fpar.n_items = s_plan_out.p;
-        if (tc_dynamic_sched()) {
-            fpar.ticket = s_plan_out.p + 4;
-            KB2_CUDA_CHECK(cudaMemsetAsync(fpar.ticket, 0, 4, st));
-        }
-        fpar.item_list = item_list;
-        fpar.item_q0 = item_q0;
-        fpar.item_nq = item_nq;
-        fpar.pair_q = s_pair_q.p;
-        fpar.qnorm2 = s_qnorm.p;
-        fpar.bound = s_cbound.p;
-        fpar.list_off = s_coff.p;
-        fpar.list_len = s_clen.p;
-        fpar.xnorm2 = cnorms.p;
-        fpar.bitset = nullptr;
-        fpar.rows = nullptr;
-        const int grid = (int)std::min<int64_t>(num_sms(), n_it);
-        const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(m * 1024 / grid, 32768), 1 << 20);
-        s_log.ensure((size_t)num_sms() * log_cap);
-        s_logcnt.ensure(num_sms() + 8);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (num_sms() + 8) * 4, st));
-        fpar.log = s_log.p;
-        fpar.log_cnt = s_logcnt.p;
-        fpar.log_cap = log_cap;
-        fpar.counters = nullptr;
-#define KB2_FL_LAUNCH(MM, BR) \
-    fltc::ivfflat_tc_kernel<MM, BR><<<grid, fltc::THREADS, fltc::FlCfg<BR>::SMEM_BYTES, st>>>(tx, thi, tlo, fpar);
-        if (metric == KB2_METRIC_L2) {
-            if (item_cap == 32) { KB2_FL_LAUNCH(KB2_METRIC_L2, 32) } else { KB2_FL_LAUNCH(KB2_METRIC_L2, 128) }
-        } else {
-            if (item_cap == 32) { KB2_FL_LAUNCH(KB2_METRIC_IP, 32) } else { KB2_FL_LAUNCH(KB2_METRIC_IP, 128) }
-        }
-#undef KB2_FL_LAUNCH
-        KB2_CUDA_CHECK(cudaGetLastError());
-        uint32_t* qflag = s_cand_cnt.p + m;
-        fltc::scatter_kernel<<<dim3(16, grid), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p, kTcCandCap, qflag);
-        fltc::check_counts_kernel<<<grid1d(m, 256), 256, 0, st>>>(s_cand_cnt.p, qflag, m, (uint32_t)std::min<int64_t>(need, nlist),
-                                                                s_logcnt.p + grid, d_counter.p + 8);
-        last.launches += 8;
-        FinalizeParams fp{};
-        fp.partial = s_cand.p;
-        fp.partial_stride = kTcCandCap;
-        fp.n_partial = kTcCandCap;
-        fp.counts = s_cand_cnt.p;
-        fp.k_sel = (int)std::min<int64_t>(need, nlist);
-        fp.k_out = nprobe;
-        fp.rerank = 1;
-        fp.raw = centroids.p;
-        fp.raw_by_pos = 1;
-        fp.queries = Q;
-        fp.d = dim;
-        fp.metric = metric;
-        fp.out_ids = out_ids;
-        fp.out_dist = out_dis;
-        launch_finalize(*this, fp, m);
-    }
-
     void
     coarse_probes(const float* dq, int64_t q_lo, int64_t q_hi, int nprobe) {
         const int64_t m = q_hi - q_lo;
         if (m <= 0) return;
-        if (!distributed() && use_coarse_tc(m, nprobe)) {
-            coarse_probes_tc(dq + q_lo * dim, m, nprobe, s_probe_ids.p + q_lo * nprobe, s_probe_dis.p + q_lo * nprobe);
-            return;
-        }
         DensePlan pl = dense_candidates(*this, dq + q_lo * dim, m, centroids.p, cnorms.p, nlist, dim, metric, nprobe + 16, nullptr,
                                         nullptr);
         FinalizeParams fp{};
@@ -1527,7 +1310,6 @@ struct IvfIndex : IndexBase {
             d_dist = s_out_dist.p;
         }
 
-        KB2_CUDA_CHECK(cudaMemsetAsync(d_counter.p + 8, 0, 8, st));
         // ---- coarse quantizer.  With a communicator every rank ranks the centroids for its slice of the batch only and the
         //      probe lists are all-gathered (in place; slices padded to the same length).
         const int64_t per = dist ? (nq + shard_world - 1) / shard_world : nq;
@@ -1655,23 +1437,9 @@ struct IvfIndex : IndexBase {
             last.launches += 3;
         }
         unsigned long long* hc = (unsigned long long*)h_counter.p;
-        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, d_counter.p, 72, cudaMemcpyDeviceToHost, st));
+        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, d_counter.p, 64, cudaMemcpyDeviceToHost, st));
         results_out(nq, k, out_ids, out_dist, d_ids, d_dist);
         KB2_REQUIRE(hc[1] == 0 && hc[5] == 0, KB2_INTERNAL_ERROR, "ivfpq_scan_kernel: unexpected shared-memory window base");
-        if (hc[8] != 0 && !coarse_tc_disabled) {
-            // the sampled admission bound of the tensor-core coarse stage left some query short of candidates: repeat the
-            // whole search with the dense coarse path (results of this pass are discarded)
-            coarse_tc_disabled = true;
-            try {
-                search(q, nq, k, cfg, bitset, nbits, out_ids, out_dist);
-            } catch (...) {
-                coarse_tc_disabled = false;
-                throw;
-            }
-            coarse_tc_disabled = false;
-            last.flagged += (int64_t)hc[8];
-            return;
-        }
         last.survivors = (int64_t)hc[2];
         last.flagged = (int64_t)hc[7];
         const unsigned long long scanned = hc[0];

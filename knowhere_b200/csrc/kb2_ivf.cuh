@@ -67,7 +67,6 @@ struct IvfScanParams {
     const int32_t* flag_list;      //   the compacted list of flagged queries (flag_list[0..*flag_count)) x nsplit probe slices
     const uint32_t* flag_count;
     int clear_to;                  // the LAST probe slice fills its output with kEmpty from entry kout up to this entry count
-    int flags;                     // bit1: software L2 prefetch of upcoming chunks; bit2: full-sort final merge (A/B switches)
 };
 
 // probe bookkeeping in shared memory
@@ -148,10 +147,10 @@ struct PqStage {
     bool valid;     // stage holds a chunk (warp-uniform)
 };
 
-template <int G, int METRIC, bool HAS_BITSET, int NT, int NACC>
+template <int G, int METRIC, bool HAS_BITSET>
 __device__ __forceinline__ void
 ivfpq_scan_body(const IvfScanParams& p, const int64_t bq, const int split) {
-    constexpr int NW = NT / 32;
+    constexpr int NW = kScanWarps;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     unsigned char* lut = smem_raw;
     uint64_t* lists = (uint64_t*)(smem_raw + (size_t)G * 65536);
@@ -295,11 +294,11 @@ ivfpq_scan_body(const IvfScanParams& p, const int64_t bq, const int split) {
             st.w[g] = ldg_stream_u4(cp);
             // pull the chunk this warp will want four iterations from now into L2 (same list most of the
             // time; a stray prefetch into the next list or the tail padding is harmless)
-            if (p.flags & 2) asm volatile("prefetch.global.L2 [%0];" ::"l"(cp + 4 * NW * 32));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(cp + 4 * NW * 32));
         }
         if (METRIC == KB2_METRIC_L2) {
             st.t = __ldg(p.t1 + st.pos);
-            if ((p.flags & 2) && lane == 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.t1 + st.pos + 4 * NW * 32));
+            if (lane == 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.t1 + st.pos + 4 * NW * 32));
         } else {
             st.t = 0.f;
         }
@@ -307,19 +306,11 @@ ivfpq_scan_body(const IvfScanParams& p, const int64_t bq, const int split) {
         if (it_ci >= it_nch) it_load();
     };
     auto adc_key = [&](const PqStage<G>& st) -> float {
-        if (NACC == 4) {
-            float acc0 = st.t, acc1 = 0.f, acc2 = 0.f, acc3 = 0.f;
-            pq_group_sum<0>(st.w[0], lane4, acc0, acc1, acc2, acc3);
-            if (G > 1) pq_group_sum<1>(st.w[G > 1 ? 1 : 0], lane4, acc0, acc1, acc2, acc3);
-            if (G > 2) pq_group_sum<2>(st.w[G > 2 ? 2 : 0], lane4, acc0, acc1, acc2, acc3);
-            return st.d0 + ((acc0 + acc1) + (acc2 + acc3));
-        } else {
-            float acc0 = st.t, acc1 = 0.f;
-            pq_group_sum<0>(st.w[0], lane4, acc0, acc1, acc0, acc1);
-            if (G > 1) pq_group_sum<1>(st.w[G > 1 ? 1 : 0], lane4, acc0, acc1, acc0, acc1);
-            if (G > 2) pq_group_sum<2>(st.w[G > 2 ? 2 : 0], lane4, acc0, acc1, acc0, acc1);
-            return st.d0 + (acc0 + acc1);
-        }
+        float acc0 = st.t, acc1 = 0.f;
+        pq_group_sum<0>(st.w[0], lane4, acc0, acc1, acc0, acc1);
+        if (G > 1) pq_group_sum<1>(st.w[G > 1 ? 1 : 0], lane4, acc0, acc1, acc0, acc1);
+        if (G > 2) pq_group_sum<2>(st.w[G > 2 ? 2 : 0], lane4, acc0, acc1, acc0, acc1);
+        return st.d0 + (acc0 + acc1);
     };
     auto admit = [&](const PqStage<G>& st, float key, float bound) {
         bool pass = st.ok && key <= bound;            // one float compare on the hot path
@@ -359,15 +350,11 @@ ivfpq_scan_body(const IvfScanParams& p, const int64_t bq, const int split) {
         for (int i = p.kout + threadIdx.x; i < p.clear_to; i += blockDim.x) out[i] = kEmpty;
     tk.finish(lane);
     __syncthreads();
-    if (p.flags & 4) {
-        block_emit_topk(lists, p.K, out, p.kout, NW);   // A/B switch: plain full sort of all warp buffers
-    } else {
-        block_emit_topk_bounded(lists, p.K, NW, *sh_V_final, merge_tmp, 4 * p.K, merge_ctr, out, p.kout);
-    }
+    block_emit_topk_bounded(lists, p.K, NW, *sh_V_final, merge_tmp, 4 * p.K, merge_ctr, out, p.kout);
 }
 
-template <int G, int METRIC, bool HAS_BITSET, int NT, int NACC = 2>
-__global__ void __launch_bounds__(NT, G == 1 ? (NT == 512 ? 2 : 3) : 1)
+template <int G, int METRIC, bool HAS_BITSET>
+__global__ void __launch_bounds__(kScanThreads, G == 1 ? 3 : 1)
 ivfpq_scan_kernel(IvfScanParams p) {
     if (p.only_flagged) {
         // redo pass of the tensor-core engine: a small grid walks the (query, probe slice) units and scans only the
@@ -377,12 +364,12 @@ ivfpq_scan_kernel(IvfScanParams p) {
             const int64_t bq = p.flag_list[w / p.nsplit];
             const int split = (int)(w % p.nsplit);
             if (threadIdx.x == 0 && split == 0 && p.counters) atomicAdd(p.counters + 3, 1ull);   // queries redone by this pass
-            ivfpq_scan_body<G, METRIC, HAS_BITSET, NT, NACC>(p, bq, split);
+            ivfpq_scan_body<G, METRIC, HAS_BITSET>(p, bq, split);
             __syncthreads();
         }
         return;
     }
-    ivfpq_scan_body<G, METRIC, HAS_BITSET, NT, NACC>(p, (int64_t)(blockIdx.x / p.nsplit), (int)(blockIdx.x % p.nsplit));
+    ivfpq_scan_body<G, METRIC, HAS_BITSET>(p, (int64_t)(blockIdx.x / p.nsplit), (int)(blockIdx.x % p.nsplit));
 }
 
 // =====================================================================================

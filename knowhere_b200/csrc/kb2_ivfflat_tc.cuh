@@ -50,7 +50,7 @@ constexpr float kSlack = 3e-5f;   // 3xTF32 contraction error, relative to |q|^2
 struct Params {
     int metric, d;
     const int32_t* n_items;
-    int32_t* ticket;              // optional work counter (see pqtc::Params::ticket)
+    int32_t* ticket;              // work counter (see pqtc::Params::ticket)
     const int32_t* item_list;
     const int32_t* item_q0;       // first pair of the item
     const int32_t* item_nq;
@@ -173,7 +173,6 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         sch_ready[threadIdx.x] = -1;
     }
     auto item_at_thread = [&](int seq) -> int {
-        if (!p.ticket) return (int)blockIdx.x + seq * (int)gridDim.x;
         const int sl = seq & (SCHED_R - 1);
         if (sch_ready[sl] != seq) {
             if (atomicCAS(sch_claim + sl, seq - SCHED_R, seq) == seq - SCHED_R) {
@@ -382,29 +381,6 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         p.log_cnt[blockIdx.x] = min(*log_cursor, p.log_cap);
         if (p.counters) atomicAdd(p.counters, n_rows);
     }
-}
-
-// items that cut ONE pseudo-list of rows (the coarse quantizer's centroids) into chunks of `cap` consecutive queries
-__global__ void
-uniform_items_kernel(int64_t nq, int cap, int32_t* __restrict__ item_list, int32_t* __restrict__ item_q0, int32_t* __restrict__ item_nq,
-                     int32_t* __restrict__ n_items, int32_t* __restrict__ pair_q) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t ni = (nq + cap - 1) / cap;
-    if (i == 0) *n_items = (int32_t)ni;
-    if (i < ni) {
-        item_list[i] = 0;
-        item_q0[i] = (int32_t)(i * cap);
-        item_nq[i] = (int32_t)min((int64_t)cap, nq - i * cap);
-    }
-    if (i < nq) pair_q[i] = (int32_t)i;
-}
-// queries whose candidate row cannot serve the selection (fewer than `need` entries, or overflowed) -> *out += 1 each
-__global__ void
-check_counts_kernel(const uint32_t* __restrict__ cand_cnt, const uint32_t* __restrict__ qflag, int64_t nq, uint32_t need,
-                    const uint32_t* __restrict__ log_over, unsigned long long* __restrict__ out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i == 0 && *log_over) atomicAdd(out, 1ull);
-    if (i < nq && (qflag[i] || cand_cnt[i] < need)) atomicAdd(out, 1ull);
 }
 
 // survivors of all CTA logs -> per-query candidate rows as packed (key, position)   (grid = (x, number of logs))

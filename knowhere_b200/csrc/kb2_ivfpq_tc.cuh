@@ -88,8 +88,8 @@ struct Params {
     const float* qnorm;            // [nq]
     // plan
     const int32_t* n_items;        // device scalar
-    int32_t* ticket;               // optional work counter (zeroed before the launch): CTAs draw items from it in order, so a
-                                   // CTA that got short items simply draws more (NULL: item = blockIdx.x + seq * gridDim.x)
+    int32_t* ticket;               // work counter (zeroed before the launch): CTAs draw items from it in order, so a
+                                   // CTA that got short items simply draws more
     const int32_t* item_list;      // [items]
     const int32_t* item_q0;        // [items] first pair of the chunk
     const int32_t* item_nq;        // [items]
@@ -112,12 +112,11 @@ struct Params {
     const uint8_t* bitset;
     const int32_t* rows;
     // output
-    uint4* log;                    // [2*gridDim.x + 1][log_cap] survivors {query, position, key base bits, 0}: one log per
-                                   // epilogue group, the last one shared by all for tiles that overflow the smem queue
-    uint32_t* log_cnt;             // [2*gridDim.x] entries per private log; [2G] cursor of the shared log;
+    uint4* log;                    // [2*gridDim.x][log_cap] survivors {query, position, key base bits, 0}: one log per
+                                   // epilogue group
+    uint32_t* log_cnt;             // [2*gridDim.x] entries per log; [2G] unused;
                                    // [2G + 1] = 1 when any log overflowed; [2G + 2..3] diagnostics
-    uint32_t log_cap;              // entries per private log
-    uint32_t shared_cap;           // entries of the shared log
+    uint32_t log_cap;              // entries per log
     uint32_t* qflag;               // [nq] 1: redo this query with the LUT kernel
     unsigned long long* counters;  // [0] codes scanned (pairs x codes), [2] survivors re-evaluated, [3] flagged
 };
@@ -228,7 +227,6 @@ ivfpq_tc_filter_kernel(Params p) {
         sch_ready[threadIdx.x] = -1;
     }
     auto item_at = [&](int seq) -> int {   // warp-uniform call
-        if (!p.ticket) return (int)blockIdx.x + seq * (int)gridDim.x;
         int v = 0;
         if (lane == 0) {
             const int sl = seq & (SCHED_R - 1);
@@ -457,7 +455,7 @@ ivfpq_tc_filter_kernel(Params p) {
         const int eg = et >> 7;                  // group
         const int e = et & 127;                  // thread inside the group
         const int we = warp & 3;                 // warp inside the warpgroup: rows 16 we .. 16 we + 15 of a 64-row half
-        const uint32_t n_logs = 2u * gridDim.x;  // private logs (log n_logs, the former shared one, stays empty)
+        const uint32_t n_logs = 2u * gridDim.x;  // logs: one per epilogue group
         uint4* my_log = p.log + (size_t)(2 * blockIdx.x + eg) * p.log_cap;
         uint32_t* my_cursor = qcnt + eg;
         bool log_over = false;
@@ -653,10 +651,9 @@ plan_kernel(const int32_t* __restrict__ lcount, int nlist, int32_t* __restrict__
     if (threadIdx.x == 0) *n_items = carry_b;
 }
 
-// ---- static load balancing of the persistent kernels.  CTA b processes items b, b + G, b + 2G, ...; in list order the per-CTA
-// totals differ by +-30 % (list length x queries per list has a heavy tail), and the launch lasts as long as its slowest CTA.
-// Items are therefore sorted by descending cost estimate and dealt out in snake order (round r forwards, round r+1
-// backwards), the classic longest-processing-time deal.
+// ---- load balancing of the persistent kernels.  Item costs have a heavy tail (list length x queries per list), and the
+// launch lasts as long as its slowest CTA.  Items are therefore sorted by descending cost estimate and drawn in that order
+// through Params::ticket (longest processing time first): a CTA that got short items simply draws more.
 __global__ void
 item_cost_kernel(const int32_t* __restrict__ n_items, const int32_t* __restrict__ item_list, const int32_t* __restrict__ item_nq,
                  const int32_t* __restrict__ list_len, int64_t max_items, int tile_cost, int col_cost, uint32_t* __restrict__ key,
@@ -673,22 +670,15 @@ item_cost_kernel(const int32_t* __restrict__ n_items, const int32_t* __restrict_
     idx[i] = (int32_t)i;
 }
 __global__ void
-deal_items_kernel(const int32_t* __restrict__ n_items, const int32_t* __restrict__ sorted_idx, int G, const int32_t* __restrict__ in_list,
+deal_items_kernel(const int32_t* __restrict__ n_items, const int32_t* __restrict__ sorted_idx, const int32_t* __restrict__ in_list,
                   const int32_t* __restrict__ in_q0, const int32_t* __restrict__ in_nq, int32_t* __restrict__ out_list,
                   int32_t* __restrict__ out_q0, int32_t* __restrict__ out_nq) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;   // rank by descending cost
-    const int n = *n_items;
-    if (j >= n) return;
-    int dst = j;   // G == 0: plain descending-cost order (drawn dynamically through Params::ticket)
-    if (G > 0) {
-        const int r = j / G, b = j % G;
-        const bool full_round = (r + 1) * G <= n;
-        dst = r * G + (((r & 1) && full_round) ? (G - 1 - b) : b);
-    }
+    if (j >= *n_items) return;
     const int src = sorted_idx[j];
-    out_list[dst] = in_list[src];
-    out_q0[dst] = in_q0[src];
-    out_nq[dst] = in_nq[src];
+    out_list[j] = in_list[src];
+    out_q0[j] = in_q0[src];
+    out_nq[j] = in_nq[src];
 }
 
 __global__ void
@@ -761,9 +751,9 @@ unrotate_codes_kernel(const uint8_t* __restrict__ rot, int64_t total_words /* G 
 // survivors of all CTA logs -> per-query rows (thread per log entry; grid = (x, number of logs))
 __global__ void
 scatter_survivors_kernel(const uint4* __restrict__ log, const uint32_t* __restrict__ log_cnt, uint32_t log_cap,
-                         uint32_t shared_cap, uint64_t* __restrict__ cand, uint32_t* __restrict__ cand_cnt, int cap, uint32_t* __restrict__ qflag,
+                         uint64_t* __restrict__ cand, uint32_t* __restrict__ cand_cnt, int cap, uint32_t* __restrict__ qflag,
                          unsigned long long* __restrict__ counters) {
-    const uint32_t n = min(log_cnt[blockIdx.y], blockIdx.y + 1 == gridDim.y ? shared_cap : log_cap);   // last log = shared one
+    const uint32_t n = min(log_cnt[blockIdx.y], log_cap);
     const uint4* src = log + (size_t)blockIdx.y * log_cap;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint4 e = src[i];
@@ -1088,12 +1078,12 @@ compact_flags_kernel(const uint32_t* __restrict__ qflag, int64_t nq, int32_t* __
 // row[w] = LUT[w % 16][j]; lane i reads word (i % 16) + s at step s, i.e. sub-quantizer (pos + s) % 16 — the address
 // is one byte-permute plus an immediate (PRMT + LDS + FADD per look-up, like the LUT kernel), lanes i and i+16 share
 // a bank (2 wavefronts per gather).  The keys go to shared memory and the bound is read off a 1024-bin histogram
-// (no top-k structure at all).  grid = nq, block = NT (128 or 256); dynamic smem = bound_smem(ROWW, bound_kmax(...)) (48 KB at C3).
+// (no top-k structure at all).  grid = nq, block = NT (128 or 256); dynamic smem = bound_smem(bound_kmax(...)) (48 KB at C3).
 #define KB2_BOUND_STEP(WORD, KB, S, ACC)                                                      \
     {                                                                                         \
         const uint32_t _x = __byte_perm((WORD), lane4, 0x6504u | ((KB) << 4));                \
         float _v;                                                                             \
-        asm("ld.shared.f32 %0, [%1+%2];" : "=f"(_v) : "r"(_x >> (ROWW == 32 ? 1 : 0)), "n"(KB2_SMEM_BASE + 4 * (S))); \
+        asm("ld.shared.f32 %0, [%1+%2];" : "=f"(_v) : "r"(_x >> 1), "n"(KB2_SMEM_BASE + 4 * (S))); \
         ACC += _v;                                                                            \
     }
 // pqc [M][256][dsub] -> pqc_t [M/16][256][16][dsub] (the 16 sub-quantizers of a group adjacent: coalesced table builds)
@@ -1109,23 +1099,21 @@ transpose_codebook_kernel(const float* __restrict__ pqc, int M, int dsub, float*
 }
 constexpr int BOUND_KMAX = 6144;    // keys held per query (phase A looks at no more codes than this)
 constexpr int BOUND_BINS = 1024;
-// ROWW = words per code-value row of the skewed table: 32 (32 KB: lanes i and i+16 share a bank, 2 wavefronts per gather,
-// 3 CTAs/SM) or 64 (64 KB: conflict-free like the LUT kernel, 2 CTAs/SM)
 // keys actually held for a launch: the requested number of codes rounded up (C3: 3000 -> 3008 keys = 12 KB instead of 24 KB, i.e.
 // 48 KB per CTA and four CTAs per SM instead of three)
 __host__ __device__ constexpr int bound_kmax(int min_codes, int k_need) {
     const int want = ((min_codes > k_need ? min_codes : k_need) + 63) & ~63;
     return want < BOUND_KMAX ? want : BOUND_KMAX;
 }
-constexpr size_t bound_smem(int roww, int kmax = BOUND_KMAX) { return (size_t)roww * 1024 + (size_t)kmax * 4 + BOUND_BINS * 4 + 128; }
-constexpr size_t BOUND_SMEM = bound_smem(32);
+// the 32 KB skewed table, the keys, the histogram and the reduction words
+constexpr size_t bound_smem(int kmax) { return (size_t)32 * 1024 + (size_t)kmax * 4 + BOUND_BINS * 4 + 128; }
 
 // G > 1 (m = 16 G sub-quantizers, e.g. m48 x dsub2): the groups are scanned one after the other through the same 32 KB
 // table -- group g's table is built in the kernel from the query and the transposed codebook `pqc_t`
 // ([g][code value][16 sub-quantizers][dsub], see transpose_codebook_kernel), the partial sums of the earlier groups wait in
 // the shared key array.
 // NT = threads per CTA: 128 (4 warps) or 256 (8 warps over the same tables: twice the gathers in flight per shared-memory byte)
-template <int METRIC, int ROWW, int G = 1, int DSUB = 8, int NT = 128>
+template <int METRIC, int G, int DSUB, int NT>
 __global__ void __launch_bounds__(NT)
 bound_kernel(const float* __restrict__ lut, const int32_t* __restrict__ qlist, const uint32_t* __restrict__ qcount, int64_t nq,
              const int64_t* __restrict__ probe_ids, const float* __restrict__ probe_dis,
@@ -1134,15 +1122,14 @@ bound_kernel(const float* __restrict__ lut, const int32_t* __restrict__ qlist, c
              const uint8_t* __restrict__ bitset, const int32_t* __restrict__ rows, float* __restrict__ out,
              unsigned long long* __restrict__ counters, int64_t npad = 0, const float* __restrict__ queries = nullptr,
              const float* __restrict__ pqc_t = nullptr) {
-    static_assert(G == 1 || ROWW == 32, "multi-group phase A uses the 32-word table rows");
     static_assert(NT == 128 || NT == 256, "bound_kernel block size");
     constexpr int NW = NT / 32;               // warps
     constexpr int BPT = BOUND_BINS / NT;      // histogram bins owned by a thread
     // work list: table i / query qlist[i] for i < *qcount (qlist == NULL: query i, i < nq); CTAs stride the list
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    float* s_lut = (float*)smem_raw;                              // [256][ROWW]
+    float* s_lut = (float*)smem_raw;                              // [256][32]
     const int key_cap = bound_kmax(min_codes, k_need);            // (the host sizes the shared memory with the same function)
-    float* s_keys = (float*)(smem_raw + ROWW * 1024);             // [key_cap]
+    float* s_keys = (float*)(smem_raw + 32 * 1024);               // [key_cap]
     uint32_t* s_hist = (uint32_t*)(s_keys + key_cap);             // [BOUND_BINS]
     float* s_red = (float*)(s_hist + BOUND_BINS);                 // [32]: min [0,8) max [8,16) warp sums [16,24)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1171,8 +1158,8 @@ bound_kernel(const float* __restrict__ lut, const int32_t* __restrict__ qlist, c
 #pragma unroll
             for (int x = 0; x < DSUB; x++) a = fmaf(qv[x], __ldg(cp + x), a);
             a *= scale;
-            s_lut[j * ROWW + mm] = a;
-            s_lut[j * ROWW + 16 + mm] = a;
+            s_lut[j * 32 + mm] = a;
+            s_lut[j * 32 + 16 + mm] = a;
         }
     } else {
         // lut[q][j*16 + m] -> s_lut[j*32 + m] and s_lut[j*32 + 16 + m]
@@ -1181,18 +1168,16 @@ bound_kernel(const float* __restrict__ lut, const int32_t* __restrict__ qlist, c
         for (int i = 0; i < 1024 / NT; i++) {
             const int idx = threadIdx.x + i * NT;        // float4 index: j = idx / 4, m4 = (idx % 4) * 4
             const float4 v = __ldg(src + idx);
-            float4* dst = reinterpret_cast<float4*>(s_lut + (idx >> 2) * ROWW + (idx & 3) * 4);
+            float4* dst = reinterpret_cast<float4*>(s_lut + (idx >> 2) * 32 + (idx & 3) * 4);
             dst[0] = v;
             dst[4] = v;
-            if (ROWW == 64) { dst[8] = v; dst[12] = v; }
         }
     }
     if (g == 0)
         for (int i = threadIdx.x; i < BOUND_BINS; i += NT) s_hist[i] = 0;
     __syncthreads();
     // PRMT builds (byte << 8) | (lane16 << 3) ; >> 1 = byte * 128 + lane16 * 4 (row pitch 128 B)
-    // ROWW = 64: (byte << 8) | (lane << 2) is the address itself (row pitch 256 B, word lane + s)
-    const uint32_t lane4 = (ROWW == 32) ? ((uint32_t)(lane & 15) << 3) : ((uint32_t)lane << 2);
+    const uint32_t lane4 = (uint32_t)(lane & 15) << 3;
     const uint4* gcodes = codes + (int64_t)g * npad;   // code plane of this group
     const bool first_g = (g == 0), last_g = (g == G - 1);
     seen = 0;

@@ -424,16 +424,3 @@ def test_ivfpq_low_precision_refine_store(kb, rtype):
     assert np.array_equal(ra[0], rc[0]) and np.array_equal(ra[1], rc[1])
     assert a.size() < b.size() - nb * d * 1.5
 
-
-def test_coarse_stage_on_tensor_core_kernel_matches_dense_path(kb):
-    """The coarse quantizer served by the list-major tensor-core kernel (sampled admission bound + check, kb2_index.cuh
-    coarse_probes_tc) must give the probe lists of the dense path (key matrix + selection): same final answers."""
-    nb, d, nlist, nq, k = 150000, 64, 2048, 3000, 10
-    xb = datagen.clustered(nb, d, 42)
-    xq = datagen.clustered(nq, d, 43)
-    for metric in ("L2", "IP"):
-        ix = kb.Index("IVF_FLAT", metric, d, {"nlist": nlist})
-        ix.build(xb)
-        a = _with_env("KB2_COARSE", "tc", lambda: ix.search(xq, k, {"nprobe": 24}))
-        b = _with_env("KB2_COARSE", "dense", lambda: ix.search(xq, k, {"nprobe": 24}))
-        assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]), metric
