@@ -1075,6 +1075,9 @@ struct IvfIndex : IndexBase {
 #undef KB2_TC_LAUNCH
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev3, st));
         KB2_CUDA_CHECK(cudaGetLastError());
+#ifdef KB2_FILTER_STALLS
+        pqtc::filter_stalls_print_kernel<<<1, 1, 0, st>>>(num_sms());
+#endif
         mark("tc_filter");
         // ---- survivors: group by query, exact fp32 keys (bit-identical to the LUT engine's)
         pqtc::scatter_survivors_kernel<<<dim3(16, n_logs), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p,

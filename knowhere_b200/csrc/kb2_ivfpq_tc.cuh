@@ -179,6 +179,34 @@ make_desc_ns(uint32_t smem_addr, uint32_t grp_bytes) {
     return d;   // layout type 0 (no swizzle), base offset 0
 }
 
+// Cycle accounting of the filter kernel's roles, compiled in only with -DKB2_FILTER_STALLS (scripts/filter_stalls.py):
+// one thread per group sums clock64() intervals into stall[slot] and stores them in g_filter_stalls at the end of the
+// launch; filter_stalls_print_kernel, launched after the filter kernel, prints each CTA's sums over both groups of each
+// role (a printf inside the filter kernel is a function call, and ptxas serializes the wgmmas of a kernel that makes
+// one).  Without the macro these expand to nothing, so the default build is unchanged.
+#ifdef KB2_FILTER_STALLS
+#define KB2_STALL_BEGIN(v) const long long v = clock64()
+#define KB2_STALL_END(slot, v) stall[slot] += clock64() - (v)
+constexpr int kStallMaxCtas = 1024, kStallSlots = 8;
+// [CTA][role: 0 decoders, 1 consumers][group][slot]
+__device__ unsigned long long g_filter_stalls[kStallMaxCtas][2][2][kStallSlots];
+__global__ void
+filter_stalls_print_kernel(int ctas) {
+    for (int b = 0; b < min(ctas, kStallMaxCtas); b++) {
+        printf("KB2STALL cta=%d", b);
+        for (int r = 0; r < 2; r++) {
+            printf(r == 0 ? " dec=" : " cons=");
+            for (int i = 0; i < kStallSlots; i++)
+                printf(i ? ",%llu" : "%llu", g_filter_stalls[b][r][0][i] + g_filter_stalls[b][r][1][i]);
+        }
+        printf("\n");
+    }
+}
+#else
+#define KB2_STALL_BEGIN(v)
+#define KB2_STALL_END(slot, v)
+#endif
+
 // x = hi + mid + lo with three bf16 terms (24 significant bits: exact for finite fp32 up to 2^-27 |x|); +-inf -> (+-inf, 0, 0)
 __device__ __forceinline__ void
 split3_bf16(float x, uint32_t& hi, uint32_t& mid, uint32_t& lo) {
@@ -258,6 +286,10 @@ ivfpq_tc_filter_kernel(Params p) {
         qcnt[0] = qcnt[1] = qcnt[2] = qcnt[3] = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+#ifdef KB2_FILTER_STALLS
+    long long stall[kStallSlots] = {0, 0, 0, 0, 0, 0, 0, 0};
+    KB2_STALL_BEGIN(t_role);
+#endif
     // bf16 codebooks -> shared memory
     {
         uint4* tab = (uint4*)(sm + OFF_TAB);
@@ -275,6 +307,7 @@ ivfpq_tc_filter_kernel(Params p) {
         // per-column thresholds of one item -> meta buffer (it & 1), one column per decoder thread; written one item
         // AHEAD of its use so that the dependent global loads (pair -> bound, norm) stay off the critical path
         auto write_meta = [&](int item, int it) {
+            KB2_STALL_BEGIN(t_meta);
             const int par = it & 1;
             mbar_wait_g(bar_meta_free(par), (((uint32_t)it >> 1) & 1u) ^ 1u);
             const int q0 = p.item_q0[item];
@@ -304,6 +337,7 @@ ivfpq_tc_filter_kernel(Params p) {
             m_base[j] = bs;
             m_q[j] = q;
             tc::mbar_arrive(bar_meta_full(par));
+            KB2_STALL_END(5, t_meta);
         };
         uint32_t g0 = 0;   // global tile counter at the start of the item
         int it = 0;
@@ -330,6 +364,7 @@ ivfpq_tc_filter_kernel(Params p) {
                 if (METRIC == KB2_METRIC_L2) t_next = __ldg(p.t1 + off + (int64_t)t_first * TM + tid);
             }
             auto decode_tile = [&](int t) {
+                KB2_STALL_BEGIN(t_dec);
                 const uint32_t g = g0 + (uint32_t)t;      // g & 1 == dg
                 uint4 w[G];
 #pragma unroll
@@ -348,7 +383,9 @@ ivfpq_tc_filter_kernel(Params p) {
                 if (t * TM + tid < len) r = (METRIC == KB2_METRIC_L2) ? 0.5f * tv : 0.f;
                 uint32_t rh, rm, rl;
                 split3_bf16(-r, rh, rm, rl);
+                KB2_STALL_BEGIN(t_ae);
                 mbar_wait_g(bar_a_empty(dg), ((g >> 1) & 1u) ^ 1u);
+                KB2_STALL_END(1, t_ae);
                 unsigned char* A = sm + OFF_A + dg * A_BYTES + (tid >> 3) * GRP_BYTES + (tid & 7) * 16;
                 if constexpr (DSUB == 8) {
                     // chunk = one sub-quantizer (8 bf16): 16 gathers per group through the rotated code bytes.  The table is
@@ -401,14 +438,18 @@ ivfpq_tc_filter_kernel(Params p) {
                 *reinterpret_cast<uint4*>(A + (XCHUNK + 1) * 128) = make_uint4(0u, 0u, 0u, 0u);
                 tc::fence_proxy_async();
                 tc::mbar_arrive(bar_a_full(dg));
+                KB2_STALL_END(3, t_dec);
             };
             // the first tile of each group only needs a free A buffer: decode it while the tensor pipe still works on
             // the previous item, then stage the B operand (which must wait for that item's last MMA)
             if (t_first < ntiles) decode_tile(t_first);
             // ---- B operand: the item's queries (bf16) gathered by index with cp.async, K-major no-swizzle layout,
             //      plus the threshold chunk [1, 1, 1, h_hi, h_mid, h_lo, 0, 0] of every column
+            KB2_STALL_BEGIN(t_b);
             asm volatile("bar.sync 2, 256;" ::: "memory");          // meta[par] (thresholds, query indices) written by all decoders
+            KB2_STALL_BEGIN(t_bf);
             mbar_wait_g(bar_b_free, ((uint32_t)it & 1u) ^ 1u);
+            KB2_STALL_END(2, t_bf);
             {
                 const float* m_h = (const float*)(sm + OFF_META + par * META_BYTES);
                 const int* m_q = (const int*)(m_h + 2 * NQT);
@@ -438,6 +479,7 @@ ivfpq_tc_filter_kernel(Params p) {
             }
             tc::fence_proxy_async();
             tc::mbar_arrive(bar_b_full);
+            KB2_STALL_END(4, t_b);
             // thresholds of the NEXT item (other meta buffer)
             if (item_next < n_items) write_meta(item_next, it + 1);
             // ---- this group's remaining tiles
@@ -476,46 +518,66 @@ ivfpq_tc_filter_kernel(Params p) {
             const int64_t off = p.list_off[l];
             const int ntiles = (len + TM - 1) / TM;
             const int par = it & 1;
+            KB2_STALL_BEGIN(t_mf);
             mbar_wait_g(bar_meta_full(par), ((uint32_t)it >> 1) & 1u);
+            KB2_STALL_END(1, t_mf);
             const float* m_base = (const float*)(sm + OFF_META + par * META_BYTES) + NQT;
             const int* m_q = (const int*)(m_base + NQT);
             if (et == 0) n_codes += (unsigned long long)len * (unsigned long long)nqi;
             const int t_first = (int)((eg - (int)(g0 & 1u)) & 1);
+            KB2_STALL_BEGIN(t_bfull);
             mbar_wait_g(bar_b_full, (uint32_t)it & 1u);
+            KB2_STALL_END(2, t_bfull);
             const uint32_t a0 = base + OFF_A + eg * A_BYTES;
             const uint32_t b0 = base + OFF_B;
+            const uint32_t la0 = (uint32_t)make_desc_ns(a0, GRP_BYTES), lb0 = (uint32_t)make_desc_ns(b0, GRP_BYTES);
+            constexpr uint64_t desc_hi = (uint64_t)(GRP_BYTES >> 4) << 32;   // high word of make_desc_ns (SBO)
             for (int t = t_first; t < ntiles; t += 2) {
                 const uint32_t g = g0 + (uint32_t)t;   // g & 1 == eg
+                KB2_STALL_BEGIN(t_af);
                 mbar_wait_g(bar_a_full(eg), (g >> 1) & 1u);
+                KB2_STALL_END(3, t_af);
                 auto issue = [&](float (&acc)[32], int h, int c) {
-                    const uint32_t a = a0 + (uint32_t)(h * 8 * GRP_BYTES), b = b0 + (uint32_t)(c * 8 * GRP_BYTES);
+                    KB2_STALL_BEGIN(t_is);
+                    // the operand descriptors of the wgmmas differ only in the start-address field (address >> 4) of the
+                    // low word.  Every shared-memory address of the CTA lies below 2^18, so that 14-bit field never carries
+                    // and an offset of x bytes is a 32-bit add of x / 16: one add per descriptor instead of rebuilding it.
+                    const uint32_t la = la0 + (uint32_t)(h * 8 * GRP_BYTES / 16), lb = lb0 + (uint32_t)(c * 8 * GRP_BYTES / 16);
                     tc::fence_operand(acc);
                     tc::wgmma_fence();
 #pragma unroll
                     for (int ks = 0; ks < KSTEPS; ks++)
-                        tc::wgmma_bf16_n64(acc, make_desc_ns(a + ks * 256, GRP_BYTES), make_desc_ns(b + ks * 256, GRP_BYTES), ks > 0 ? 1u : 0u);
+                        tc::wgmma_bf16_n64(acc, desc_hi | (la + ks * 16u), desc_hi | (lb + ks * 16u), ks > 0 ? 1u : 0u);
                     tc::wgmma_commit();
                     tc::fence_operand(acc);
+                    KB2_STALL_END(6, t_is);
                 };
                 // sign test of one block -> bits (c * 16 + 2 j + cc) of the masks of the thread's two rows of half h.  Branch-free:
                 // it runs between the issue and the wait of the next block, where divergent code would make ptxas serialize
                 // the wgmmas.
                 uint64_t mh[2][2] = {{0ull, 0ull}, {0ull, 0ull}};
                 auto test = [&](const float (&v)[32], int h, int c) {
+                    KB2_STALL_BEGIN(t_te);
                     // column 8 j + cc of the block is valid iff 8 j + cc < lim; lim is even, so iff j < ceil(lim / 8)
                     const int lim = nmma - c * 64 - 2 * (lane & 3);
                     const uint32_t valid = (1u << (2 * min(8, max(0, (lim + 7) >> 3)))) - 1u;
-                    uint32_t m0 = 0u, m1 = 0u;
+                    // sign bit of column 8 j + cc (i = 2 j + cc) of the thread's first / second row -> bit i of n0 / n1.  A
+                    // funnel shift (n << 1) | (x >> 31) appends one sign bit in one instruction; columns go in from the
+                    // highest i down, in two chains per row (i < 8, i >= 8) for instruction-level parallelism.
+                    uint32_t n0l = 0u, n0h = 0u, n1l = 0u, n1h = 0u;
 #pragma unroll
-                    for (int j = 0; j < 8; j++) {
-#pragma unroll
-                        for (int cc = 0; cc < 2; cc++) {
-                            m0 |= (~__float_as_uint(v[4 * j + cc]) >> 31) << (2 * j + cc);
-                            m1 |= (~__float_as_uint(v[4 * j + 2 + cc]) >> 31) << (2 * j + cc);
-                        }
+                    for (int i = 7; i >= 0; i--) {
+                        const int x = 4 * (i >> 1) + (i & 1);   // register of column i of the first row; + 2: second row
+                        n0l = __funnelshift_l(__float_as_uint(v[x]), n0l, 1);
+                        n0h = __funnelshift_l(__float_as_uint(v[x + 16]), n0h, 1);
+                        n1l = __funnelshift_l(__float_as_uint(v[x + 2]), n1l, 1);
+                        n1h = __funnelshift_l(__float_as_uint(v[x + 18]), n1h, 1);
                     }
+                    // a pair survives iff its sign bit is clear
+                    const uint32_t m0 = ~((n0h << 8) | n0l), m1 = ~((n1h << 8) | n1l);
                     mh[h][0] |= (uint64_t)(m0 & valid) << (c * 16);   // h and c are compile-time indices (unrolled pipeline)
                     mh[h][1] |= (uint64_t)(m1 & valid) << (c * 16);
+                    KB2_STALL_END(7, t_te);
                 };
                 // survivors of the thread's two rows of half h -> the group's log
                 auto flush = [&](int h) {
@@ -567,9 +629,13 @@ ivfpq_tc_filter_kernel(Params p) {
                         if constexpr (b + 1 < NBT) {
                             if constexpr ((b + 1) & 1) issue(vb, (b + 1) / NB, (b + 1) % NB);
                             else issue(va, (b + 1) / NB, (b + 1) % NB);
+                            KB2_STALL_BEGIN(t_w);
                             tc::wgmma_wait<1>();
+                            KB2_STALL_END(4, t_w);
                         } else {
+                            KB2_STALL_BEGIN(t_w);
                             tc::wgmma_wait<0>();
+                            KB2_STALL_END(4, t_w);
                         }
                         if constexpr (b & 1) {
                             tc::fence_operand(vb);
@@ -581,8 +647,10 @@ ivfpq_tc_filter_kernel(Params p) {
                     });
                 });
                 tc::mbar_arrive(bar_a_empty(eg));   // every wgmma of this tile has retired: hand the A buffer back
+                KB2_STALL_BEGIN(t_fl);
                 flush(0);
                 flush(1);
+                KB2_STALL_END(5, t_fl);
             }
             tc::mbar_arrive(bar_b_free);            // this group's wgmmas of the item have all retired
             tc::mbar_arrive(bar_meta_free(par));
@@ -597,6 +665,16 @@ ivfpq_tc_filter_kernel(Params p) {
         }
         if (et == 0 && p.counters) atomicAdd(p.counters, n_codes);
     }
+#ifdef KB2_FILTER_STALLS
+    // decoder slots: total, a_empty wait, b_free wait, decode_tile (incl. its a_empty wait), B staging (incl. its b_free
+    // wait), write_meta
+    // consumer slots: total, meta_full wait, b_full wait, a_full wait, wgmma_wait, flush, wgmma issue, sign test
+    KB2_STALL_END(0, t_role);
+    if ((threadIdx.x & 127) == 0 && blockIdx.x < kStallMaxCtas) {
+        for (int i = 0; i < kStallSlots; i++)
+            g_filter_stalls[blockIdx.x][warp >= 8][(threadIdx.x >> 7) & 1][i] = (unsigned long long)stall[i];
+    }
+#endif
 }
 
 // ---------------------------------------------------------------- plan: (query, probe) pairs grouped by list
