@@ -382,4 +382,51 @@ select_keys_hist_kernel(const float* __restrict__ keys, int64_t ldk, int ncols, 
     for (int i = ctl[2] + threadIdx.x; i < K_cap; i += blockDim.x) out[i] = kEmpty;
 }
 
+// ---------------------------------------------------------------- exact scan of the queries finalize could not certify
+// grid (count, nsplit): CTA (i, s) scans row slice s (multiples of 32 rows) of query qlist[i] with the directly accumulated
+// sum((q-x)^2) / sum(q*x) -- no norm expansion, so nothing cancels -- and writes its best K keys, sorted, to
+// partial[q][s][0..K).  Position = row.  dynamic smem: kScanWarps * 2K entries | query
+template <int METRIC>
+__global__ void __launch_bounds__(kScanThreads)
+flat_exact_scan_kernel(const float* __restrict__ Q, const float* __restrict__ X, int64_t n, int d,
+                       const uint8_t* __restrict__ bitset, int64_t bit_base, const uint32_t* __restrict__ qlist, int K,
+                       uint64_t* __restrict__ partial) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    uint64_t* lists = (uint64_t*)smem_raw;
+    float* s_q = (float*)(lists + kScanWarps * 2 * K);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t q = qlist[blockIdx.x];
+    const int nsplit = gridDim.y, s = blockIdx.y;
+    const int64_t per = ((n + nsplit - 1) / nsplit + 31) / 32 * 32;
+    const int64_t r0 = min(n, (int64_t)s * per), r1 = min(n, r0 + per);
+    for (int j = threadIdx.x; j < d; j += blockDim.x) s_q[j] = Q[q * d + j];
+    WarpTopK tk;
+    tk.init(lists + warp * 2 * K, K, lane);
+    __syncthreads();
+    for (int64_t base = r0 + warp * kWarp; base < r1; base += kScanWarps * kWarp) {
+        const int nrows = (int)min((int64_t)kWarp, r1 - base);
+        float mykey = INFINITY;
+        for (int r = 0; r < nrows; r++) {
+            const float* x = X + (base + r) * d;
+            float acc = 0.f;
+            for (int j = lane; j < d; j += kWarp) {
+                if (METRIC == KB2_METRIC_L2) {
+                    const float t = s_q[j] - x[j];
+                    acc = fmaf(t, t, acc);
+                } else {
+                    acc = fmaf(s_q[j], x[j], acc);
+                }
+            }
+            acc = warp_sum(acc);
+            if (lane == r) mykey = (METRIC == KB2_METRIC_L2) ? acc : -acc;
+        }
+        bool valid = lane < nrows;
+        if (valid && bitset) valid = !bit_is_set(bitset, bit_base + base + lane);
+        tk.push(pack_kp(mykey, (uint32_t)(base + lane)), valid, lane);
+    }
+    uint64_t* out = partial + (q * nsplit + s) * (int64_t)K;
+    tk.finish(lane);
+    block_emit_topk(lists, K, out, K);
+}
+
 }  // namespace kb2

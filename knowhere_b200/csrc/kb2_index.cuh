@@ -33,6 +33,8 @@ init_kernel_attributes() {
         set((const void*)reduce_partials_kernel);
         set((const void*)select_keys_kernel);
         set((const void*)select_keys_hist_kernel);
+        set((const void*)flat_exact_scan_kernel<KB2_METRIC_L2>);
+        set((const void*)flat_exact_scan_kernel<KB2_METRIC_IP>);
         set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, false>);
         set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, true>);
         set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, false>);
@@ -67,7 +69,9 @@ init_kernel_attributes() {
 
 struct Counters {
     int64_t launches = 0, codes = 0, code_bytes = 0, pairs = 0, h2d = 0, d2h = 0;
-    int64_t survivors = 0, flagged = 0;   // tensor-core PQ engine: codes re-evaluated exactly / queries redone by the LUT kernel
+    // tensor-core PQ engine: codes re-evaluated exactly / queries redone by the LUT kernel.  FLAT: flagged = queries whose
+    // re-ranked window was not certified and which were redone by flat_exact_scan_kernel
+    int64_t survivors = 0, flagged = 0;
 };
 
 // grow-by-doubling append of `count` elements (device->device or host->device)
@@ -436,7 +440,13 @@ struct FlatIndex : IndexBase {
         fp.out_ids = d_ids;
         fp.out_dist = d_dist;
         fp.out_pos = nullptr;
+        // certification of the re-ranked window (fin_certify) needs max |x|^2 over the base
+        s_cert.ensure((size_t)nq + 2);
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_cert.p, 0, 8, stream));
+        pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, stream>>>(norms.p, n, s_cert.p);
+        fp.cert = s_cert.p;
         launch_finalize(*this, fp, nq);
+        redo_uncertified(fp, nq, pl.Ksel, dq, n, dbits, shard_world > 1 ? shard_lo : 0);
         last.codes = nq * n;
         last.code_bytes = n * (int64_t)dim * 4;  // list-major contraction reads the base once per batch
         last.pairs = nq;
@@ -446,6 +456,40 @@ struct FlatIndex : IndexBase {
             KB2_CUDA_CHECK(cudaEventElapsedTime(&last_stage_ms, ev0, ev1));
             last_kernel_ms = last_stage_ms;
         }
+    }
+
+    // Queries whose re-ranked window finalize could not certify (data whose norms are large against the distances: the
+    // norm-expanded keys cancel) are searched again with directly accumulated distances, and their rows of the result are
+    // finalized again from those candidates.  On ordinary data the list is empty and this costs one 4-byte copy.
+    DevBuf<uint32_t> s_cert;   // [0] max |x|^2 (float bits), [1] uncertified count, [2..] uncertified queries
+    void
+    redo_uncertified(FinalizeParams fp, int64_t nq, int K, const float* dq, int64_t n, const uint8_t* dbits, int64_t bit_base) {
+        uint32_t* hc = (uint32_t*)h_counter.p;
+        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, s_cert.p + 1, 4, cudaMemcpyDeviceToHost, stream));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
+        const int64_t nredo = hc[0];
+        last.flagged = nredo;
+        if (nredo == 0) return;
+        int nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nredo - 1) / nredo), std::max<int64_t>(1, n / 1024));
+        nsplit = std::min(nsplit, kMaxSortEntries / K);
+        s_partial2.ensure((size_t)nq * nsplit * K);
+        const size_t smem = (size_t)kScanWarps * 2 * K * 8 + (size_t)dim * 4;
+        KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "FLAT: dimension too large for the exact redo scan");
+        const dim3 g((unsigned)nredo, (unsigned)nsplit);
+        if (metric == KB2_METRIC_L2)
+            flat_exact_scan_kernel<KB2_METRIC_L2><<<g, kScanThreads, smem, stream>>>(dq, base.p, n, dim, dbits, bit_base, s_cert.p + 2,
+                                                                                   K, s_partial2.p);
+        else
+            flat_exact_scan_kernel<KB2_METRIC_IP><<<g, kScanThreads, smem, stream>>>(dq, base.p, n, dim, dbits, bit_base, s_cert.p + 2,
+                                                                                   K, s_partial2.p);
+        last.launches++;
+        KB2_CUDA_CHECK(cudaGetLastError());
+        fp.partial = s_partial2.p;
+        fp.partial_stride = (int64_t)nsplit * K;
+        fp.n_partial = nsplit * K;
+        fp.cert = nullptr;
+        fp.qlist = (const int32_t*)(s_cert.p + 2);
+        launch_finalize(*this, fp, nredo);
     }
 
     void
@@ -779,10 +823,10 @@ struct IvfIndex : IndexBase {
         const size_t common_smem = (size_t)kScanWarps * 2 * Ksel * 8 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12 +
                                    (size_t)dim * 4 + 64 + 8 * (2 * kScanWarps + 4) + (size_t)4 * Ksel * 8;   // + CTA bound block + merge buffer
         if (is_pq) {
-            if (G > 0) {
-                const size_t smem = (size_t)G * 65536 + common_smem;
-                KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "IVF_PQ: k too large for shared memory");
-#define KB2_LAUNCH_PQ(GG)                                                                                      \
+            const size_t smem_skewed = (size_t)G * 65536 + common_smem;
+            if (G > 0 && smem_skewed <= (size_t)kMaxDynSmem) {
+                const size_t smem = smem_skewed;
+#define KB2_LAUNCH_PQ(GG)                                                                                     \
     if (metric == KB2_METRIC_L2) {                                                                             \
         if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_L2, true><<<grid, kScanThreads, smem, st>>>(sp);           \
         else ivfpq_scan_kernel<GG, KB2_METRIC_L2, false><<<grid, kScanThreads, smem, st>>>(sp);                \
@@ -793,12 +837,15 @@ struct IvfIndex : IndexBase {
                 if (G == 1) { KB2_LAUNCH_PQ(1) } else if (G == 2) { KB2_LAUNCH_PQ(2) } else { KB2_LAUNCH_PQ(3) }
 #undef KB2_LAUNCH_PQ
             } else {
-                const size_t smem = (size_t)M * 1024 + common_smem;
+                // one M KB table instead of 64 KB per 16 sub-quantizers: any m, and the skewed kernel's fallback at large k
+                // (its 2K-entry candidate buffers) or many probes per CTA, where the replicated tables do not fit beside them
+                const size_t smem = (size_t)M * 1024 + (size_t)kScanWarps * 2 * Ksel * 8 + (size_t)(np_max + 1) * 4 +
+                                    (size_t)np_max * 12 + (size_t)dim * 4;
                 KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "IVF_PQ: m too large for the generic kernel");
                 if (metric == KB2_METRIC_L2)
-                    ivfpq_scan_generic_kernel<KB2_METRIC_L2><<<grid, kScanThreads, smem, st>>>(sp, codes.p);
+                    ivfpq_scan_generic_kernel<KB2_METRIC_L2><<<grid, kScanThreads, smem, st>>>(sp, codes.p, G);
                 else
-                    ivfpq_scan_generic_kernel<KB2_METRIC_IP><<<grid, kScanThreads, smem, st>>>(sp, codes.p);
+                    ivfpq_scan_generic_kernel<KB2_METRIC_IP><<<grid, kScanThreads, smem, st>>>(sp, codes.p, G);
             }
         } else {
             KB2_REQUIRE(dim % 4 == 0, KB2_NOT_IMPLEMENTED, "IVF_FLAT: dim must be a multiple of 4 on the GPU path");

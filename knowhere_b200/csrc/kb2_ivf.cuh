@@ -373,13 +373,15 @@ ivfpq_scan_kernel(IvfScanParams p) {
 }
 
 // =====================================================================================
-// IVF_PQ generic fallback (any M, nbits=8): plain [M][256] table (bank-conflicted), codes stored
-// un-rotated as bytes codes_b[pos*M + m].  Same math, used when M % 16 != 0 or M > 48.
+// IVF_PQ scan with a plain [M][256] table (M KB of shared memory, bank-conflicted gathers), any M, nbits=8.  Same math
+// as ivfpq_scan_kernel in another summation order.  Used when M % 16 != 0 or M > 48 (G == 0: codes stored un-rotated as
+// bytes codes_b[pos*M + m]), and as the fallback of the skewed kernel (G > 0: the rotated groups of p.codes) when its
+// 64 KB per 16 sub-quantizers do not fit beside the candidate buffers of a large k or the probe arrays of many probes.
 // dynamic smem: M*1024 | lists | probes | query
 // =====================================================================================
 template <int METRIC>
-__global__ void __launch_bounds__(kScanThreads)
-ivfpq_scan_generic_kernel(IvfScanParams p, const uint8_t* __restrict__ codes_b) {
+__device__ __forceinline__ void
+ivfpq_scan_generic_body(const IvfScanParams& p, const uint8_t* __restrict__ codes_b, int G, const int64_t bq, const int split) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* lut = (float*)smem_raw;
     uint64_t* lists = (uint64_t*)(smem_raw + (size_t)p.M * 1024);
@@ -392,11 +394,15 @@ ivfpq_scan_generic_kernel(IvfScanParams p, const uint8_t* __restrict__ codes_b) 
     float* s_q = ps.dis0 + np_max;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t q = blockIdx.x / p.nsplit;
-    const int split = blockIdx.x % p.nsplit;
+    const int64_t q = p.qperm ? (int64_t)p.qperm[bq] : bq;
     const int j0 = min(p.nprobe, split * np_max), j1 = min(p.nprobe, j0 + np_max);
     for (int i = threadIdx.x; i < p.d; i += blockDim.x) s_q[i] = p.queries[q * p.d + i];
     const int nchunks = setup_probes(p, q, j0, j1, ps);
+    if (p.counters && threadIdx.x == 0) {
+        unsigned long long tot = 0;
+        for (int j = 0; j < j1 - j0; j++) tot += (unsigned long long)ps.len[j];
+        atomicAdd(p.counters, tot);   // codes scanned by this CTA
+    }
     const float scale = (METRIC == KB2_METRIC_L2) ? -2.f : -1.f;
     for (int e = threadIdx.x; e < p.M * 256; e += blockDim.x) {
         const int m = e >> 8;
@@ -416,16 +422,46 @@ ivfpq_scan_generic_kernel(IvfScanParams p, const uint8_t* __restrict__ codes_b) 
         bool valid = (int)rel < ps.len[cur];
         float acc = 0.f;
         if (valid) {
-            const uint8_t* cb = codes_b + (int64_t)pos * p.M;
             acc = (METRIC == KB2_METRIC_L2) ? p.t1[pos] : 0.f;
-            for (int m = 0; m < p.M; m++) acc += lut[m * 256 + cb[m]];
+            if (G > 0) {
+                // byte s of group g's 16-byte word holds sub-quantizer g*16 + ((s + pos) % 16)
+                for (int g = 0; g < G; g++) {
+                    const uint8_t* cb = (const uint8_t*)(p.codes + (int64_t)g * p.npad + pos);
+                    for (int s = 0; s < 16; s++) acc += lut[(g * 16 + ((s + pos) & 15)) * 256 + cb[s]];
+                }
+            } else {
+                const uint8_t* cb = codes_b + (int64_t)pos * p.M;
+                for (int m = 0; m < p.M; m++) acc += lut[m * 256 + cb[m]];
+            }
             if (p.bitset) valid = !bit_is_set(p.bitset, p.rows[pos]);
         }
         tk.push(pack_kp(ps.dis0[cur] + acc, pos), valid, lane);
     }
-    uint64_t* out = p.partial + ((int64_t)q * p.nsplit + split) * p.kout;
+    uint64_t* out = p.partial_stride ? p.partial + (int64_t)q * p.partial_stride + (int64_t)split * p.kout
+                                     : p.partial + ((int64_t)q * p.nsplit + split) * p.kout;
+    if (split == p.nsplit - 1)   // only the last slice clears the rest of the row
+        for (int i = p.kout + threadIdx.x; i < p.clear_to; i += blockDim.x) out[i] = kEmpty;
     tk.finish(lane);
     block_emit_topk(lists, p.K, out, p.kout);
+}
+
+// codes_b: un-rotated bytes (G == 0) or unused (G > 0: p.codes)
+template <int METRIC>
+__global__ void __launch_bounds__(kScanThreads)
+ivfpq_scan_generic_kernel(IvfScanParams p, const uint8_t* __restrict__ codes_b, int G) {
+    if (p.only_flagged) {
+        // redo pass of the tensor-core engine (see ivfpq_scan_kernel)
+        const int64_t units = (int64_t)(*p.flag_count) * p.nsplit;
+        for (int64_t w = blockIdx.x; w < units; w += gridDim.x) {
+            const int64_t bq = p.flag_list[w / p.nsplit];
+            const int split = (int)(w % p.nsplit);
+            if (threadIdx.x == 0 && split == 0 && p.counters) atomicAdd(p.counters + 3, 1ull);
+            ivfpq_scan_generic_body<METRIC>(p, codes_b, G, bq, split);
+            __syncthreads();
+        }
+        return;
+    }
+    ivfpq_scan_generic_body<METRIC>(p, codes_b, G, (int64_t)(blockIdx.x / p.nsplit), (int)(blockIdx.x % p.nsplit));
 }
 
 // =====================================================================================

@@ -240,7 +240,40 @@ struct FinalizeParams {
     const uint32_t* count_flags;   // ... unless count_flags[q] != 0 (then all n_partial are)
     int split_small;           // > 0: rows with at most this many valid entries were handled by finalize_warp_kernel: skip them
     int64_t row_loop_nq;       // > 0: finalize_kernel strides the rows [0, row_loop_nq) with its grid (0: row = blockIdx.x)
+    uint32_t* cert;            // optional certification of an exact re-rank of norm-expanded keys (FLAT, see fin_certify):
+                               //   [0] bits of max |x|^2 over the base (input); [1] count and [2..] list of the queries
+                               //   whose result is not certified (output; requires rerank)
+    const int32_t* qlist;      // optional: row i of the launch is query qlist[i] (the FLAT redo of uncertified queries)
 };
+
+// Relative error of the approximate FLAT keys |q|^2 + |x|^2 - 2 q.x (L2) and -q.x (IP), as a share of |q|^2 + max|x|^2 (L2)
+// or |q| max|x| (IP): fin_cert_rel(d) = max(3e-5, (d + 8) 2^-22).
+//  * (d + 8) 2^-22 comes from the rounding model of the contraction: every fp32 sum of the dot product and of the norms is
+//    off by at most 2^-23 of the running magnitude, and each 3xTF32 product (hi*hi + hi*lo + lo*hi) by at most 3 * 2^-22 of
+//    |q_i x_i|; summed over d terms and bounded with Cauchy-Schwarz that is below (d + 6) 2^-23 for the dot product, and the
+//    L2 key adds d 2^-24 for the norms and 2^-22 for its two additions -- both then covered by doubling.  The tensor cores'
+//    internal accumulation is not specified to the last bit, so for the 3xTF32 path this is a model, not a proof.
+//  * 3e-5 is the IVF_FLAT tensor-core engine's admission slack (fltc::kSlack); the largest error measured at d = 128 is
+//    5e-6.  It keeps the margin of short contractions, where the model's bound gets small.
+constexpr float kCertSlack = 3e-5f;
+__device__ __forceinline__ float
+fin_cert_rel(int d) {
+    return fmaxf(kCertSlack, (float)(d + 8) * 0x1p-22f);
+}
+
+// A row that the selection did not keep has an approximate key >= `last`, the largest one kept, so its exact key is at least
+// last - err with err = fin_cert_rel(d) * (|q|^2 + max|x|^2) (L2) or fin_cert_rel(d) * |q| max|x| (IP).  The result is
+// certified when its k-th exact key `kth` is at most that; when fewer candidates than k_sel existed (last = +inf) nothing
+// was cut.  Otherwise the query is appended to the redo list.  When the norms are large against the distances (data with a
+// large common offset) the fp32 key cancels and the re-ranked window can miss true neighbours: this is what catches it.
+__device__ __forceinline__ void
+fin_certify(const FinalizeParams& p, int64_t q, float last, float kth, float qq) {
+    if (last == INFINITY || kth == INFINITY) return;
+    const float xx = __uint_as_float(p.cert[0]);
+    const float err = fin_cert_rel(p.d) * ((p.metric == KB2_METRIC_L2) ? qq + xx : sqrtf(qq * xx));
+    if (kth <= last - err) return;
+    p.cert[2 + atomicAdd(p.cert + 1, 1u)] = (uint32_t)q;
+}
 
 // dynamic smem: n_sort*8 + k_sel*(4+8+4) + d*4
 __device__ __forceinline__ void
@@ -284,6 +317,8 @@ finalize_row(FinalizeParams p, const int64_t q) {   // p by value: the variable-
     }
 
     const int ksel = p.k_sel;
+    const uint64_t e_last = (ksel - 1 < p.n_sort) ? s_sort[ksel - 1] : kEmpty;   // largest approximate key kept (fin_certify)
+    const float last = (e_last == kEmpty) ? INFINITY : unpack_key(e_last);
     for (int i = threadIdx.x; i < ksel; i += blockDim.x) {
         uint64_t e = (i < p.n_sort) ? s_sort[i] : kEmpty;
         if (e == kEmpty) {
@@ -411,9 +446,19 @@ finalize_row(FinalizeParams p, const int64_t q) {   // p by value: the variable-
                 p.out_dist[o] = (p.metric == KB2_METRIC_L2) ? ki : -ki;
                 if (p.out_pos) p.out_pos[o] = (int32_t)s_pos[i];
             }
+            if (p.cert && rank == p.k_out - 1) s_q[p.d] = ki;   // k-th exact key (in the spare word after the query)
         }
     }
     // k_out > k_sel cannot happen (host guarantees k_sel >= k_out)
+    if (p.cert) {
+        __syncthreads();
+        if (threadIdx.x < kWarp) {
+            float qq = 0.f;
+            for (int j = threadIdx.x; j < p.d; j += kWarp) qq = fmaf(s_q[j], s_q[j], qq);
+            qq = warp_sum(qq);
+            if (threadIdx.x == 0) fin_certify(p, q, last, s_q[p.d], qq);
+        }
+    }
 }
 
 // grid = nq (one CTA per query), or -- p.row_loop_nq > 0 -- any grid striding the rows: as the tail pass after
@@ -423,11 +468,11 @@ __global__ void __launch_bounds__(256)
 finalize_kernel(FinalizeParams p) {
     if (p.row_loop_nq > 0) {
         for (int64_t q = blockIdx.x; q < p.row_loop_nq; q += gridDim.x) {
-            finalize_row(p, q);
+            finalize_row(p, p.qlist ? (int64_t)p.qlist[q] : q);
             __syncthreads();
         }
     } else {
-        finalize_row(p, (int64_t)blockIdx.x);
+        finalize_row(p, p.qlist ? (int64_t)p.qlist[blockIdx.x] : (int64_t)blockIdx.x);
     }
 }
 
@@ -550,8 +595,9 @@ finalize_warp_kernel(FinalizeParams p, int64_t nq) {
     uint64_t* s_e = (uint64_t*)(s_label + 128);
     float* s_key = (float*)(s_e + 128);
     uint32_t* s_pos = (uint32_t*)(s_key + 128);
-    const int64_t q = (int64_t)blockIdx.x * kFinWarps + warp;
-    if (q >= nq) return;
+    const int64_t row = (int64_t)blockIdx.x * kFinWarps + warp;
+    if (row >= nq) return;
+    const int64_t q = p.qlist ? (int64_t)p.qlist[row] : row;
 
     // ---- 1. approximate order
     int n = p.n_partial;
@@ -565,6 +611,7 @@ finalize_warp_kernel(FinalizeParams p, int64_t nq) {
     else finalize_warp_select<4>(p, src, n, lane, s_pos, s_key, s_label);
     const int ksel = p.k_sel;
     __syncwarp();
+    const float last = p.cert ? s_key[ksel - 1] : INFINITY;   // largest approximate key kept (+inf: none), before the re-rank
 
     // ---- 2. exact keys (same arithmetic and summation order as finalize_kernel)
     if (p.rerank) {
@@ -690,6 +737,7 @@ finalize_warp_kernel(FinalizeParams p, int64_t nq) {
 #pragma unroll
         for (int r = 0; r < 4; r++) f[r] = ((uint64_t)f2ord(g[r].key) << 32) | g[r].pos;
     }
+    float kth = INFINITY;   // k-th exact key (fin_certify), held by lane (k_out - 1) / 4
 #pragma unroll
     for (int r = 0; r < 4; r++) {
         const int i = lane * 4 + r;
@@ -706,8 +754,16 @@ finalize_warp_kernel(FinalizeParams p, int64_t nq) {
                 p.out_ids[o] = s_label[slot];
                 p.out_dist[o] = (p.metric == KB2_METRIC_L2) ? key : -key;
                 if (p.out_pos) p.out_pos[o] = (int32_t)pos;
+                if (i == p.k_out - 1) kth = key;
             }
         }
+    }
+    if (p.cert) {
+        kth = __shfl_sync(0xffffffffu, kth, (p.k_out - 1) >> 2);
+        float qq = 0.f;
+        for (int j = lane; j < p.d; j += kWarp) qq = fmaf(s_q[j], s_q[j], qq);
+        qq = warp_sum(qq);
+        if (lane == 0) fin_certify(p, q, last, kth, qq);
     }
 }
 
