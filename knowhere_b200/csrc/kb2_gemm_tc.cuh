@@ -55,19 +55,28 @@ __device__ __forceinline__ void
 mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void
-mbar_wait(uint32_t bar, uint32_t parity) {
+__device__ __forceinline__ bool
+mbar_try(uint32_t bar, uint32_t parity) {
+    uint32_t ok;
     asm volatile(
         "{\n\t"
         ".reg .pred P1;\n\t"
-        "KB2_WAIT:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra KB2_DONE;\n\t"
-        "bra KB2_WAIT;\n\t"
-        "KB2_DONE:\n\t"
-        "}" ::"r"(bar),
-        "r"(parity)
+        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
+        "selp.b32 %0, 1, 0, P1;\n\t"
+        "}"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
         : "memory");
+    return ok != 0;
+}
+// bounded wait (~3 s of SM clocks): a protocol bug must end the launch with an error, never hang the GPU
+__device__ __forceinline__ void
+mbar_wait(uint32_t bar, uint32_t parity) {
+    if (mbar_try(bar, parity)) return;
+    const long long t0 = clock64();
+    while (!mbar_try(bar, parity)) {
+        if (clock64() - t0 > 6000000000ll) __trap();
+    }
 }
 __device__ __forceinline__ void
 tma_load_2d(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar) {

@@ -900,24 +900,60 @@ struct IvfIndex : IndexBase {
         if (ev_join) cudaEventDestroy(ev_join);
         if (side_stream) cudaStreamDestroy(side_stream);
     }
-    // sort the items by descending cost (the persistent kernels draw them in this order); returns the new item arrays
-    int32_t*
-    balance_items(int32_t* items, int64_t max_items, int tile_cost, int col_cost, cudaStream_t st = nullptr) {
-        if (!st) st = stream;
+    // ---- the list-major pipeline (kb2_listmajor.cuh) of both tensor-core engines
+    struct ItemTable {
+        const int32_t *list, *q0, *nq;   // [*n_items] in descending estimated cost
+        const int32_t* n_items;
+        int32_t* ticket;                 // zeroed: the persistent kernel draws the items through it
+    };
+    // Plan on stream ps: the (query, probe) pairs grouped by list (-> s_pair_q, s_pair_base), cut into items of <= item_cap
+    // queries (a multiple of 16) and sorted by the estimated cost tiles x (tile_cost + col_cost x columns).
+    ItemTable
+    plan_items(const int64_t* probe_ids, const float* probe_dis, int64_t nq, int nprobe, int item_cap, int tile_cost, int col_cost,
+               cudaStream_t ps) {
+        const int64_t npairs = nq * nprobe;
+        const int64_t max_items = nlist + npairs / item_cap + 2;
+        s_lcount.ensure((size_t)2 * nlist);
+        s_lstart.ensure((size_t)nlist);
+        s_items.ensure((size_t)3 * max_items);
         s_items2.ensure((size_t)3 * max_items);
         s_bal_key.ensure((size_t)max_items); s_bal_key2.ensure((size_t)max_items);
         s_bal_idx.ensure((size_t)max_items); s_bal_idx2.ensure((size_t)max_items);
-        pqtc::item_cost_kernel<<<grid1d(max_items, 256), 256, 0, st>>>(s_plan_out.p, items, items + 2 * max_items, list_len.p, max_items,
+        s_plan_out.ensure(8);
+        s_pair_q.ensure((size_t)npairs);
+        s_pair_base.ensure((size_t)npairs);
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_lcount.p, 0, (size_t)2 * nlist * 4, ps));
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_plan_out.p + 4, 0, 4, ps));
+        lm::count_pairs_kernel<<<grid1d(npairs, 256), 256, 0, ps>>>(probe_ids, npairs, list_len.p, s_lcount.p);
+        int32_t* items = s_items.p;   // list | q0 | nq
+        lm::plan_kernel<<<1, 1024, 0, ps>>>(s_lcount.p, (int)nlist, item_cap, s_lstart.p, items, items + max_items,
+                                            items + 2 * max_items, s_plan_out.p);
+        lm::item_cost_kernel<<<grid1d(max_items, 256), 256, 0, ps>>>(s_plan_out.p, items, items + 2 * max_items, list_len.p, max_items,
                                                                      tile_cost, col_cost, s_bal_key.p, s_bal_idx.p);
         size_t tmp_bytes = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, s_bal_key.p, s_bal_key2.p, s_bal_idx.p, s_bal_idx2.p, (int)max_items, 0, 16, st);
+        cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, s_bal_key.p, s_bal_key2.p, s_bal_idx.p, s_bal_idx2.p, (int)max_items, 0, 16, ps);
         s_sort_tmp.ensure(tmp_bytes);
-        cub::DeviceRadixSort::SortPairs(s_sort_tmp.p, tmp_bytes, s_bal_key.p, s_bal_key2.p, s_bal_idx.p, s_bal_idx2.p, (int)max_items, 0, 16, st);
-        pqtc::deal_items_kernel<<<grid1d(max_items, 256), 256, 0, st>>>(s_plan_out.p, s_bal_idx2.p, items, items + max_items,
+        cub::DeviceRadixSort::SortPairs(s_sort_tmp.p, tmp_bytes, s_bal_key.p, s_bal_key2.p, s_bal_idx.p, s_bal_idx2.p, (int)max_items, 0, 16, ps);
+        lm::deal_items_kernel<<<grid1d(max_items, 256), 256, 0, ps>>>(s_plan_out.p, s_bal_idx2.p, items, items + max_items,
                                                                       items + 2 * max_items, s_items2.p, s_items2.p + max_items,
                                                                       s_items2.p + 2 * max_items);
-        last.launches += 4;
-        return s_items2.p;
+        lm::fill_pairs_kernel<<<grid1d(npairs, 256), 256, 0, ps>>>(probe_ids, probe_dis, npairs, nprobe, metric, list_len.p, s_lstart.p,
+                                                                   s_lcount.p + nlist, s_pair_q.p, s_pair_base.p);
+        last.launches += 7;
+        return {s_items2.p, s_items2.p + max_items, s_items2.p + 2 * max_items, s_plan_out.p, s_plan_out.p + 4};
+    }
+    // n_logs survivor logs of cap entries each; the counts and the overflow word cnt[n_logs] are zeroed on the handle's stream
+    struct SurvivorLogs {
+        uint4* log;
+        uint32_t* cnt;
+        uint32_t cap;
+    };
+    SurvivorLogs
+    alloc_logs(int n_logs, uint32_t cap) {
+        s_log.ensure((size_t)n_logs * cap);
+        s_logcnt.ensure((size_t)n_logs + 1);
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, ((size_t)n_logs + 1) * 4, stream));
+        return {s_log.p, s_logcnt.p, cap};
     }
 
     bool
@@ -962,7 +998,6 @@ struct IvfIndex : IndexBase {
             tc_rowmax = 0.5f * h[M] * 1.0001f;   // max |t1| / 2: the largest row term of the admission test
             tc_ready = true;
         }
-        const int64_t npairs = nq * nprobe;
         // development aid: KB2_TC_VERBOSE=1 prints the device time of every stage of this engine
         const bool verbose = getenv("KB2_TC_VERBOSE") != nullptr;
         std::vector<std::pair<const char*, cudaEvent_t>> marks;
@@ -1035,35 +1070,14 @@ struct IvfIndex : IndexBase {
         }
         if (dist) comm->all_reduce_min_f32(s_bound.p, s_bound.p, (size_t)nq, st);
         mark("phaseA");
-        // ---- plan: pairs grouped by list, work items
-        const int64_t max_items = nlist + npairs / pqtc::NQT + 2;
-        s_lcount.ensure((size_t)2 * nlist);
-        s_lstart.ensure((size_t)nlist);
-        s_items.ensure((size_t)3 * max_items);
-        s_plan_out.ensure(8);
-        s_pair_q.ensure((size_t)npairs);
-        s_pair_base.ensure((size_t)npairs);
+        // ---- plan: pairs grouped by list, work items of <= 256 queries.  Per tile: decode ~ constant, contraction ~ columns
+        //      (+ the test K-step)
+        const ItemTable items = plan_items(sp.probe_ids, sp.probe_dis, nq, nprobe, pqtc::NQT, 600, 5, ps);
         s_qb16.ensure((size_t)nq * dim);
         s_qnorm.ensure((size_t)nq);
         s_cand.ensure((size_t)nq * kTcCandCap);
         s_cand_cnt.ensure((size_t)2 * nq);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_lcount.p, 0, (size_t)2 * nlist * 4, ps));
         KB2_CUDA_CHECK(cudaMemsetAsync(s_cand_cnt.p, 0, (size_t)2 * nq * 4, ps));
-        pqtc::count_pairs_kernel<<<grid1d(npairs, 256), 256, 0, ps>>>(sp.probe_ids, npairs, list_len.p, s_lcount.p);
-        int32_t* item_list = s_items.p;
-        int32_t* item_q0 = s_items.p + max_items;
-        int32_t* item_nq = s_items.p + 2 * max_items;
-        pqtc::plan_kernel<<<1, 1024, 0, ps>>>(s_lcount.p, (int)nlist, s_lstart.p, item_list, item_q0, item_nq, s_plan_out.p);
-        {
-            // per tile: decode ~ constant, contraction ~ columns (+ the test K-step)
-            // items in descending cost order, CTAs take the next one when free
-            int32_t* bal = balance_items(s_items.p, max_items, 600, 5, ps);
-            item_list = bal;
-            item_q0 = bal + max_items;
-            item_nq = bal + 2 * max_items;
-        }
-        pqtc::fill_pairs_kernel<<<grid1d(npairs, 256), 256, 0, ps>>>(sp.probe_ids, sp.probe_dis, npairs, nprobe, metric, list_len.p,
-                                                                     s_lstart.p, s_lcount.p + nlist, s_pair_q.p, s_pair_base.p);
         pqtc::prepare_queries_kernel<<<grid1d(nq * 32, 256), 256, 0, ps>>>(sp.queries, nq, dim, (__nv_bfloat16*)s_qb16.p, s_qnorm.p);
         if (ov) {
             KB2_CUDA_CHECK(cudaGetLastError());
@@ -1080,12 +1094,11 @@ struct IvfIndex : IndexBase {
         tp.queries = sp.queries;
         tp.qb16 = (const __nv_bfloat16*)s_qb16.p;
         tp.qnorm = s_qnorm.p;
-        tp.n_items = s_plan_out.p;
-        tp.ticket = s_plan_out.p + 4;
-        KB2_CUDA_CHECK(cudaMemsetAsync(tp.ticket, 0, 4, st));
-        tp.item_list = item_list;
-        tp.item_q0 = item_q0;
-        tp.item_nq = item_nq;
+        tp.n_items = items.n_items;
+        tp.ticket = items.ticket;
+        tp.item_list = items.list;
+        tp.item_q0 = items.q0;
+        tp.item_nq = items.nq;
         tp.pair_q = s_pair_q.p;
         tp.pair_base = s_pair_base.p;
         tp.bound = s_bound.p;
@@ -1103,13 +1116,10 @@ struct IvfIndex : IndexBase {
         tp.bitset = sp.bitset;
         tp.rows = rows.p;
         const int n_logs = 2 * num_sms();   // one per epilogue group
-        const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(nq * 1024 / n_logs, 16384), 1 << 19);
-        s_log.ensure((size_t)n_logs * log_cap);
-        s_logcnt.ensure(n_logs + 8);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (n_logs + 8) * 4, st));
-        tp.log = s_log.p;
-        tp.log_cnt = s_logcnt.p;
-        tp.log_cap = log_cap;
+        const SurvivorLogs logs = alloc_logs(n_logs, (uint32_t)std::clamp<int64_t>(nq * 1024 / n_logs, 16384, 1 << 19));
+        tp.log = logs.log;
+        tp.log_cnt = logs.cnt;
+        tp.log_cap = logs.cap;
         tp.qflag = s_cand_cnt.p + nq;
         tp.counters = d_counter.p;
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
@@ -1127,13 +1137,13 @@ struct IvfIndex : IndexBase {
 #endif
         mark("tc_filter");
         // ---- survivors: group by query, exact fp32 keys (bit-identical to the LUT engine's)
-        pqtc::scatter_survivors_kernel<<<dim3(16, n_logs), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p,
-                                                                     kTcCandCap, tp.qflag, d_counter.p);
+        lm::scatter_survivors_kernel<<<dim3(16, n_logs), 256, 0, st>>>(logs.log, logs.cnt, logs.cap, s_cand.p, s_cand_cnt.p, kTcCandCap,
+                                                                       tp.qflag, d_counter.p);
         // exact_eval trims every survivor row to its k_base best.  Measured at C3: step 1.977 -> 1.957 ms
 #define KB2_TC_EVAL(MM, GG, DD)                                                                                                      \
     pqtc::exact_eval_kernel<MM, GG, DD><<<(unsigned)nq, 128, 0, st>>>(sp.queries, pqc.p, eval_lut, s_bound.p, (const uint4*)codes.p, npad, t1.p,  \
                                                                       sp.bitset, rows.p, s_cand.p, s_cand_cnt.p, kTcCandCap, tp.qflag,  \
-                                                                      s_logcnt.p + n_logs + 1, k_base);
+                                                                      logs.cnt + n_logs, k_base);
         const float* eval_lut = (tc_geom_18() && !dist) ? s_lut.p : nullptr;   // tables of the whole batch exist only without a communicator
         if (tc_geom_18()) {
             if (metric == KB2_METRIC_L2) { KB2_TC_EVAL(KB2_METRIC_L2, 1, 8) } else { KB2_TC_EVAL(KB2_METRIC_IP, 1, 8) }
@@ -1142,7 +1152,7 @@ struct IvfIndex : IndexBase {
         }
 #undef KB2_TC_EVAL
         KB2_CUDA_CHECK(cudaGetLastError());
-        last.launches += 7;
+        last.launches += 4;
         mark("scatter+eval");
         // ---- flagged queries (no bound / buffer overflow): complete LUT scan into their candidate rows
         {
@@ -1219,34 +1229,14 @@ struct IvfIndex : IndexBase {
             if (distributed()) comm->all_reduce_min_f32(s_bound.p, s_bound.p, (size_t)nq, st);
             last.launches += 1;
         }
-        // ---- plan: pairs grouped by list, items of <= 128 queries
-        const int64_t max_items = nlist + npairs / item_cap + 2;
-        s_lcount.ensure((size_t)2 * nlist);
-        s_lstart.ensure((size_t)nlist);
-        s_items.ensure((size_t)3 * max_items);
-        s_plan_out.ensure(8);
-        s_pair_q.ensure((size_t)npairs);
-        s_pair_base.ensure((size_t)npairs);
+        // ---- plan: pairs grouped by list, items of <= item_cap queries (a tile is bound by its HBM stream)
+        const ItemTable items = plan_items(sp.probe_ids, sp.probe_dis, nq, nprobe, item_cap, 1000, 2, st);
         s_qnorm.ensure((size_t)nq);
         s_cand.ensure((size_t)nq * kTcCandCap);
         s_cand_cnt.ensure((size_t)2 * nq + 4);
         s_qhi.ensure((size_t)npairs_pad * dim);
         s_qlo.ensure((size_t)npairs_pad * dim);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_lcount.p, 0, (size_t)2 * nlist * 4, st));
         KB2_CUDA_CHECK(cudaMemsetAsync(s_cand_cnt.p, 0, ((size_t)2 * nq + 4) * 4, st));
-        pqtc::count_pairs_kernel<<<grid1d(npairs, 256), 256, 0, st>>>(sp.probe_ids, npairs, list_len.p, s_lcount.p);
-        int32_t* item_list = s_items.p;
-        int32_t* item_q0 = s_items.p + max_items;
-        int32_t* item_nq = s_items.p + 2 * max_items;
-        fltc::plan_kernel<<<1, 1024, 0, st>>>(s_lcount.p, (int)nlist, item_cap, s_lstart.p, item_list, item_q0, item_nq, s_plan_out.p);
-        {
-            int32_t* bal = balance_items(s_items.p, max_items, 1000, 2);   // a tile is bound by its HBM stream
-            item_list = bal;
-            item_q0 = bal + max_items;
-            item_nq = bal + 2 * max_items;
-        }
-        pqtc::fill_pairs_kernel<<<grid1d(npairs, 256), 256, 0, st>>>(sp.probe_ids, sp.probe_dis, npairs, nprobe, metric, list_len.p,
-                                                                     s_lstart.p, s_lcount.p + nlist, s_pair_q.p, s_pair_base.p);
         // pairs of lists owned by other shards leave holes at the end of the pair array: point them at no query
         fltc::gather_split_queries_kernel<<<grid1d(npairs_pad * 32, 256), 256, 0, st>>>(sp.queries, s_pair_q.p, npairs, npairs_pad, dim,
                                                                                      s_qhi.p, s_qlo.p);
@@ -1258,12 +1248,11 @@ struct IvfIndex : IndexBase {
         fltc::Params fpar{};
         fpar.metric = metric;
         fpar.d = dim;
-        fpar.n_items = s_plan_out.p;
-        fpar.ticket = s_plan_out.p + 4;
-        KB2_CUDA_CHECK(cudaMemsetAsync(fpar.ticket, 0, 4, st));
-        fpar.item_list = item_list;
-        fpar.item_q0 = item_q0;
-        fpar.item_nq = item_nq;
+        fpar.n_items = items.n_items;
+        fpar.ticket = items.ticket;
+        fpar.item_list = items.list;
+        fpar.item_q0 = items.q0;
+        fpar.item_nq = items.nq;
         fpar.pair_q = s_pair_q.p;
         fpar.qnorm2 = s_qnorm.p;
         fpar.bound = s_bound.p;
@@ -1272,13 +1261,11 @@ struct IvfIndex : IndexBase {
         fpar.xnorm2 = vnorm2.p;
         fpar.bitset = sp.bitset;
         fpar.rows = rows.p;
-        const uint32_t log_cap = (uint32_t)std::min<int64_t>(std::max<int64_t>(nq * 1024 / num_sms(), 32768), 1 << 20);
-        s_log.ensure((size_t)num_sms() * log_cap);
-        s_logcnt.ensure(num_sms() + 8);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_logcnt.p, 0, (num_sms() + 8) * 4, st));
-        fpar.log = s_log.p;
-        fpar.log_cnt = s_logcnt.p;
-        fpar.log_cap = log_cap;
+        const int n_logs = num_sms();   // one per CTA
+        const SurvivorLogs logs = alloc_logs(n_logs, (uint32_t)std::clamp<int64_t>(nq * 1024 / n_logs, 32768, 1 << 20));
+        fpar.log = logs.log;
+        fpar.log_cnt = logs.cnt;
+        fpar.log_cap = logs.cap;
         fpar.counters = d_counter.p;
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
 #define KB2_FL_LAUNCH(MM, BR) \
@@ -1292,9 +1279,10 @@ struct IvfIndex : IndexBase {
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev3, st));
         KB2_CUDA_CHECK(cudaGetLastError());
         uint32_t* qflag = s_cand_cnt.p + nq;
-        fltc::scatter_kernel<<<dim3(16, num_sms()), 256, 0, st>>>(s_log.p, s_logcnt.p, log_cap, s_cand.p, s_cand_cnt.p, kTcCandCap, qflag);
-        fltc::count_flags_kernel<<<grid1d(nq, 256), 256, 0, st>>>(qflag, nq, s_logcnt.p + num_sms(), s_cand_cnt.p + 2 * nq);
-        last.launches += 9;
+        lm::scatter_survivors_kernel<<<dim3(16, n_logs), 256, 0, st>>>(logs.log, logs.cnt, logs.cap, s_cand.p, s_cand_cnt.p, kTcCandCap,
+                                                                       qflag, nullptr);
+        fltc::count_flags_kernel<<<grid1d(nq, 256), 256, 0, st>>>(qflag, nq, logs.cnt + n_logs, s_cand_cnt.p + 2 * nq);
+        last.launches += 6;
         uint32_t* hflag = (uint32_t*)h_counter.p + 12;
         KB2_CUDA_CHECK(cudaMemcpyAsync(hflag, s_cand_cnt.p + 2 * nq, 4, cudaMemcpyDeviceToHost, st));
         KB2_CUDA_CHECK(cudaStreamSynchronize(st));

@@ -5,7 +5,7 @@
 // each probed list once per (query, list) pair — C2: 16.0 MB per query.
 //
 // Here the query x list distance is what it is, a dense contraction: the (query, probe) pairs are grouped by list
-// (same plan as the IVF_PQ engine), and every list is read ONCE per batch — a [128 rows] x [N queries of the list] x d
+// (the list-major plan of kb2_listmajor.cuh), and every list is read ONCE per batch — a [128 rows] x [N queries of the list] x d
 // tile product on the Hopper tensor cores (wgmma) with the operands brought by TMA.
 //   * A operand: 128 consecutive rows of the list, fp32, straight from the list-order vector store (TMA, 128-byte swizzle).
 //   * B operand: the item's queries, gathered pair-major beforehand and already split hi/lo (two TMA tiles).
@@ -17,21 +17,25 @@
 //     key of the query's nearest probed lists, from the query-major kernel, + a 3e-5 relative slack for the tf32 split)
 //     are logged as survivors; finalize_kernel re-ranks the k+16 best of them EXACTLY from the fp32 rows, so the result
 //     is the exact scan's (same guarantee as FLAT).
-// Work item = (list, <=128 of the queries probing it).  One persistent CTA per SM, 288 threads:
+// Work item = (list, <= 32 or <= 128 of the queries probing it), drawn in descending-cost order from the ticket counter;
+// survivors go to one log per CTA {query, position, f2ord(key), 0} and lm::scatter_survivors_kernel copies them into the
+// per-query candidate rows as packed (key, position) entries.  One persistent CTA per SM, 288 threads:
 //   warps 0-7 two consumer warpgroups (rows 0-63 | 64-127 of a tile: split, wgmma, epilogue) | warp 8 TMA producer.
 #pragma once
 #include "kb2_gemm_tc.cuh"
-#include "kb2_ivfpq_tc.cuh"
+#include "kb2_listmajor.cuh"
 
 namespace kb2 {
 namespace fltc {
 
-constexpr int TM = 128;         // list rows per tile (two wgmma M=64 halves)
+using lm::TM;                   // list rows per tile
 constexpr int NQ_ITEM = 128;    // most queries per item
 constexpr int BK = 32;          // floats per k-block (one 128-byte swizzle row)
 constexpr int TILE_BYTES = 128 * BK * 4;        // 16 KB: 128 rows of one k-block
 constexpr int THREADS = 288;
 constexpr int PRODUCER_WARP = 8;
+// item sequence of a CTA, shared by the two roles (< 16 items apart: the producer leads by at most STAGES k-blocks)
+using ItemRing = lm::ItemRing<32>;
 // BROWS = query rows per item the instance is built for (its B tiles are BROWS x 128 B): 32 -> 40 KB stages, 5 in flight
 // (few queries per list: C2 has ~31); 128 -> 64 KB stages, 3 in flight.  The kernel is bound by the latency of the
 // TMA -> convert -> MMA -> release chain of a stage, so the number of stages in flight sets the HBM rate it reaches.
@@ -42,7 +46,7 @@ struct FlCfg {
     static constexpr int STAGES = BROWS <= 32 ? 5 : 3;
     static constexpr int OFF_META = STAGES * STAGE_BYTES;                     // thr[128] | base[128] | qidx[128]
     static constexpr int OFF_BAR = OFF_META + 3 * NQ_ITEM * 4;
-    static constexpr size_t SMEM_BYTES = OFF_BAR + 256 + 384 /*item ring*/ + 1024 /*alignment slack*/;
+    static constexpr size_t SMEM_BYTES = OFF_BAR + 256 + ItemRing::BYTES + 1024 /*alignment slack*/;
     static_assert(SMEM_BYTES <= 227 * 1024, "IVF_FLAT tensor-core kernel shared memory");
 };
 constexpr float kSlack = 3e-5f;   // 3xTF32 contraction error, relative to |q|^2 + |x|^2 (measured 5e-6, tests/test_gemm_tc_gpu.py)
@@ -50,7 +54,7 @@ constexpr float kSlack = 3e-5f;   // 3xTF32 contraction error, relative to |q|^2
 struct Params {
     int metric, d;
     const int32_t* n_items;
-    int32_t* ticket;              // work counter (see pqtc::Params::ticket)
+    int32_t* ticket;              // work counter (zeroed before the launch)
     const int32_t* item_list;
     const int32_t* item_q0;       // first pair of the item
     const int32_t* item_nq;
@@ -62,7 +66,7 @@ struct Params {
     const float* xnorm2;          // [npad] |x|^2 per position
     const uint8_t* bitset;
     const int32_t* rows;
-    uint4* log;                   // [gridDim.x][log_cap] survivors {query, position, key bits, 0}
+    uint4* log;                   // [gridDim.x][log_cap] survivors {query, position, f2ord(key), 0}
     uint32_t* log_cnt;            // [gridDim.x] entries; [gridDim.x] = 1 when a log overflowed
     uint32_t log_cap;
     unsigned long long* counters; // [0] rows scanned (pairs x rows)
@@ -91,46 +95,6 @@ extract_bound_kernel(const uint64_t* __restrict__ partial, int64_t stride, int k
     if (q >= nq) return;
     const uint64_t e = partial[q * stride + k - 1];
     bound[q] = (e == kEmpty) ? INFINITY : unpack_key(e);
-}
-
-// plan for 128-query items (the IVF_PQ engine's plan kernel cuts at 256)
-__global__ void __launch_bounds__(1024)
-plan_kernel(const int32_t* __restrict__ lcount, int nlist, int item_cap, int32_t* __restrict__ lstart, int32_t* __restrict__ item_list,
-            int32_t* __restrict__ item_q0, int32_t* __restrict__ item_nq, int32_t* __restrict__ n_items) {
-    typedef cub::BlockScan<int, 1024> Scan;
-    __shared__ typename Scan::TempStorage tmp_a, tmp_b;
-    __shared__ int carry_a, carry_b;
-    if (threadIdx.x == 0) carry_a = carry_b = 0;
-    __syncthreads();
-    for (int b0 = 0; b0 < nlist; b0 += 1024) {
-        const int l = b0 + threadIdx.x;
-        const int c = l < nlist ? lcount[l] : 0;
-        const int nch = (c + item_cap - 1) / item_cap;
-        int ex_a, ex_b, tot_a, tot_b;
-        Scan(tmp_a).ExclusiveSum(c, ex_a, tot_a);
-        Scan(tmp_b).ExclusiveSum(nch, ex_b, tot_b);
-        const int ca = carry_a, cb = carry_b;
-        if (l < nlist) {
-            lstart[l] = ca + ex_a;
-            if (nch > 0) {
-                int per = ((c + nch - 1) / nch + 15) & ~15;
-                if ((nch - 1) * per >= c || per > item_cap) per = item_cap;
-                for (int ch = 0; ch < nch; ch++) {
-                    const int i = cb + ex_b + ch;
-                    item_list[i] = l;
-                    item_q0[i] = ca + ex_a + ch * per;
-                    item_nq[i] = max(0, min(per, c - ch * per));
-                }
-            }
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            carry_a = ca + tot_a;
-            carry_b = cb + tot_b;
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *n_items = carry_b;
 }
 
 template <int BROWS>
@@ -162,36 +126,8 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     const int n_items = *p.n_items;
     const int nkb = p.d / BK;
 
-    // item sequence of this CTA, drawn from a global counter and shared by the two roles (same scheme as the IVF_PQ filter
-    // kernel; the roles are < 16 items apart: the producer leads by at most STAGES k-blocks)
-    constexpr int SCHED_R = 32;
-    int* sch_claim = (int*)(sm + OFF_BAR + 256);
-    int* sch_item = sch_claim + SCHED_R;
-    volatile int* sch_ready = (volatile int*)(sch_item + SCHED_R);
-    if (threadIdx.x < SCHED_R) {
-        sch_claim[threadIdx.x] = (int)threadIdx.x - SCHED_R;
-        sch_ready[threadIdx.x] = -1;
-    }
-    auto item_at_thread = [&](int seq) -> int {
-        const int sl = seq & (SCHED_R - 1);
-        if (sch_ready[sl] != seq) {
-            if (atomicCAS(sch_claim + sl, seq - SCHED_R, seq) == seq - SCHED_R) {
-                const int t = atomicAdd(p.ticket, 1);
-                ((volatile int*)sch_item)[sl] = t;
-                __threadfence_block();
-                sch_ready[sl] = seq;
-            } else {
-                while (sch_ready[sl] != seq) {}
-            }
-        }
-        __threadfence_block();
-        return ((volatile int*)sch_item)[sl];
-    };
-    auto item_at = [&](int seq) -> int {   // warp-uniform call
-        int v = 0;
-        if (lane == 0) v = item_at_thread(seq);
-        return __shfl_sync(0xffffffffu, v, 0);
-    };
+    const ItemRing ring(sm + OFF_BAR + 256, p.ticket);
+    ring.init();
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; s++) {
@@ -208,7 +144,7 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         if (lane == 0) {
             uint32_t it = 0;
             int seq = 0;
-            for (int item = item_at_thread(0); item < n_items; item = item_at_thread(++seq)) {
+            for (int item = ring.at_thread(0); item < n_items; item = ring.at_thread(++seq)) {
                 const int l = p.item_list[item];
                 const int q0 = p.item_q0[item];
                 const int64_t off = p.list_off[l];
@@ -216,7 +152,7 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                 for (int t = 0; t < ntiles; t++) {
                     for (int kb = 0; kb < nkb; kb++, it++) {
                         const int s = it % STAGES;
-                        pqtc::mbar_wait_g(bar_empty(s), ((it / STAGES) & 1u) ^ 1u);
+                        tc::mbar_wait(bar_empty(s), ((it / STAGES) & 1u) ^ 1u);
                         const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
                         tc::mbar_expect_tx(bar_full(s), TILE_BYTES + 2 * B_TILE_BYTES);
                         tc::tma_load_2d(st, &tmap_x, kb * BK, (int)(off + (int64_t)t * TM), bar_full(s));
@@ -243,7 +179,7 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     for (int i = 0; i < BROWS / 2; i++) acc[i] = 0.f;
     uint32_t it = 0;
     int seq = 0;
-    for (int item = item_at(0); item < n_items; item = item_at(++seq)) {
+    for (int item = ring.at_warp(0); item < n_items; item = ring.at_warp(++seq)) {
         const int l = p.item_list[item];
         const int q0 = p.item_q0[item];
         const int nqi = p.item_nq[item];
@@ -271,7 +207,7 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
             int pending = -1;   // stage whose wgmmas may still be in flight
             for (int kb = 0; kb < nkb; kb++, it++) {
                 const int s = it % STAGES;
-                pqtc::mbar_wait_g(bar_full(s), (it / STAGES) & 1u);
+                tc::mbar_wait(bar_full(s), (it / STAGES) & 1u);
                 // split this warpgroup's 64 rows of the raw A tile into hi (in place) and lo
                 float4* hi = reinterpret_cast<float4*>(sm + (size_t)s * STAGE_BYTES + wg * (TILE_BYTES / 2));
                 float4* lo = reinterpret_cast<float4*>(sm + (size_t)s * STAGE_BYTES + TILE_BYTES + wg * (TILE_BYTES / 2));
@@ -361,7 +297,7 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                                     uint4 o;
                                     o.x = (uint32_t)m_q[col];
                                     o.y = (uint32_t)(off + rel);
-                                    o.z = __float_as_uint(key);
+                                    o.z = f2ord(key);
                                     o.w = 0u;
                                     my_log[slot] = o;
                                 } else {
@@ -383,19 +319,6 @@ ivfflat_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     }
 }
 
-// survivors of all CTA logs -> per-query candidate rows as packed (key, position)   (grid = (x, number of logs))
-__global__ void
-scatter_kernel(const uint4* __restrict__ log, const uint32_t* __restrict__ log_cnt, uint32_t log_cap, uint64_t* __restrict__ cand,
-               uint32_t* __restrict__ cand_cnt, int cap, uint32_t* __restrict__ qflag) {
-    const uint32_t n = min(log_cnt[blockIdx.y], log_cap);
-    const uint4* src = log + (size_t)blockIdx.y * log_cap;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint4 e = src[i];
-        const uint32_t slot = atomicAdd(cand_cnt + e.x, 1u);
-        if (slot < (uint32_t)cap) cand[(int64_t)e.x * cap + slot] = pack_kp(__uint_as_float(e.z), e.y);
-        else qflag[e.x] = 1u;
-    }
-}
 // number of flagged queries (or every query when a log overflowed) -> *out
 __global__ void
 count_flags_kernel(const uint32_t* __restrict__ qflag, int64_t nq, const uint32_t* __restrict__ log_over, uint32_t* __restrict__ out) {

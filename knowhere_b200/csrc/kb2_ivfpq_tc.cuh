@@ -33,24 +33,23 @@
 //                         while the next block is in flight.  Once the tile is in registers the hits are expanded -> one
 //                         shared-memory slot reservation per warp and half tile -> the group's private survivor log in global
 //                         memory (plain stores, nothing on the critical path waits for a global round trip).
-//   Items are drawn from a global ticket counter in descending-cost order (DESIGN.md 4.5).
-// Then: scatter_survivors_kernel groups the log by query, exact_eval_kernel recomputes the survivors' keys in fp32.
-// Work item = (list, chunk of <= 256 of the queries probing it); items are laid out by a single-CTA plan kernel
-// from the coarse result (count -> scan -> fill).
+// Work item = (list, chunk of <= 256 of the queries probing it).  The plan, the cost-ordered ticket scheduling and the
+// survivor logs are the list-major pipeline of kb2_listmajor.cuh (DESIGN.md 4.5); the log entries carry the key base's
+// bits.  Then lm::scatter_survivors_kernel groups the logs by query, exact_eval_kernel recomputes the survivors' keys in fp32.
 #pragma once
 #include <cuda_bf16.h>
 
-#include <cub/block/block_scan.cuh>
 #include <type_traits>
 #include <utility>
 
 #include "kb2_gemm_tc.cuh"
 #include "kb2_ivf.cuh"
+#include "kb2_listmajor.cuh"
 
 namespace kb2 {
 namespace pqtc {
 
-constexpr int TM = 128;        // codes per tile (two wgmma M=64 halves)
+using lm::TM;                  // codes per tile
 constexpr int NQT = 256;       // queries per item
 constexpr int THREADS = 512;          // warps 0-7 decoders (2 groups), 8-15 consumers (2 warpgroups)
 constexpr int GROUP_THREADS = 128;
@@ -114,8 +113,7 @@ struct Params {
     // output
     uint4* log;                    // [2*gridDim.x][log_cap] survivors {query, position, key base bits, 0}: one log per
                                    // epilogue group
-    uint32_t* log_cnt;             // [2*gridDim.x] entries per log; [2G] unused;
-                                   // [2G + 1] = 1 when any log overflowed; [2G + 2..3] diagnostics
+    uint32_t* log_cnt;             // [2*gridDim.x] entries per log; [2*gridDim.x] = 1 when any log overflowed
     uint32_t log_cap;              // entries per log
     uint32_t* qflag;               // [nq] 1: redo this query with the LUT kernel
     unsigned long long* counters;  // [0] codes scanned (pairs x codes), [2] survivors re-evaluated, [3] flagged
@@ -141,29 +139,6 @@ for_each_block_count(int n, F&& f) {
     });
 }
 
-__device__ __forceinline__ bool
-mbar_try(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, P1;\n\t"
-        "}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// bounded wait: a protocol bug must end the launch with an error, never hang the GPU
-__device__ __forceinline__ void
-mbar_wait_g(uint32_t bar, uint32_t parity) {
-    if (mbar_try(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try(bar, parity)) {
-        if (clock64() - t0 > 6000000000ll) __trap();
-    }
-}
 __device__ __forceinline__ void
 bar_sync_epi() {
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -243,36 +218,9 @@ ivfpq_tc_filter_kernel(Params p) {
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // role index, provably warp-uniform
     const int n_items = *p.n_items;
 
-    // ---- item sequence of this CTA.  The three roles walk the same sequence independently (at most ~3 items apart), so the
-    // seq-th draw is published through a small ring in shared memory: whoever needs it first claims the slot, takes a ticket
-    // from the global counter and publishes it; the others read it.
-    constexpr int SCHED_R = 8;
-    int* sch_claim = (int*)(sm + OFF_BAR + 144);
-    int* sch_item = sch_claim + SCHED_R;
-    volatile int* sch_ready = (volatile int*)(sch_item + SCHED_R);
-    if (threadIdx.x < SCHED_R) {
-        sch_claim[threadIdx.x] = (int)threadIdx.x - SCHED_R;
-        sch_ready[threadIdx.x] = -1;
-    }
-    auto item_at = [&](int seq) -> int {   // warp-uniform call
-        int v = 0;
-        if (lane == 0) {
-            const int sl = seq & (SCHED_R - 1);
-            if (sch_ready[sl] != seq) {
-                if (atomicCAS(sch_claim + sl, seq - SCHED_R, seq) == seq - SCHED_R) {
-                    const int t = atomicAdd(p.ticket, 1);
-                    ((volatile int*)sch_item)[sl] = t;
-                    __threadfence_block();
-                    sch_ready[sl] = seq;
-                } else {
-                    while (sch_ready[sl] != seq) {}
-                }
-            }
-            __threadfence_block();
-            v = ((volatile int*)sch_item)[sl];
-        }
-        return __shfl_sync(0xffffffffu, v, 0);
-    };
+    // item sequence of this CTA, shared by the three roles (at most ~3 items apart)
+    const lm::ItemRing<8> ring(sm + OFF_BAR + 144, p.ticket);
+    ring.init();
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < 2; i++) {
@@ -309,7 +257,7 @@ ivfpq_tc_filter_kernel(Params p) {
         auto write_meta = [&](int item, int it) {
             KB2_STALL_BEGIN(t_meta);
             const int par = it & 1;
-            mbar_wait_g(bar_meta_free(par), (((uint32_t)it >> 1) & 1u) ^ 1u);
+            tc::mbar_wait(bar_meta_free(par), (((uint32_t)it >> 1) & 1u) ^ 1u);
             const int q0 = p.item_q0[item];
             const int nqi = p.item_nq[item];
             float* m_h = (float*)(sm + OFF_META + par * META_BYTES);
@@ -341,10 +289,10 @@ ivfpq_tc_filter_kernel(Params p) {
         };
         uint32_t g0 = 0;   // global tile counter at the start of the item
         int it = 0;
-        int item = item_at(0);
+        int item = ring.at_warp(0);
         if (item < n_items) write_meta(item, 0);
         for (; item < n_items; it++) {
-            const int item_next = item_at(it + 1);
+            const int item_next = ring.at_warp(it + 1);
             const int l = p.item_list[item];
             const int nqi = p.item_nq[item];
             const int nmma = (nqi + 15) & ~15;
@@ -384,7 +332,7 @@ ivfpq_tc_filter_kernel(Params p) {
                 uint32_t rh, rm, rl;
                 split3_bf16(-r, rh, rm, rl);
                 KB2_STALL_BEGIN(t_ae);
-                mbar_wait_g(bar_a_empty(dg), ((g >> 1) & 1u) ^ 1u);
+                tc::mbar_wait(bar_a_empty(dg), ((g >> 1) & 1u) ^ 1u);
                 KB2_STALL_END(1, t_ae);
                 unsigned char* A = sm + OFF_A + dg * A_BYTES + (tid >> 3) * GRP_BYTES + (tid & 7) * 16;
                 if constexpr (DSUB == 8) {
@@ -448,7 +396,7 @@ ivfpq_tc_filter_kernel(Params p) {
             KB2_STALL_BEGIN(t_b);
             asm volatile("bar.sync 2, 256;" ::: "memory");          // meta[par] (thresholds, query indices) written by all decoders
             KB2_STALL_BEGIN(t_bf);
-            mbar_wait_g(bar_b_free, ((uint32_t)it & 1u) ^ 1u);
+            tc::mbar_wait(bar_b_free, ((uint32_t)it & 1u) ^ 1u);
             KB2_STALL_END(2, t_bf);
             {
                 const float* m_h = (const float*)(sm + OFF_META + par * META_BYTES);
@@ -507,7 +455,7 @@ ivfpq_tc_filter_kernel(Params p) {
         float va[32], vb[32];
 #pragma unroll
         for (int i = 0; i < 32; i++) va[i] = vb[i] = 0.f;
-        for (int item = item_at(0); item < n_items; item = item_at(++it)) {
+        for (int item = ring.at_warp(0); item < n_items; item = ring.at_warp(++it)) {
             const int l = p.item_list[item];
             const int nqi = p.item_nq[item];
             const int nmma = (nqi + 15) & ~15;
@@ -519,14 +467,14 @@ ivfpq_tc_filter_kernel(Params p) {
             const int ntiles = (len + TM - 1) / TM;
             const int par = it & 1;
             KB2_STALL_BEGIN(t_mf);
-            mbar_wait_g(bar_meta_full(par), ((uint32_t)it >> 1) & 1u);
+            tc::mbar_wait(bar_meta_full(par), ((uint32_t)it >> 1) & 1u);
             KB2_STALL_END(1, t_mf);
             const float* m_base = (const float*)(sm + OFF_META + par * META_BYTES) + NQT;
             const int* m_q = (const int*)(m_base + NQT);
             if (et == 0) n_codes += (unsigned long long)len * (unsigned long long)nqi;
             const int t_first = (int)((eg - (int)(g0 & 1u)) & 1);
             KB2_STALL_BEGIN(t_bfull);
-            mbar_wait_g(bar_b_full, (uint32_t)it & 1u);
+            tc::mbar_wait(bar_b_full, (uint32_t)it & 1u);
             KB2_STALL_END(2, t_bfull);
             const uint32_t a0 = base + OFF_A + eg * A_BYTES;
             const uint32_t b0 = base + OFF_B;
@@ -535,7 +483,7 @@ ivfpq_tc_filter_kernel(Params p) {
             for (int t = t_first; t < ntiles; t += 2) {
                 const uint32_t g = g0 + (uint32_t)t;   // g & 1 == eg
                 KB2_STALL_BEGIN(t_af);
-                mbar_wait_g(bar_a_full(eg), (g >> 1) & 1u);
+                tc::mbar_wait(bar_a_full(eg), (g >> 1) & 1u);
                 KB2_STALL_END(3, t_af);
                 auto issue = [&](float (&acc)[32], int h, int c) {
                     KB2_STALL_BEGIN(t_is);
@@ -656,7 +604,7 @@ ivfpq_tc_filter_kernel(Params p) {
             tc::mbar_arrive(bar_meta_free(par));
             g0 += (uint32_t)ntiles;
         }
-        if (log_over) p.log_cnt[n_logs + 1] = 1u;
+        if (log_over) p.log_cnt[n_logs] = 1u;
         if (eg == 0) asm volatile("bar.sync 3, 128;" ::: "memory"); else asm volatile("bar.sync 4, 128;" ::: "memory");
         if (e == 0) {
             const uint32_t n = min(*my_cursor, p.log_cap);
@@ -675,102 +623,6 @@ ivfpq_tc_filter_kernel(Params p) {
             g_filter_stalls[blockIdx.x][warp >= 8][(threadIdx.x >> 7) & 1][i] = (unsigned long long)stall[i];
     }
 #endif
-}
-
-// ---------------------------------------------------------------- plan: (query, probe) pairs grouped by list
-__global__ void
-count_pairs_kernel(const int64_t* __restrict__ probe_ids, int64_t npairs, const int32_t* __restrict__ list_len,
-                   int32_t* __restrict__ lcount) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= npairs) return;
-    const int64_t l = probe_ids[i];
-    if (l >= 0 && list_len[l] > 0) atomicAdd(lcount + l, 1);
-}
-
-// one CTA: exclusive scans over the lists -> first pair of each list, item table (list, query chunk)
-__global__ void __launch_bounds__(1024)
-plan_kernel(const int32_t* __restrict__ lcount, int nlist, int32_t* __restrict__ lstart, int32_t* __restrict__ item_list,
-            int32_t* __restrict__ item_q0, int32_t* __restrict__ item_nq, int32_t* __restrict__ n_items) {
-    typedef cub::BlockScan<int, 1024> Scan;
-    __shared__ typename Scan::TempStorage tmp_a, tmp_b;
-    __shared__ int carry_a, carry_b;
-    if (threadIdx.x == 0) carry_a = carry_b = 0;
-    __syncthreads();
-    for (int b0 = 0; b0 < nlist; b0 += 1024) {
-        const int l = b0 + threadIdx.x;
-        const int c = l < nlist ? lcount[l] : 0;
-        const int nch = (c + NQT - 1) / NQT;
-        int ex_a, ex_b, tot_a, tot_b;
-        Scan(tmp_a).ExclusiveSum(c, ex_a, tot_a);
-        Scan(tmp_b).ExclusiveSum(nch, ex_b, tot_b);
-        const int ca = carry_a, cb = carry_b;
-        if (l < nlist) {
-            lstart[l] = ca + ex_a;
-            if (nch > 0) {
-                // even chunks, multiples of 16 queries (the UMMA N granularity); full chunks when rounding would leave the
-                // last one empty (an item without queries would be an N = 0 MMA)
-                int per = ((c + nch - 1) / nch + 15) & ~15;
-                if ((nch - 1) * per >= c) per = NQT;
-                for (int ch = 0; ch < nch; ch++) {
-                    const int i = cb + ex_b + ch;
-                    item_list[i] = l;
-                    item_q0[i] = ca + ex_a + ch * per;
-                    item_nq[i] = max(0, min(per, c - ch * per));
-                }
-            }
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            carry_a = ca + tot_a;
-            carry_b = cb + tot_b;
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *n_items = carry_b;
-}
-
-// ---- load balancing of the persistent kernels.  Item costs have a heavy tail (list length x queries per list), and the
-// launch lasts as long as its slowest CTA.  Items are therefore sorted by descending cost estimate and drawn in that order
-// through Params::ticket (longest processing time first): a CTA that got short items simply draws more.
-__global__ void
-item_cost_kernel(const int32_t* __restrict__ n_items, const int32_t* __restrict__ item_list, const int32_t* __restrict__ item_nq,
-                 const int32_t* __restrict__ list_len, int64_t max_items, int tile_cost, int col_cost, uint32_t* __restrict__ key,
-                 int32_t* __restrict__ idx) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= max_items) return;
-    uint32_t k = 0xffffu;   // unused slots sort to the end; 16-bit keys = two radix passes
-    if (i < *n_items) {
-        const long long tiles = (list_len[item_list[i]] + TM - 1) / TM;
-        const long long c = (tiles * (tile_cost + (long long)col_cost * ((item_nq[i] + 15) & ~15))) >> 5;
-        k = 0xfffeu - (uint32_t)min(c, 0xfff0ll);   // ascending key = descending cost
-    }
-    key[i] = k;
-    idx[i] = (int32_t)i;
-}
-__global__ void
-deal_items_kernel(const int32_t* __restrict__ n_items, const int32_t* __restrict__ sorted_idx, const int32_t* __restrict__ in_list,
-                  const int32_t* __restrict__ in_q0, const int32_t* __restrict__ in_nq, int32_t* __restrict__ out_list,
-                  int32_t* __restrict__ out_q0, int32_t* __restrict__ out_nq) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;   // rank by descending cost
-    if (j >= *n_items) return;
-    const int src = sorted_idx[j];
-    out_list[j] = in_list[src];
-    out_q0[j] = in_q0[src];
-    out_nq[j] = in_nq[src];
-}
-
-__global__ void
-fill_pairs_kernel(const int64_t* __restrict__ probe_ids, const float* __restrict__ probe_dis, int64_t npairs, int nprobe,
-                  int metric, const int32_t* __restrict__ list_len, const int32_t* __restrict__ lstart,
-                  int32_t* __restrict__ lcursor, int32_t* __restrict__ pair_q, float* __restrict__ pair_base) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= npairs) return;
-    const int64_t l = probe_ids[i];
-    if (l < 0 || list_len[l] <= 0) return;
-    const int slot = lstart[l] + atomicAdd(lcursor + l, 1);
-    pair_q[slot] = (int32_t)(i / nprobe);
-    const float dv = probe_dis[i];
-    pair_base[slot] = (metric == KB2_METRIC_L2) ? dv : -dv;
 }
 
 // bf16 copy + norm of the queries (warp per query, d % 4 == 0)
@@ -824,24 +676,6 @@ unrotate_codes_kernel(const uint8_t* __restrict__ rot, int64_t total_words /* G 
     const int64_t word = t >> 4;
     const int64_t pos = word % npad;
     plain[word * 16 + ((s + (int)(pos & 15)) & 15)] = rot[t];
-}
-
-// survivors of all CTA logs -> per-query rows (thread per log entry; grid = (x, number of logs))
-__global__ void
-scatter_survivors_kernel(const uint4* __restrict__ log, const uint32_t* __restrict__ log_cnt, uint32_t log_cap,
-                         uint64_t* __restrict__ cand, uint32_t* __restrict__ cand_cnt, int cap, uint32_t* __restrict__ qflag,
-                         unsigned long long* __restrict__ counters) {
-    const uint32_t n = min(log_cnt[blockIdx.y], log_cap);
-    const uint4* src = log + (size_t)blockIdx.y * log_cap;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint4 e = src[i];
-        const uint32_t slot = atomicAdd(cand_cnt + e.x, 1u);
-        if (slot < (uint32_t)cap) cand[(int64_t)e.x * cap + slot] = ((uint64_t)e.z << 32) | e.y;   // (key base bits, position)
-        else {
-            qflag[e.x] = 1u;
-            if (counters) atomicAdd(counters + 6, 1ull);
-        }
-    }
 }
 
 // Per-query ADC tables for the whole batch:  lut[q][j*16 + m] = scale * <q_m, c_pq[m][j]>  (scale -2 for L2, -1 for IP),
