@@ -150,19 +150,55 @@ wgmma_tf32_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumu
         : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
+// D (+)= A * B with bf16 operands, A = 64 rows, B = N = 16 .. 128 rows (multiple of 16); D in the first N / 2 registers
+// of d, in the fragment layout of wgmma_tf32_n128
+#define KB2_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define KB2_ACC8 KB2_D8(0)
+#define KB2_ACC16 KB2_ACC8, KB2_D8(8)
+#define KB2_ACC24 KB2_ACC16, KB2_D8(16)
+#define KB2_ACC32 KB2_ACC24, KB2_D8(24)
+#define KB2_ACC40 KB2_ACC32, KB2_D8(32)
+#define KB2_ACC48 KB2_ACC40, KB2_D8(40)
+#define KB2_ACC56 KB2_ACC48, KB2_D8(48)
+#define KB2_ACC64 KB2_ACC56, KB2_D8(56)
+template <int N, int R>
 __device__ __forceinline__ void
-wgmma_bf16_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t"
-        "}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
-        : "memory");
+wgmma_bf16(float (&d)[R], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    static_assert(N % 16 == 0 && N >= 16 && N <= 128 && N / 2 <= R, "wgmma_bf16: N = 16 .. 128 in steps of 16");
+    if constexpr (N == 16) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC8 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 32) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC16 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 48) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC24 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 64) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC32 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 80) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC40 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 96) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC48 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 112) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55}, %56, %57, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC56 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+    else if constexpr (N == 128) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : KB2_ACC64 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
 }
+#undef KB2_ACC8
+#undef KB2_ACC16
+#undef KB2_ACC24
+#undef KB2_ACC32
+#undef KB2_ACC40
+#undef KB2_ACC48
+#undef KB2_ACC56
+#undef KB2_ACC64
+#undef KB2_D8
 // round-to-nearest into the 19-bit tf32 container (low 13 mantissa bits cleared)
 __device__ __forceinline__ float
 tf32_rn(float x) {

@@ -27,7 +27,8 @@
 //                         the B operand (bf16 queries of the item, gathered by index, + [1, 1, 1, h_hi, h_mid, h_lo, 0, 0])
 //                         and the per-column meta data, one item ahead.
 //   warps 8-15 consumers: two warpgroups, warpgroup e owns the tiles g % 2 == e (A buffer e).  A tile is contracted in
-//                         blocks of 64 codes x 64 queries (K/16 + 1 x wgmma m64n64k16 bf16 into 32 registers per thread), the
+//                         blocks of 64 codes x at most MAXW queries, each exactly as wide as its share of the item's columns
+//                         (K/16 + 1 x wgmma m64nNk16 bf16 into N / 2 registers per thread), the
 //                         next block of the tile (of either 64-code half) is issued before the current one is tested; the accumulator
 //                         holds D = S' + h - r, so "survives" is a clear sign bit, collected branch-free into per-row masks
 //                         while the next block is in flight.  Once the tile is in registers the hits are expanded -> one
@@ -53,6 +54,10 @@ using lm::TM;                  // codes per tile
 constexpr int NQT = 256;       // queries per item
 constexpr int THREADS = 512;          // warps 0-7 decoders (2 groups), 8-15 consumers (2 warpgroups)
 constexpr int GROUP_THREADS = 128;
+// widest wgmma block of the consumers (columns).  Two blocks are in flight per warpgroup, and ptxas (CUDA 12.9) fits their
+// accumulators under the kernel's 128-register cap only up to this width: wider blocks make it serialize the wgmmas
+// (C7511 / C7512), and raising the consumers' budget with setmaxnreg does not change that.
+constexpr int MAXW = 80;
 constexpr int META_BYTES = 3 * NQT * 4;   // h | base | qidx
 // geometry of one engine instance: G groups of 16 sub-quantizers of DSUB dimensions (K = 16 G DSUB).
 // Instances: <1, 8> (m = 16, d = 128: BASELINE C3) and <3, 2> (m = 48, d = 96: BASELINE C5).
@@ -130,13 +135,22 @@ __device__ __forceinline__ void
 static_for(F&& f) {
     static_for_impl(f, std::make_integer_sequence<int, N>{});
 }
-// f(std::integral_constant<int, n>{}) for the run-time block count n = 1 .. NQT / 64 (warp-uniform)
-template <typename F>
+// columns C0 .. C0 + W - 1 of an item, contracted in one wgmma block
+template <int C0_, int W_>
+struct BlockCols {
+    static constexpr int C0 = C0_, W = W_;
+};
+// f(std::integral_constant<int, n>{}) for the run-time value n = LO .. HI (warp-uniform), by binary search
+template <int LO, int HI, typename F>
 __device__ __forceinline__ void
-for_each_block_count(int n, F&& f) {
-    static_for<NQT / 64>([&](auto i) {
-        if (n == decltype(i)::value + 1) f(std::integral_constant<int, decltype(i)::value + 1>{});
-    });
+dispatch_range(int n, F&& f) {
+    if constexpr (LO == HI) {
+        f(std::integral_constant<int, LO>{});
+    } else {
+        constexpr int MID = (LO + HI) / 2;
+        if (n <= MID) dispatch_range<LO, MID>(n, f);
+        else dispatch_range<MID + 1, HI>(n, f);
+    }
 }
 
 __device__ __forceinline__ void
@@ -331,28 +345,22 @@ ivfpq_tc_filter_kernel(Params p) {
                 if (t * TM + tid < len) r = (METRIC == KB2_METRIC_L2) ? 0.5f * tv : 0.f;
                 uint32_t rh, rm, rl;
                 split3_bf16(-r, rh, rm, rl);
-                KB2_STALL_BEGIN(t_ae);
-                tc::mbar_wait(bar_a_empty(dg), ((g >> 1) & 1u) ^ 1u);
-                KB2_STALL_END(1, t_ae);
-                unsigned char* A = sm + OFF_A + dg * A_BYTES + (tid >> 3) * GRP_BYTES + (tid & 7) * 16;
+                // The chunks of the row are gathered from the codebook into registers BEFORE the A buffer is free: after
+                // the consumers hand it back only the stores remain between them and the next tile.
+                uint4 v[XCHUNK];
                 if constexpr (DSUB == 8) {
                     // chunk = one sub-quantizer (8 bf16): 16 gathers per group through the rotated code bytes.  The table is
                     // laid out [code value][sub-quantizer] (16 B entries): the 8 lanes of a quarter-warp hold 8 consecutive
                     // sub-quantizers, i.e. 8 different 16-byte bank groups whatever their code values => every LDS.128 is
                     // conflict-free (a [sub-quantizer][code value] table costs ~3x the wavefronts with random codes).
+                    // v[16 gg + s] is sub-quantizer 16 gg + (s + pos) % 16, pos % 16 == tid % 16.
 #pragma unroll
                     for (int gg = 0; gg < G; gg++) {
                         const uint32_t ww[4] = {w[gg].x, w[gg].y, w[gg].z, w[gg].w};
 #pragma unroll
-                        for (int h0 = 0; h0 < 16; h0 += 8) {     // 8 gathers in flight, then 8 stores
-                            uint4 v[8];
-#pragma unroll
-                            for (int s = 0; s < 8; s++) {
-                                const uint32_t byte = (ww[(h0 + s) >> 2] >> (8 * ((h0 + s) & 3))) & 255u;
-                                v[s] = tab[byte * (16 * G) + gg * 16 + ((h0 + s + tid) & 15)];   // pos % 16 == tid % 16
-                            }
-#pragma unroll
-                            for (int s = 0; s < 8; s++) *reinterpret_cast<uint4*>(A + (gg * 16 + ((h0 + s + tid) & 15)) * 128) = v[s];
+                        for (int s = 0; s < 16; s++) {
+                            const uint32_t byte = (ww[s >> 2] >> (8 * (s & 3))) & 255u;
+                            v[gg * 16 + s] = tab[byte * (16 * G) + gg * 16 + ((s + tid) & 15)];
                         }
                     }
                 } else {
@@ -361,25 +369,29 @@ ivfpq_tc_filter_kernel(Params p) {
                     constexpr int WPS = DSUB / 2;              // 32-bit words per sub-quantizer entry
                     const uint32_t* tab32 = reinterpret_cast<const uint32_t*>(tab);
 #pragma unroll
-                    for (int c0 = 0; c0 < XCHUNK; c0 += 4) {   // 4 chunks (16 words) in flight
-                        uint32_t v[4][4];
+                    for (int c = 0; c < XCHUNK; c++) {
+                        uint32_t u[4];
 #pragma unroll
-                        for (int cc = 0; cc < 4; cc++) {
+                        for (int j = 0; j < SPC; j++) {
+                            const int m = c * SPC + j;
+                            const uint4 wg = w[m >> 4];
+                            const int b = m & 15;
+                            const uint32_t word = (b < 4) ? wg.x : (b < 8) ? wg.y : (b < 12) ? wg.z : wg.w;
+                            const uint32_t byte = (word >> (8 * (b & 3))) & 255u;
 #pragma unroll
-                            for (int j = 0; j < SPC; j++) {
-                                const int m = (c0 + cc) * SPC + j;
-                                const uint4 wg = w[m >> 4];
-                                const int b = m & 15;
-                                const uint32_t word = (b < 4) ? wg.x : (b < 8) ? wg.y : (b < 12) ? wg.z : wg.w;
-                                const uint32_t byte = (word >> (8 * (b & 3))) & 255u;
-#pragma unroll
-                                for (int x = 0; x < WPS; x++) v[cc][j * WPS + x] = tab32[(m * 256 + byte) * WPS + x];
-                            }
+                            for (int x = 0; x < WPS; x++) u[j * WPS + x] = tab32[(m * 256 + byte) * WPS + x];
                         }
-#pragma unroll
-                        for (int cc = 0; cc < 4; cc++)
-                            *reinterpret_cast<uint4*>(A + (c0 + cc) * 128) = make_uint4(v[cc][0], v[cc][1], v[cc][2], v[cc][3]);
+                        v[c] = make_uint4(u[0], u[1], u[2], u[3]);
                     }
+                }
+                KB2_STALL_BEGIN(t_ae);
+                tc::mbar_wait(bar_a_empty(dg), ((g >> 1) & 1u) ^ 1u);
+                KB2_STALL_END(1, t_ae);
+                unsigned char* A = sm + OFF_A + dg * A_BYTES + (tid >> 3) * GRP_BYTES + (tid & 7) * 16;
+#pragma unroll
+                for (int c = 0; c < XCHUNK; c++) {
+                    const int chunk = (DSUB == 8) ? (c & ~15) + ((c + tid) & 15) : c;
+                    *reinterpret_cast<uint4*>(A + chunk * 128) = v[c];
                 }
                 // test chunk: [-r_hi, -r_mid, -r_lo, 1, 1, 1, 0, 0] (bf16 1.0 = 0x3F80); then a zero chunk
                 *reinterpret_cast<uint4*>(A + XCHUNK * 128) = make_uint4(rh | (rm << 16), rl | (0x3F80u << 16), 0x3F803F80u, 0u);
@@ -438,9 +450,9 @@ ivfpq_tc_filter_kernel(Params p) {
     } else {
         // =========================== consumers: two warpgroups, warpgroup e owns A buffer e (tiles g % 2 == e) ==========
         // The accumulator holds D = S' + h_col - r_row: a (code, query) pair survives iff D >= 0, i.e. iff its sign bit is
-        // clear.  "No survivor in this 64 x 64 block" is an AND over the thread's 32 words (LOP3 tree); survivors are rare
-        // (~0.1 %), so the exact mask is built only on a hit and the entries go straight to the group's survivor log in global
-        // memory (slot range reserved with one shared-memory atomic per warp and half tile; plain stores, nothing waits for them).
+        // clear.  The sign bits are packed into per-row masks while the next block is in flight; survivors are rare
+        // (~0.1 %), and go straight to the group's survivor log in global memory (slot range reserved with one
+        // shared-memory atomic per thread with survivors and tile; plain stores, nothing waits for them).
         const int et = threadIdx.x - 256;        // 0..255
         const int eg = et >> 7;                  // group
         const int e = et & 127;                  // thread inside the group
@@ -452,16 +464,12 @@ ivfpq_tc_filter_kernel(Params p) {
         unsigned long long n_codes = 0;
         uint32_t g0 = 0;
         int it = 0;
-        float va[32], vb[32];
-#pragma unroll
-        for (int i = 0; i < 32; i++) va[i] = vb[i] = 0.f;
         for (int item = ring.at_warp(0); item < n_items; item = ring.at_warp(++it)) {
             const int l = p.item_list[item];
             const int nqi = p.item_nq[item];
-            const int nmma = (nqi + 15) & ~15;
-            const int nblk = __shfl_sync(0xffffffffu, (nmma + 63) >> 6, 0);   // 64-query blocks; columns >= nmma of the last one are masked.
-            // The broadcast makes the block-count dispatch provably warp-uniform: with a bound ptxas must treat as divergent it
-            // serializes the wgmmas (C7518).
+            // wgmma columns of the item, in 16-column units (1 .. NQT / 16).  The broadcast makes the width dispatch provably
+            // warp-uniform: with a bound ptxas must treat as divergent it serializes the wgmmas (C7518).
+            const int ncls = __shfl_sync(0xffffffffu, (nqi + 15) >> 4, 0);
             const int len = p.list_len[l];
             const int64_t off = p.list_off[l];
             const int ntiles = (len + TM - 1) / TM;
@@ -485,98 +493,114 @@ ivfpq_tc_filter_kernel(Params p) {
                 KB2_STALL_BEGIN(t_af);
                 tc::mbar_wait(bar_a_full(eg), (g >> 1) & 1u);
                 KB2_STALL_END(3, t_af);
-                auto issue = [&](float (&acc)[32], int h, int c) {
+                // one block: the 64 codes of half h against the blk::W columns from column blk::C0, into the first W / 2
+                // registers of acc
+                auto issue = [&](auto& acc, int h, auto blk) {
+                    using B = decltype(blk);
                     KB2_STALL_BEGIN(t_is);
                     // the operand descriptors of the wgmmas differ only in the start-address field (address >> 4) of the
                     // low word.  Every shared-memory address of the CTA lies below 2^18, so that 14-bit field never carries
                     // and an offset of x bytes is a 32-bit add of x / 16: one add per descriptor instead of rebuilding it.
-                    const uint32_t la = la0 + (uint32_t)(h * 8 * GRP_BYTES / 16), lb = lb0 + (uint32_t)(c * 8 * GRP_BYTES / 16);
+                    uint32_t la = la0 + (uint32_t)(h * 8 * GRP_BYTES / 16), lb = lb0 + (uint32_t)(B::C0 / 8 * GRP_BYTES / 16);
+                    // <1, 8>: computed here, not hoisted out of the tile loop, where the compiler would keep every K-step's
+                    // descriptors in registers that the accumulators need (ptxas then serializes the wgmmas, C7511).  The
+                    // <3, 2> geometry is the other way round: it serializes with this barrier and not without.
+                    if constexpr (G == 1) asm volatile("" : "+r"(la), "+r"(lb));
                     tc::fence_operand(acc);
                     tc::wgmma_fence();
 #pragma unroll
                     for (int ks = 0; ks < KSTEPS; ks++)
-                        tc::wgmma_bf16_n64(acc, desc_hi | (la + ks * 16u), desc_hi | (lb + ks * 16u), ks > 0 ? 1u : 0u);
+                        tc::wgmma_bf16<B::W>(acc, desc_hi | (la + ks * 16u), desc_hi | (lb + ks * 16u), ks > 0 ? 1u : 0u);
                     tc::wgmma_commit();
                     tc::fence_operand(acc);
                     KB2_STALL_END(6, t_is);
                 };
-                // sign test of one block -> bits (c * 16 + 2 j + cc) of the masks of the thread's two rows of half h.  Branch-free:
-                // it runs between the issue and the wait of the next block, where divergent code would make ptxas serialize
-                // the wgmmas.
+                // sign test of one block -> bits C0 / 4 + 2 j + cc of the masks of the thread's two rows of half h (column
+                // C0 + 8 j + 2 (lane % 4) + cc).  Every column of the block lies below the item's wgmma width, and the
+                // columns past its queries fail through h = -inf, so no column mask is needed.  Branch-free: it runs between
+                // the issue and the wait of the next block, where divergent code would make ptxas serialize the wgmmas.
                 uint64_t mh[2][2] = {{0ull, 0ull}, {0ull, 0ull}};
-                auto test = [&](const float (&v)[32], int h, int c) {
+                auto test = [&](const auto& v, int h, auto blk) {
+                    using B = decltype(blk);
+                    constexpr int NBIT = B::W / 4, HALF = NBIT / 2;   // bits per row, per chain
                     KB2_STALL_BEGIN(t_te);
-                    // column 8 j + cc of the block is valid iff 8 j + cc < lim; lim is even, so iff j < ceil(lim / 8)
-                    const int lim = nmma - c * 64 - 2 * (lane & 3);
-                    const uint32_t valid = (1u << (2 * min(8, max(0, (lim + 7) >> 3)))) - 1u;
                     // sign bit of column 8 j + cc (i = 2 j + cc) of the thread's first / second row -> bit i of n0 / n1.  A
                     // funnel shift (n << 1) | (x >> 31) appends one sign bit in one instruction; columns go in from the
-                    // highest i down, in two chains per row (i < 8, i >= 8) for instruction-level parallelism.
+                    // highest i down, in two chains per row (i < HALF, i >= HALF) for instruction-level parallelism.
                     uint32_t n0l = 0u, n0h = 0u, n1l = 0u, n1h = 0u;
 #pragma unroll
-                    for (int i = 7; i >= 0; i--) {
+                    for (int i = HALF - 1; i >= 0; i--) {
                         const int x = 4 * (i >> 1) + (i & 1);   // register of column i of the first row; + 2: second row
+                        const int xh = 4 * ((i + HALF) >> 1) + ((i + HALF) & 1);
                         n0l = __funnelshift_l(__float_as_uint(v[x]), n0l, 1);
-                        n0h = __funnelshift_l(__float_as_uint(v[x + 16]), n0h, 1);
+                        n0h = __funnelshift_l(__float_as_uint(v[xh]), n0h, 1);
                         n1l = __funnelshift_l(__float_as_uint(v[x + 2]), n1l, 1);
-                        n1h = __funnelshift_l(__float_as_uint(v[x + 18]), n1h, 1);
+                        n1h = __funnelshift_l(__float_as_uint(v[xh + 2]), n1h, 1);
                     }
                     // a pair survives iff its sign bit is clear
-                    const uint32_t m0 = ~((n0h << 8) | n0l), m1 = ~((n1h << 8) | n1l);
-                    mh[h][0] |= (uint64_t)(m0 & valid) << (c * 16);   // h and c are compile-time indices (unrolled pipeline)
-                    mh[h][1] |= (uint64_t)(m1 & valid) << (c * 16);
+                    constexpr uint32_t mask = (1u << NBIT) - 1u;
+                    const uint32_t m0 = ~((n0h << HALF) | n0l) & mask, m1 = ~((n1h << HALF) | n1l) & mask;
+                    mh[h][0] |= (uint64_t)m0 << (B::C0 / 4);   // h and C0 are compile-time (unrolled pipeline)
+                    mh[h][1] |= (uint64_t)m1 << (B::C0 / 4);
                     KB2_STALL_END(7, t_te);
                 };
-                // survivors of the thread's two rows of half h -> the group's log
-                auto flush = [&](int h) {
-                    const uint32_t total = (uint32_t)(__popcll(mh[h][0]) + __popcll(mh[h][1]));
-                    if (__any_sync(0xffffffffu, total != 0u)) {
-                        uint32_t incl = total;
+                // survivors of the thread's four rows of the tile -> the group's log.  Survivors are rare (a few per warp and
+                // tile), so each thread that has any reserves its own slot range with one shared-memory atomic.
+                auto flush = [&]() {
+                    const uint32_t total =
+                        (uint32_t)(__popcll(mh[0][0]) + __popcll(mh[0][1]) + __popcll(mh[1][0]) + __popcll(mh[1][1]));
+                    if (total != 0u) {
+                        uint32_t slot = atomicAdd(my_cursor, total);
 #pragma unroll
-                        for (int o = 1; o < 32; o <<= 1) {
-                            const uint32_t tv = __shfl_up_sync(0xffffffffu, incl, o);
-                            if (lane >= o) incl += tv;
-                        }
-                        uint32_t wbase = 0;
-                        if (lane == 31) wbase = atomicAdd(my_cursor, incl);
-                        wbase = __shfl_sync(0xffffffffu, wbase, 31);
-                        uint32_t slot = wbase + incl - total;
+                        for (int h = 0; h < 2; h++) {
 #pragma unroll
-                        for (int i = 0; i < 2; i++) {
-                            const int rel = t * TM + h * 64 + we * 16 + (lane >> 2) + 8 * i;
-                            uint64_t m = mh[h][i];
-                            while (m) {
-                                const int bit = __ffsll((long long)m) - 1;
-                                m &= m - 1;
-                                const int col = (bit >> 4) * 64 + 8 * ((bit & 15) >> 1) + 2 * (lane & 3) + (bit & 1);
-                                if (slot < p.log_cap) {
-                                    uint4 o;
-                                    o.x = (uint32_t)m_q[col];
-                                    o.y = (uint32_t)(off + rel);
-                                    o.z = __float_as_uint(m_base[col]);
-                                    o.w = 0u;
-                                    my_log[slot] = o;
-                                } else {
-                                    log_over = true;
+                            for (int i = 0; i < 2; i++) {
+                                const int rel = t * TM + h * 64 + we * 16 + (lane >> 2) + 8 * i;
+                                uint64_t m = mh[h][i];
+                                while (m) {
+                                    const int bit = __ffsll((long long)m) - 1;
+                                    m &= m - 1;
+                                    const int col = 8 * (bit >> 1) + 2 * (lane & 3) + (bit & 1);
+                                    if (slot < p.log_cap) {
+                                        uint4 o;
+                                        o.x = (uint32_t)m_q[col];
+                                        o.y = (uint32_t)(off + rel);
+                                        o.z = __float_as_uint(m_base[col]);
+                                        o.w = 0u;
+                                        my_log[slot] = o;
+                                    } else {
+                                        log_over = true;
+                                    }
+                                    slot++;
                                 }
-                                slot++;
                             }
                         }
                     }
                 };
-                // software pipeline over the 2 nblk blocks of the tile (half-major, va / vb alternating): the wgmmas of block
-                // b+1 run while block b is tested, across the boundary between the halves too; the survivors are expanded
-                // once the whole tile is in registers.  The sequence is unrolled for each block count, so every issue, wait
-                // and test sits in straight-line code: with the wait inside a run-time loop ptxas cannot prove that the
-                // tested buffer has retired, and serializes every wgmma of the kernel (C7514).
-                for_each_block_count(nblk, [&](auto nb) {
-                    constexpr int NB = decltype(nb)::value, NBT = 2 * NB;
-                    issue(va, 0, 0);
+                // software pipeline over the blocks of the tile: each 64-code half is contracted in NB = ceil(width / MAXW)
+                // blocks of near-equal width (half-major, va / vb alternating).  The wgmmas of block b+1 run while block b
+                // is tested, across the boundary between the halves too; the survivors are expanded once the whole tile is
+                // in registers.  The sequence is unrolled for each width, so every issue, wait and test sits in straight-line
+                // code: with the wait inside a run-time loop ptxas cannot prove that the tested buffer has retired, and
+                // serializes every wgmma of the kernel (C7514).
+                dispatch_range<1, NQT / 16>(ncls, [&](auto nc) {
+                    constexpr int NC = decltype(nc)::value, NB = (16 * NC + MAXW - 1) / MAXW, NBT = 2 * NB;
+                    // block c of a half: U + (c < X) 16-column units from unit c U + min(c, X)
+                    constexpr int U = NC / NB, X = NC % NB;
+                    auto blk = [](auto cc) {
+                        constexpr int c = decltype(cc)::value;
+                        return BlockCols<16 * (c * U + (c < X ? c : X)), 16 * (U + (c < X ? 1 : 0))>{};
+                    };
+                    // the accumulators live only in here, sized for the widest block (block 0).  The first K-step of a
+                    // block overwrites the registers it uses, so they need no initial value.
+                    float va[8 * (U + (X > 0 ? 1 : 0))], vb[8 * (U + (X > 0 ? 1 : 0))];
+                    issue(va, 0, blk(std::integral_constant<int, 0>{}));
                     static_for<NBT>([&](auto bc) {
                         constexpr int b = decltype(bc)::value;
                         if constexpr (b + 1 < NBT) {
-                            if constexpr ((b + 1) & 1) issue(vb, (b + 1) / NB, (b + 1) % NB);
-                            else issue(va, (b + 1) / NB, (b + 1) % NB);
+                            constexpr auto bn = blk(std::integral_constant<int, (b + 1) % NB>{});
+                            if constexpr ((b + 1) & 1) issue(vb, (b + 1) / NB, bn);
+                            else issue(va, (b + 1) / NB, bn);
                             KB2_STALL_BEGIN(t_w);
                             tc::wgmma_wait<1>();
                             KB2_STALL_END(4, t_w);
@@ -585,19 +609,19 @@ ivfpq_tc_filter_kernel(Params p) {
                             tc::wgmma_wait<0>();
                             KB2_STALL_END(4, t_w);
                         }
+                        constexpr auto bb = blk(std::integral_constant<int, b % NB>{});
                         if constexpr (b & 1) {
                             tc::fence_operand(vb);
-                            test(vb, b / NB, b % NB);
+                            test(vb, b / NB, bb);
                         } else {
                             tc::fence_operand(va);
-                            test(va, b / NB, b % NB);
+                            test(va, b / NB, bb);
                         }
                     });
                 });
                 tc::mbar_arrive(bar_a_empty(eg));   // every wgmma of this tile has retired: hand the A buffer back
                 KB2_STALL_BEGIN(t_fl);
-                flush(0);
-                flush(1);
+                flush();
                 KB2_STALL_END(5, t_fl);
             }
             tc::mbar_arrive(bar_b_free);            // this group's wgmmas of the item have all retired
