@@ -29,35 +29,23 @@ launch_gemm_keys(cudaStream_t st, int mode, int metric, const float* Q, const fl
     if (mode == 1 && (ldk & 3) == 0) {
         CUtensorMap tq, tx;
         if (tc::make_tmap(&tq, Q, nq, d) && tc::make_tmap(&tx, X, cols, d)) {
-            static PerDeviceOnce once;
-            once.run([] {
-                cudaFuncSetAttribute((const void*)tc::gemm_keys_tc_kernel<KB2_METRIC_L2, 3>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::smem_bytes(3));
-                cudaFuncSetAttribute((const void*)tc::gemm_keys_tc_kernel<KB2_METRIC_IP, 3>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::smem_bytes(3));
-                cudaFuncSetAttribute((const void*)tc::gemm_keys_tc_kernel<KB2_METRIC_L2, 1>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::smem_bytes(1));
-                cudaFuncSetAttribute((const void*)tc::gemm_keys_tc_kernel<KB2_METRIC_IP, 1>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::smem_bytes(1));
-            });
             dim3 g((unsigned)((cols + tc::BN - 1) / tc::BN), (unsigned)((nq + tc::BM - 1) / tc::BM));
-#define KB2_GEMM_LAUNCH(MM, NST)                                                                                                  \
-    tc::gemm_keys_tc_kernel<MM, NST><<<g, tc::THREADS, tc::smem_bytes(NST), st>>>(tq, tx, qn, xn, nq, cols, d, keys, ldk, bitset, \
-                                                                                  rows, row_base)
-            if (d <= tc::SHORT_K) {
-                if (metric == KB2_METRIC_L2) KB2_GEMM_LAUNCH(KB2_METRIC_L2, 1); else KB2_GEMM_LAUNCH(KB2_METRIC_IP, 1);
-            } else {
-                if (metric == KB2_METRIC_L2) KB2_GEMM_LAUNCH(KB2_METRIC_L2, 3); else KB2_GEMM_LAUNCH(KB2_METRIC_IP, 3);
-            }
-#undef KB2_GEMM_LAUNCH
+            with_metric(metric, [&](auto m) {
+                constexpr int MM = decltype(m)::value;
+                if (d <= tc::SHORT_K)
+                    launch<tc::gemm_keys_tc_kernel<MM, 1>, (int)tc::smem_bytes(1)>(g, tc::THREADS, tc::smem_bytes(1), st, tq, tx, qn,
+                                                                                   xn, nq, cols, d, keys, ldk, bitset, rows, row_base);
+                else
+                    launch<tc::gemm_keys_tc_kernel<MM, 3>, (int)tc::smem_bytes(3)>(g, tc::THREADS, tc::smem_bytes(3), st, tq, tx, qn,
+                                                                                   xn, nq, cols, d, keys, ldk, bitset, rows, row_base);
+            });
             return true;
         }
     }
     dim3 g((unsigned)((cols + GK_BN - 1) / GK_BN), (unsigned)((nq + GK_BM - 1) / GK_BM));
-    if (metric == KB2_METRIC_L2)
-        gemm_keys_kernel<KB2_METRIC_L2><<<g, 256, 0, st>>>(Q, X, qn, xn, nq, cols, d, keys, ldk, bitset, rows, row_base);
-    else
-        gemm_keys_kernel<KB2_METRIC_IP><<<g, 256, 0, st>>>(Q, X, qn, xn, nq, cols, d, keys, ldk, bitset, rows, row_base);
+    with_metric(metric, [&](auto m) {
+        gemm_keys_kernel<decltype(m)::value><<<g, 256, 0, st>>>(Q, X, qn, xn, nq, cols, d, keys, ldk, bitset, rows, row_base);
+    });
     return false;
 }
 

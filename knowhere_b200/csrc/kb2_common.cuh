@@ -9,6 +9,8 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
+#include <utility>
 
 #include "../../include/knowhere_b200.h"
 
@@ -206,7 +208,7 @@ struct PinnedBuf {
     }
 };
 
-// Run `f` once per CUDA device (cudaFuncSetAttribute & friends apply to the current device only; one process may hold
+// Run `f` once per CUDA device (kernel attributes apply to the current device only; one process may hold
 // indexes on several GPUs — the C ABI takes a device ordinal per handle).
 struct PerDeviceOnce {
     std::once_flag flags[64];
@@ -218,6 +220,34 @@ struct PerDeviceOnce {
         std::call_once(flags[dev], f);
     }
 };
+
+constexpr int kMaxDynSmem = 227 * 1024;   // dynamic shared memory one CTA may use on sm_90
+
+// Launches one kernel instance.  A launch with more than the 48 KB of dynamic shared memory every kernel gets by default
+// first raises that instance's limit to MaxSmem, once per device, so no launch depends on a list of instances kept
+// elsewhere.  (The default is 48 KB less the kernel's static shared memory; no kernel launched with dynamic shared
+// memory here has any.)
+template <auto Kernel, int MaxSmem = kMaxDynSmem, typename... Args>
+inline void
+launch(dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    if (smem > 48 * 1024) {
+        static PerDeviceOnce once;
+        once.run([] {
+            KB2_CUDA_CHECK(cudaFuncSetAttribute((const void*)Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MaxSmem));
+        });
+    }
+    Kernel<<<grid, block, smem, st>>>(std::forward<Args>(args)...);
+}
+
+// Calls f(std::integral_constant<int, M>{}) with M the metric as a compile-time constant (COSINE runs as IP).
+template <typename F>
+inline void
+with_metric(int metric, F&& f) {
+    if (metric == KB2_METRIC_L2)
+        f(std::integral_constant<int, KB2_METRIC_L2>{});
+    else
+        f(std::integral_constant<int, KB2_METRIC_IP>{});
+}
 
 // SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe): sizes the persistent grids and the per-CTA
 // buffers that go with them.  Read once per device.

@@ -20,52 +20,6 @@ namespace kb2 {
 
 constexpr int kMaxK = 1024;            // largest k' any selection kernel keeps
 constexpr int kMaxSortEntries = 8192;  // finalize sorts at most this many candidates per query
-constexpr int kMaxDynSmem = 227 * 1024;
-
-inline void
-init_kernel_attributes() {
-    static PerDeviceOnce once;
-    once.run([] {
-        auto set = [](const void* f) {
-            cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-        };
-        set((const void*)finalize_kernel);
-        set((const void*)reduce_partials_kernel);
-        set((const void*)select_keys_kernel);
-        set((const void*)select_keys_hist_kernel);
-        set((const void*)flat_exact_scan_kernel<KB2_METRIC_L2>);
-        set((const void*)flat_exact_scan_kernel<KB2_METRIC_IP>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, false>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_L2, true>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, false>);
-        set((const void*)ivfpq_scan_kernel<1, KB2_METRIC_IP, true>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, false>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_L2, true>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, false>);
-        set((const void*)ivfpq_scan_kernel<2, KB2_METRIC_IP, true>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, false>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_L2, true>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, false>);
-        set((const void*)ivfpq_scan_kernel<3, KB2_METRIC_IP, true>);
-        set((const void*)ivfpq_scan_generic_kernel<KB2_METRIC_L2>);
-        set((const void*)ivfpq_scan_generic_kernel<KB2_METRIC_IP>);
-        set((const void*)ivfflat_scan_kernel<KB2_METRIC_L2>);
-        set((const void*)ivfflat_scan_kernel<KB2_METRIC_IP>);
-        set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_L2, 1, 8>);
-        set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, 1, 8>);
-        set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_L2, 3, 2>);
-        set((const void*)pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, 3, 2>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 1, 8, 256>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 1, 8, 256>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_L2, 3, 2, 128>);
-        set((const void*)pqtc::bound_kernel<KB2_METRIC_IP, 3, 2, 128>);
-        set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_L2, 32>);
-        set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_IP, 32>);
-        set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_L2, 128>);
-        set((const void*)fltc::ivfflat_tc_kernel<KB2_METRIC_IP, 128>);
-        cudaGetLastError();
-    });
-}
 
 struct Counters {
     int64_t launches = 0, codes = 0, code_bytes = 0, pairs = 0, h2d = 0, d2h = 0;
@@ -130,6 +84,28 @@ struct IndexBase {
         s_g_dist.ensure((size_t)shard_world * nq * k);
     }
     DevBuf<uint8_t> s_typed_raw;
+    DevBuf<uint32_t> s_cert;   // dense_knn: [0] max |x|^2 (float bits), [1] uncertified count, [2..] uncertified queries
+
+    // device buffers a search writes its [nq][k] result to: the caller's, or s_out_* when the caller's are on the host
+    void
+    device_out(int64_t nq, int k, int64_t* out_ids, float* out_dist, int64_t*& d_ids, float*& d_dist) {
+        d_ids = out_ids;
+        d_dist = out_dist;
+        if (is_device_ptr(out_ids)) return;
+        s_out_ids.ensure((size_t)nq * k);
+        s_out_dist.ensure((size_t)nq * k);
+        d_ids = s_out_ids.p;
+        d_dist = s_out_dist.p;
+    }
+    // sharded search: one fused all-gather ships every shard's local top-k (s_loc_*), and the merge kernel writes the result
+    void
+    gather_merge(int64_t nq, int k, int64_t* d_ids, float* d_dist) {
+        if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev_c2, stream));
+        comm->all_gather2(s_loc_ids.p, s_g_ids.p, (size_t)nq * k * 8, s_loc_dist.p, s_g_dist.p, (size_t)nq * k * 4, stream);
+        launch_merge_topk(metric, shard_world, nq, k, s_g_ids.p, s_g_dist.p, d_ids, d_dist, stream);
+        if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev_c3, stream));
+        last.launches += 3;
+    }
 
     // L2-normalised device copy of n rows (COSINE)
     const float*
@@ -160,7 +136,6 @@ struct IndexBase {
     void
     init_common() {
         KB2_CUDA_CHECK(cudaSetDevice(device));
-        init_kernel_attributes();
         KB2_CUDA_CHECK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         own_stream = true;
         KB2_CUDA_CHECK(cudaEventCreate(&ev0));
@@ -244,7 +219,7 @@ struct DensePlan {
 
 inline DensePlan
 dense_candidates(IndexBase& ix, const float* Q, int64_t nq, const float* X, const float* xn, int64_t n, int d,
-                 int metric, int k_need, const uint8_t* bitset, const int32_t* rows, int64_t bit_offset = 0) {
+                 int metric, int k_need, const uint8_t* bitset, int64_t bit_offset) {
     cudaStream_t st = ix.stream;
     DensePlan pl;
     pl.Ksel = next_pow2(std::max(32, k_need));
@@ -277,20 +252,20 @@ dense_candidates(IndexBase& ix, const float* Q, int64_t nq, const float* X, cons
         if (pl.used + nsplit > pl.S) {
             const int n_in = pl.used * pl.Ksel;
             const int n_sort = next_pow2(n_in);
-            reduce_partials_kernel<<<(unsigned)nq, 256, (size_t)n_sort * 8, st>>>(ix.s_partial.p, (int)pl.stride(), n_in,
-                                                                                 n_sort, pl.Ksel);
+            launch<reduce_partials_kernel>((unsigned)nq, 256, (size_t)n_sort * 8, st, ix.s_partial.p, (int)pl.stride(), n_in,
+                                           n_sort, pl.Ksel);
             ix.last.launches++;
             pl.used = 1;
         }
         launch_gemm_keys(st, 1, metric, Q, X + c0 * d, ix.s_qn.p, xn + c0, (int)nq, (int)cols, d, ix.s_keys.p, ldk,
-                         bitset, rows, c0 + bit_offset);
+                         bitset, nullptr, c0 + bit_offset);
         const int per_slice = (int)(((cols + nsplit - 1) / nsplit + 31) / 32 * 32);
         const size_t hist_smem = (size_t)per_slice * 4 + 4160;
         if (pl.Ksel >= 64 && hist_smem <= (size_t)kMaxDynSmem) {
-            select_keys_hist_kernel<<<dim3((unsigned)nq, nsplit), 256, hist_smem, st>>>(
+            launch<select_keys_hist_kernel>(dim3((unsigned)nq, nsplit), 256, hist_smem, st,
                 ix.s_keys.p, ldk, (int)cols, std::min(k_need, pl.Ksel), pl.Ksel, ix.s_partial.p, pl.S, pl.used, (uint32_t)c0);
         } else {
-            select_keys_kernel<<<dim3((unsigned)nq, nsplit), kScanThreads, sel_smem, st>>>(
+            launch<select_keys_kernel>(dim3((unsigned)nq, nsplit), kScanThreads, sel_smem, st,
                 ix.s_keys.p, ldk, (int)cols, pl.Ksel, pl.Ksel, ix.s_partial.p, pl.S, pl.used, (uint32_t)c0);
         }
         ix.last.launches += 2;
@@ -312,9 +287,9 @@ launch_finalize(IndexBase& ix, FinalizeParams fp, int64_t nq) {
         const size_t smem_w = (size_t)kFinWarps * ((size_t)((fp.d + 3) & ~3) * 4 + 128 * 24);
         const unsigned g = (unsigned)((nq + kFinWarps - 1) / kFinWarps);
         if (fp.n_partial <= 128)
-            finalize_warp_kernel<4><<<g, kFinWarps * 32, smem_w, ix.stream>>>(fp, nq);
+            launch<finalize_warp_kernel<4>>(g, kFinWarps * 32, smem_w, ix.stream, fp, nq);
         else
-            finalize_warp_kernel<8><<<g, kFinWarps * 32, smem_w, ix.stream>>>(fp, nq);
+            launch<finalize_warp_kernel<8>>(g, kFinWarps * 32, smem_w, ix.stream, fp, nq);
         ix.last.launches++;
         KB2_CUDA_CHECK(cudaGetLastError());
         if (fp.n_partial <= 256) return;
@@ -326,9 +301,75 @@ launch_finalize(IndexBase& ix, FinalizeParams fp, int64_t nq) {
         grid = 8u * num_sms();
         fp.row_loop_nq = nq;
     }
-    finalize_kernel<<<grid, 256, smem, ix.stream>>>(fp);
+    launch<finalize_kernel>(grid, 256, smem, ix.stream, fp);
     ix.last.launches++;
     KB2_CUDA_CHECK(cudaGetLastError());
+}
+
+// Exact dense k-NN of the nq queries Q against the n rows X with norms xn (FLAT, BruteForce, HNSW's exact fallback, the IVF
+// coarse quantizer): candidates from the norm-expanded keys, then finalize re-ranks the k_sel best of each query exactly
+// and writes the k_out best.  `bit_base` is the bitset position of row 0; `labels` (or nullptr: the row) is the reported id.
+// With `certify`, queries whose re-ranked window finalize could not certify (data whose norms are large against the
+// distances: the norm-expanded keys cancel) are searched again with directly accumulated distances, and their rows of the
+// result are finalized again from those candidates.  On ordinary data there are none and this costs one 4-byte copy.
+// `ev_cand`, if given, is recorded once the candidates are queued.  Returns the number of queries redone.
+inline int64_t
+dense_knn(IndexBase& ix, const float* Q, int64_t nq, const float* X, const float* xn, int64_t n, int d, int metric, int k_out,
+          int k_sel, const uint8_t* bitset, int64_t bit_base, const int64_t* labels, int64_t* out_ids, float* out_dist,
+          bool certify, cudaEvent_t ev_cand = nullptr) {
+    cudaStream_t st = ix.stream;
+    const DensePlan pl = dense_candidates(ix, Q, nq, X, xn, n, d, metric, k_out + 16, bitset, bit_base);
+    if (ev_cand) KB2_CUDA_CHECK(cudaEventRecord(ev_cand, st));
+    FinalizeParams fp{};
+    fp.partial = ix.s_partial.p;
+    fp.partial_stride = pl.stride();
+    fp.n_partial = pl.used * pl.Ksel;
+    fp.k_sel = std::min(pl.Ksel, k_sel);
+    fp.k_out = k_out;
+    fp.labels = labels;
+    fp.rerank = 1;
+    fp.raw = X;
+    fp.raw_by_pos = 1;
+    fp.queries = Q;
+    fp.d = d;
+    fp.metric = metric;
+    fp.out_ids = out_ids;
+    fp.out_dist = out_dist;
+    if (certify) {
+        // certification of the re-ranked window (fin_certify) needs max |x|^2 over the rows
+        ix.s_cert.ensure((size_t)nq + 2);
+        KB2_CUDA_CHECK(cudaMemsetAsync(ix.s_cert.p, 0, 8, st));
+        pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, st>>>(xn, n, ix.s_cert.p);
+        fp.cert = ix.s_cert.p;
+    }
+    launch_finalize(ix, fp, nq);
+    if (!certify) return 0;
+    uint32_t* hc = (uint32_t*)ix.h_counter.p;
+    KB2_CUDA_CHECK(cudaMemcpyAsync(hc, ix.s_cert.p + 1, 4, cudaMemcpyDeviceToHost, st));
+    KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+    const int64_t nredo = hc[0];
+    if (nredo == 0) return 0;
+    const int K = pl.Ksel;
+    int nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nredo - 1) / nredo), std::max<int64_t>(1, n / 1024));
+    nsplit = std::min(nsplit, kMaxSortEntries / K);
+    ix.s_partial2.ensure((size_t)nq * nsplit * K);
+    const size_t smem = (size_t)kScanWarps * 2 * K * 8 + (size_t)d * 4;
+    KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "dimension too large for the exact redo scan");
+    const dim3 g((unsigned)nredo, (unsigned)nsplit);
+    const uint32_t* qlist = ix.s_cert.p + 2;
+    with_metric(metric, [&](auto m) {
+        launch<flat_exact_scan_kernel<decltype(m)::value>>(g, kScanThreads, smem, st, Q, X, n, d, bitset, bit_base, qlist, K,
+                                                           ix.s_partial2.p);
+    });
+    ix.last.launches++;
+    KB2_CUDA_CHECK(cudaGetLastError());
+    fp.partial = ix.s_partial2.p;
+    fp.partial_stride = (int64_t)nsplit * K;
+    fp.n_partial = nsplit * K;
+    fp.cert = nullptr;
+    fp.qlist = (const int32_t*)qlist;
+    launch_finalize(ix, fp, nredo);
+    return nredo;
 }
 
 // ============================================================================================
@@ -406,47 +447,16 @@ struct FlatIndex : IndexBase {
         KB2_REQUIRE(k > 0 && k <= kMaxK - 16, KB2_INVALID_ARGS, "k out of range (1..1008)");
         const float* dq = to_device(q, (size_t)nq * dim, s_q);
         const uint8_t* dbits = bitset_to_device(bitset, nbits);
-        const bool dev_out = is_device_ptr(out_ids);
-        int64_t* d_ids = out_ids;
-        float* d_dist = out_dist;
-        if (!dev_out) {
-            s_out_ids.ensure((size_t)nq * k);
-            s_out_dist.ensure((size_t)nq * k);
-            d_ids = s_out_ids.p;
-            d_dist = s_out_dist.p;
-        }
+        int64_t* d_ids;
+        float* d_dist;
+        device_out(nq, k, out_ids, out_dist, d_ids, d_dist);
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev0, stream));
         // bitset indexes internal rows == labels when labels are the identity (like BitsetView over segment offsets);
         // a shard holds the contiguous slice [shard_lo, shard_lo + n) of ONE add() call, so bit = shard_lo + local row
         KB2_REQUIRE(!(dbits && shard_world > 1 && n_add_calls > 1), KB2_NOT_IMPLEMENTED,
                     "FLAT shard: bitset after several add() calls");
-        DensePlan pl = dense_candidates(*this, dq, nq, base.p, norms.p, n, dim, metric, k + 16, dbits, nullptr,
-                                        shard_world > 1 ? shard_lo : 0);
-        if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev1, stream));
-        FinalizeParams fp{};
-        fp.partial = s_partial.p;
-        fp.partial_stride = pl.stride();
-        fp.n_partial = pl.used * pl.Ksel;
-        fp.k_sel = std::min(pl.Ksel, k + 16);
-        fp.k_out = k;
-        fp.rows = nullptr;
-        fp.labels = custom_labels ? labels.p : nullptr;
-        fp.rerank = 1;
-        fp.raw = base.p;
-        fp.raw_by_pos = 1;
-        fp.queries = dq;
-        fp.d = dim;
-        fp.metric = metric;
-        fp.out_ids = d_ids;
-        fp.out_dist = d_dist;
-        fp.out_pos = nullptr;
-        // certification of the re-ranked window (fin_certify) needs max |x|^2 over the base
-        s_cert.ensure((size_t)nq + 2);
-        KB2_CUDA_CHECK(cudaMemsetAsync(s_cert.p, 0, 8, stream));
-        pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, stream>>>(norms.p, n, s_cert.p);
-        fp.cert = s_cert.p;
-        launch_finalize(*this, fp, nq);
-        redo_uncertified(fp, nq, pl.Ksel, dq, n, dbits, shard_world > 1 ? shard_lo : 0);
+        last.flagged = dense_knn(*this, dq, nq, base.p, norms.p, n, dim, metric, k, k + 16, dbits, shard_world > 1 ? shard_lo : 0,
+                                 custom_labels ? labels.p : nullptr, d_ids, d_dist, true, timing ? ev1 : nullptr);
         last.codes = nq * n;
         last.code_bytes = n * (int64_t)dim * 4;  // list-major contraction reads the base once per batch
         last.pairs = nq;
@@ -456,40 +466,6 @@ struct FlatIndex : IndexBase {
             KB2_CUDA_CHECK(cudaEventElapsedTime(&last_stage_ms, ev0, ev1));
             last_kernel_ms = last_stage_ms;
         }
-    }
-
-    // Queries whose re-ranked window finalize could not certify (data whose norms are large against the distances: the
-    // norm-expanded keys cancel) are searched again with directly accumulated distances, and their rows of the result are
-    // finalized again from those candidates.  On ordinary data the list is empty and this costs one 4-byte copy.
-    DevBuf<uint32_t> s_cert;   // [0] max |x|^2 (float bits), [1] uncertified count, [2..] uncertified queries
-    void
-    redo_uncertified(FinalizeParams fp, int64_t nq, int K, const float* dq, int64_t n, const uint8_t* dbits, int64_t bit_base) {
-        uint32_t* hc = (uint32_t*)h_counter.p;
-        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, s_cert.p + 1, 4, cudaMemcpyDeviceToHost, stream));
-        KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
-        const int64_t nredo = hc[0];
-        last.flagged = nredo;
-        if (nredo == 0) return;
-        int nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nredo - 1) / nredo), std::max<int64_t>(1, n / 1024));
-        nsplit = std::min(nsplit, kMaxSortEntries / K);
-        s_partial2.ensure((size_t)nq * nsplit * K);
-        const size_t smem = (size_t)kScanWarps * 2 * K * 8 + (size_t)dim * 4;
-        KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "FLAT: dimension too large for the exact redo scan");
-        const dim3 g((unsigned)nredo, (unsigned)nsplit);
-        if (metric == KB2_METRIC_L2)
-            flat_exact_scan_kernel<KB2_METRIC_L2><<<g, kScanThreads, smem, stream>>>(dq, base.p, n, dim, dbits, bit_base, s_cert.p + 2,
-                                                                                   K, s_partial2.p);
-        else
-            flat_exact_scan_kernel<KB2_METRIC_IP><<<g, kScanThreads, smem, stream>>>(dq, base.p, n, dim, dbits, bit_base, s_cert.p + 2,
-                                                                                   K, s_partial2.p);
-        last.launches++;
-        KB2_CUDA_CHECK(cudaGetLastError());
-        fp.partial = s_partial2.p;
-        fp.partial_stride = (int64_t)nsplit * K;
-        fp.n_partial = nsplit * K;
-        fp.cert = nullptr;
-        fp.qlist = (const int32_t*)(s_cert.p + 2);
-        launch_finalize(*this, fp, nredo);
     }
 
     void
@@ -826,33 +802,34 @@ struct IvfIndex : IndexBase {
             const size_t smem_skewed = (size_t)G * 65536 + common_smem;
             if (G > 0 && smem_skewed <= (size_t)kMaxDynSmem) {
                 const size_t smem = smem_skewed;
-#define KB2_LAUNCH_PQ(GG)                                                                                     \
-    if (metric == KB2_METRIC_L2) {                                                                             \
-        if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_L2, true><<<grid, kScanThreads, smem, st>>>(sp);           \
-        else ivfpq_scan_kernel<GG, KB2_METRIC_L2, false><<<grid, kScanThreads, smem, st>>>(sp);                \
-    } else {                                                                                                   \
-        if (dbits) ivfpq_scan_kernel<GG, KB2_METRIC_IP, true><<<grid, kScanThreads, smem, st>>>(sp);           \
-        else ivfpq_scan_kernel<GG, KB2_METRIC_IP, false><<<grid, kScanThreads, smem, st>>>(sp);                \
-    }
-                if (G == 1) { KB2_LAUNCH_PQ(1) } else if (G == 2) { KB2_LAUNCH_PQ(2) } else { KB2_LAUNCH_PQ(3) }
-#undef KB2_LAUNCH_PQ
+                with_metric(metric, [&](auto m) {
+                    constexpr int MM = decltype(m)::value;
+                    if (G == 1) {
+                        if (dbits) launch<ivfpq_scan_kernel<1, MM, true>>(grid, kScanThreads, smem, st, sp);
+                        else launch<ivfpq_scan_kernel<1, MM, false>>(grid, kScanThreads, smem, st, sp);
+                    } else if (G == 2) {
+                        if (dbits) launch<ivfpq_scan_kernel<2, MM, true>>(grid, kScanThreads, smem, st, sp);
+                        else launch<ivfpq_scan_kernel<2, MM, false>>(grid, kScanThreads, smem, st, sp);
+                    } else {
+                        if (dbits) launch<ivfpq_scan_kernel<3, MM, true>>(grid, kScanThreads, smem, st, sp);
+                        else launch<ivfpq_scan_kernel<3, MM, false>>(grid, kScanThreads, smem, st, sp);
+                    }
+                });
             } else {
                 // one M KB table instead of 64 KB per 16 sub-quantizers: any m, and the skewed kernel's fallback at large k
                 // (its 2K-entry candidate buffers) or many probes per CTA, where the replicated tables do not fit beside them
                 const size_t smem = (size_t)M * 1024 + (size_t)kScanWarps * 2 * Ksel * 8 + (size_t)(np_max + 1) * 4 +
                                     (size_t)np_max * 12 + (size_t)dim * 4;
                 KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "IVF_PQ: m too large for the generic kernel");
-                if (metric == KB2_METRIC_L2)
-                    ivfpq_scan_generic_kernel<KB2_METRIC_L2><<<grid, kScanThreads, smem, st>>>(sp, codes.p, G);
-                else
-                    ivfpq_scan_generic_kernel<KB2_METRIC_IP><<<grid, kScanThreads, smem, st>>>(sp, codes.p, G);
+                with_metric(metric, [&](auto m) {
+                    launch<ivfpq_scan_generic_kernel<decltype(m)::value>>(grid, kScanThreads, smem, st, sp, codes.p, G);
+                });
             }
         } else {
             KB2_REQUIRE(dim % 4 == 0, KB2_NOT_IMPLEMENTED, "IVF_FLAT: dim must be a multiple of 4 on the GPU path");
-            if (metric == KB2_METRIC_L2)
-                ivfflat_scan_kernel<KB2_METRIC_L2><<<grid, kScanThreads, common_smem, st>>>(sp);
-            else
-                ivfflat_scan_kernel<KB2_METRIC_IP><<<grid, kScanThreads, common_smem, st>>>(sp);
+            with_metric(metric, [&](auto m) {
+                launch<ivfflat_scan_kernel<decltype(m)::value>>(grid, kScanThreads, common_smem, st, sp);
+            });
         }
         last.launches++;
         KB2_CUDA_CHECK(cudaGetLastError());
@@ -1045,26 +1022,24 @@ struct IvfIndex : IndexBase {
         }
         {
             const size_t smem = pqtc::bound_smem(pqtc::bound_kmax(kTcACodes, k_base));
-            if (tc_geom_32()) {
-                // m48 x dsub2: three groups through one in-kernel table each (no [nq][m][256] table in global memory)
-#define KB2_BOUND_LAUNCH3(MM)                                                                                                       \
-    pqtc::bound_kernel<MM, 3, 2, 128><<<bound_grid, 128, smem, st>>>(                                                               \
-        nullptr, qlist, qcount, nq, sp.probe_ids, sp.probe_dis, nprobe, p0, kTcACodes, k_base, list_off.p, list_len.p,              \
-        (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p, d_counter.p + 4, npad, sp.queries, tc_pqc_t.p);
-                if (metric == KB2_METRIC_L2) { KB2_BOUND_LAUNCH3(KB2_METRIC_L2) } else { KB2_BOUND_LAUNCH3(KB2_METRIC_IP) }
-#undef KB2_BOUND_LAUNCH3
-            } else {
-                // m16 x dsub8: the batch's tables from lut_build_kernel, 8 warps per CTA over them
-#define KB2_BOUND_LAUNCH(MM)                                                                                                        \
-    pqtc::lut_build_kernel<MM><<<num_sms(), 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);                             \
-    mark("lut");                                                                                                                    \
-    pqtc::bound_kernel<MM, 1, 8, 256><<<bound_grid, 256, smem, st>>>(s_lut.p, qlist, qcount, nq, sp.probe_ids, sp.probe_dis,         \
-                                                                     nprobe, p0, kTcACodes, k_base, list_off.p, list_len.p,         \
-                                                                     (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p,     \
-                                                                     d_counter.p + 4);
-                if (metric == KB2_METRIC_L2) { KB2_BOUND_LAUNCH(KB2_METRIC_L2) } else { KB2_BOUND_LAUNCH(KB2_METRIC_IP) }
-#undef KB2_BOUND_LAUNCH
-            }
+            with_metric(metric, [&](auto m) {
+                constexpr int MM = decltype(m)::value;
+                if (tc_geom_32()) {
+                    // m48 x dsub2: three groups through one in-kernel table each (no [nq][m][256] table in global memory)
+                    launch<pqtc::bound_kernel<MM, 3, 2, 128>>(bound_grid, 128, smem, st, nullptr, qlist, qcount, nq, sp.probe_ids,
+                                                              sp.probe_dis, nprobe, p0, kTcACodes, k_base, list_off.p, list_len.p,
+                                                              (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p,
+                                                              d_counter.p + 4, npad, sp.queries, tc_pqc_t.p);
+                } else {
+                    // m16 x dsub8: the batch's tables from lut_build_kernel, 8 warps per CTA over them
+                    pqtc::lut_build_kernel<MM><<<num_sms(), 256, 0, st>>>(sp.queries, nq, qlist, qcount, pqc.p, s_lut.p);
+                    mark("lut");
+                    launch<pqtc::bound_kernel<MM, 1, 8, 256>>(bound_grid, 256, smem, st, s_lut.p, qlist, qcount, nq, sp.probe_ids,
+                                                              sp.probe_dis, nprobe, p0, kTcACodes, k_base, list_off.p, list_len.p,
+                                                              (const uint4*)codes.p, t1.p, sp.bitset, rows.p, s_bound.p,
+                                                              d_counter.p + 4, 0, nullptr, nullptr);
+                }
+            });
             KB2_CUDA_CHECK(cudaGetLastError());
             last.launches += 2;
         }
@@ -1123,13 +1098,13 @@ struct IvfIndex : IndexBase {
         tp.qflag = s_cand_cnt.p + nq;
         tp.counters = d_counter.p;
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
-#define KB2_TC_LAUNCH(GG, DD)                                                                                                         \
-    if (metric == KB2_METRIC_L2)                                                                                                     \
-        pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_L2, GG, DD><<<num_sms(), pqtc::THREADS, pqtc::TcCfg<GG, DD>::SMEM_BYTES, st>>>(tp);    \
-    else                                                                                                                             \
-        pqtc::ivfpq_tc_filter_kernel<KB2_METRIC_IP, GG, DD><<<num_sms(), pqtc::THREADS, pqtc::TcCfg<GG, DD>::SMEM_BYTES, st>>>(tp);
-        if (tc_geom_18()) { KB2_TC_LAUNCH(1, 8) } else { KB2_TC_LAUNCH(3, 2) }
-#undef KB2_TC_LAUNCH
+        with_metric(metric, [&](auto m) {
+            constexpr int MM = decltype(m)::value;
+            if (tc_geom_18())
+                launch<pqtc::ivfpq_tc_filter_kernel<MM, 1, 8>>(num_sms(), pqtc::THREADS, pqtc::TcCfg<1, 8>::SMEM_BYTES, st, tp);
+            else
+                launch<pqtc::ivfpq_tc_filter_kernel<MM, 3, 2>>(num_sms(), pqtc::THREADS, pqtc::TcCfg<3, 2>::SMEM_BYTES, st, tp);
+        });
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev3, st));
         KB2_CUDA_CHECK(cudaGetLastError());
 #ifdef KB2_FILTER_STALLS
@@ -1140,17 +1115,18 @@ struct IvfIndex : IndexBase {
         lm::scatter_survivors_kernel<<<dim3(16, n_logs), 256, 0, st>>>(logs.log, logs.cnt, logs.cap, s_cand.p, s_cand_cnt.p, kTcCandCap,
                                                                        tp.qflag, d_counter.p);
         // exact_eval trims every survivor row to its k_base best.  Measured at C3: step 1.977 -> 1.957 ms
-#define KB2_TC_EVAL(MM, GG, DD)                                                                                                      \
-    pqtc::exact_eval_kernel<MM, GG, DD><<<(unsigned)nq, 128, 0, st>>>(sp.queries, pqc.p, eval_lut, s_bound.p, (const uint4*)codes.p, npad, t1.p,  \
-                                                                      sp.bitset, rows.p, s_cand.p, s_cand_cnt.p, kTcCandCap, tp.qflag,  \
-                                                                      logs.cnt + n_logs, k_base);
         const float* eval_lut = (tc_geom_18() && !dist) ? s_lut.p : nullptr;   // tables of the whole batch exist only without a communicator
-        if (tc_geom_18()) {
-            if (metric == KB2_METRIC_L2) { KB2_TC_EVAL(KB2_METRIC_L2, 1, 8) } else { KB2_TC_EVAL(KB2_METRIC_IP, 1, 8) }
-        } else {
-            if (metric == KB2_METRIC_L2) { KB2_TC_EVAL(KB2_METRIC_L2, 3, 2) } else { KB2_TC_EVAL(KB2_METRIC_IP, 3, 2) }
-        }
-#undef KB2_TC_EVAL
+        with_metric(metric, [&](auto m) {
+            constexpr int MM = decltype(m)::value;
+            if (tc_geom_18())
+                pqtc::exact_eval_kernel<MM, 1, 8><<<(unsigned)nq, 128, 0, st>>>(sp.queries, pqc.p, eval_lut, s_bound.p, (const uint4*)codes.p,
+                                                                               npad, t1.p, sp.bitset, rows.p, s_cand.p, s_cand_cnt.p,
+                                                                               kTcCandCap, tp.qflag, logs.cnt + n_logs, k_base);
+            else
+                pqtc::exact_eval_kernel<MM, 3, 2><<<(unsigned)nq, 128, 0, st>>>(sp.queries, pqc.p, eval_lut, s_bound.p, (const uint4*)codes.p,
+                                                                               npad, t1.p, sp.bitset, rows.p, s_cand.p, s_cand_cnt.p,
+                                                                               kTcCandCap, tp.qflag, logs.cnt + n_logs, k_base);
+        });
         KB2_CUDA_CHECK(cudaGetLastError());
         last.launches += 4;
         mark("scatter+eval");
@@ -1268,14 +1244,13 @@ struct IvfIndex : IndexBase {
         fpar.log_cap = logs.cap;
         fpar.counters = d_counter.p;
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev2, st));
-#define KB2_FL_LAUNCH(MM, BR) \
-    fltc::ivfflat_tc_kernel<MM, BR><<<num_sms(), fltc::THREADS, fltc::FlCfg<BR>::SMEM_BYTES, st>>>(tx, thi, tlo, fpar);
-        if (metric == KB2_METRIC_L2) {
-            if (item_cap == 32) { KB2_FL_LAUNCH(KB2_METRIC_L2, 32) } else { KB2_FL_LAUNCH(KB2_METRIC_L2, 128) }
-        } else {
-            if (item_cap == 32) { KB2_FL_LAUNCH(KB2_METRIC_IP, 32) } else { KB2_FL_LAUNCH(KB2_METRIC_IP, 128) }
-        }
-#undef KB2_FL_LAUNCH
+        with_metric(metric, [&](auto m) {
+            constexpr int MM = decltype(m)::value;
+            if (item_cap == 32)
+                launch<fltc::ivfflat_tc_kernel<MM, 32>>(num_sms(), fltc::THREADS, fltc::FlCfg<32>::SMEM_BYTES, st, tx, thi, tlo, fpar);
+            else
+                launch<fltc::ivfflat_tc_kernel<MM, 128>>(num_sms(), fltc::THREADS, fltc::FlCfg<128>::SMEM_BYTES, st, tx, thi, tlo, fpar);
+        });
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev3, st));
         KB2_CUDA_CHECK(cudaGetLastError());
         uint32_t* qflag = s_cand_cnt.p + nq;
@@ -1296,23 +1271,9 @@ struct IvfIndex : IndexBase {
     coarse_probes(const float* dq, int64_t q_lo, int64_t q_hi, int nprobe) {
         const int64_t m = q_hi - q_lo;
         if (m <= 0) return;
-        DensePlan pl = dense_candidates(*this, dq + q_lo * dim, m, centroids.p, cnorms.p, nlist, dim, metric, nprobe + 16, nullptr,
-                                        nullptr);
-        FinalizeParams fp{};
-        fp.partial = s_partial.p;
-        fp.partial_stride = pl.stride();
-        fp.n_partial = pl.used * pl.Ksel;
-        fp.k_sel = (int)std::min<int64_t>(std::min(pl.Ksel, nprobe + 16), nlist);
-        fp.k_out = nprobe;
-        fp.rerank = 1;
-        fp.raw = centroids.p;
-        fp.raw_by_pos = 1;
-        fp.queries = dq + q_lo * dim;
-        fp.d = dim;
-        fp.metric = metric;
-        fp.out_ids = s_probe_ids.p + q_lo * nprobe;
-        fp.out_dist = s_probe_dis.p + q_lo * nprobe;
-        launch_finalize(*this, fp, m);
+        dense_knn(*this, dq + q_lo * dim, m, centroids.p, cnorms.p, nlist, dim, metric, nprobe,
+                  (int)std::min<int64_t>(nprobe + 16, nlist), nullptr, 0, nullptr, s_probe_ids.p + q_lo * nprobe,
+                  s_probe_dis.p + q_lo * nprobe, false);
     }
 
     // ---------------------------------------------------------------- Search (ivf.cc:887-1168)
@@ -1338,15 +1299,9 @@ struct IvfIndex : IndexBase {
         //  e2e 2.10 / 2.03 ms without vs 2.12 / 2.09 ms with -- four quarter-size coarse passes cost what the copy hides.)
         const float* dq = to_device(q, (size_t)nq * dim, s_q);
         const uint8_t* dbits = bitset_to_device(bitset, nbits);
-        const bool dev_out = is_device_ptr(out_ids);
-        int64_t* d_ids = out_ids;
-        float* d_dist = out_dist;
-        if (!dev_out) {
-            s_out_ids.ensure((size_t)nq * k);
-            s_out_dist.ensure((size_t)nq * k);
-            d_ids = s_out_ids.p;
-            d_dist = s_out_dist.p;
-        }
+        int64_t* d_ids;
+        float* d_dist;
+        device_out(nq, k, out_ids, out_dist, d_ids, d_dist);
 
         // ---- coarse quantizer.  With a communicator every rank ranks the centroids for its slice of the batch only and the
         //      probe lists are all-gathered (in place; slices padded to the same length).
@@ -1467,13 +1422,7 @@ struct IvfIndex : IndexBase {
             fp.out_dist = dist ? s_loc_dist.p : d_dist;
             launch_finalize(*this, fp, nq);
         }
-        if (dist) {
-            if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev_c2, st));
-            comm->all_gather2(s_loc_ids.p, s_g_ids.p, (size_t)nq * k * 8, s_loc_dist.p, s_g_dist.p, (size_t)nq * k * 4, st);
-            launch_merge_topk(metric, shard_world, nq, k, s_g_ids.p, s_g_dist.p, d_ids, d_dist, st);
-            if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev_c3, st));
-            last.launches += 3;
-        }
+        if (dist) gather_merge(nq, k, d_ids, d_dist);
         unsigned long long* hc = (unsigned long long*)h_counter.p;
         KB2_CUDA_CHECK(cudaMemcpyAsync(hc, d_counter.p, 64, cudaMemcpyDeviceToHost, st));
         results_out(nq, k, out_ids, out_dist, d_ids, d_dist);

@@ -151,10 +151,6 @@ inline void
 range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius, float range_filter, bool has_filter,
                    const JsonObj& cfg, const uint8_t* bitset, int64_t nbits, int64_t** out_lims, int64_t** out_ids,
                    float** out_dist) {
-    static PerDeviceOnce once;
-    once.run([] {
-        cudaFuncSetAttribute((const void*)range_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-    });
     cudaStream_t st = ix.stream;
     FlatIndex* fi = dynamic_cast<FlatIndex*>(&ix);
     IvfIndex* iv = dynamic_cast<IvfIndex*>(&ix);
@@ -205,26 +201,9 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
         iv->seal();
         nprobe = (int)std::min<int64_t>(std::max<int64_t>(cfg.get_int("nprobe", 8), 1), iv->nlist);
         max_empty = (int)cfg.get_int("max_empty_result_buckets", 2);
-        // coarse probes (same as Search)
         ix.s_probe_ids.ensure((size_t)nq * nprobe);
         ix.s_probe_dis.ensure((size_t)nq * nprobe);
-        DensePlan pl = dense_candidates(ix, dq, nq, iv->centroids.p, iv->cnorms.p, iv->nlist, ix.dim, ix.metric,
-                                        nprobe + 16, nullptr, nullptr);
-        FinalizeParams fp{};
-        fp.partial = ix.s_partial.p;
-        fp.partial_stride = pl.stride();
-        fp.n_partial = pl.used * pl.Ksel;
-        fp.k_sel = (int)std::min<int64_t>(std::min(pl.Ksel, nprobe + 16), iv->nlist);
-        fp.k_out = nprobe;
-        fp.rerank = 1;
-        fp.raw = iv->centroids.p;
-        fp.raw_by_pos = 1;
-        fp.queries = dq;
-        fp.d = ix.dim;
-        fp.metric = ix.metric;
-        fp.out_ids = ix.s_probe_ids.p;
-        fp.out_dist = ix.s_probe_dis.p;
-        launch_finalize(ix, fp, nq);
+        iv->coarse_probes(dq, 0, nq, nprobe);
         sp.probe_ids = ix.s_probe_ids.p;
         sp.probe_dis = ix.s_probe_dis.p;
         sp.nprobe = nprobe;
@@ -256,7 +235,7 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
         rp.hits = hits.p;
         rp.count = cnt.p;
         rp.cap = cap;
-        range_scan_kernel<<<(unsigned)(nq * sp.nsplit), kScanThreads, smem, st>>>(rp);
+        launch<range_scan_kernel>((unsigned)(nq * sp.nsplit), kScanThreads, smem, st, rp);
         ix.last.launches++;
         KB2_CUDA_CHECK(cudaGetLastError());
         KB2_CUDA_CHECK(cudaMemcpyAsync(&found, cnt.p, 8, cudaMemcpyDeviceToHost, st));

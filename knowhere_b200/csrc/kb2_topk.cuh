@@ -823,11 +823,7 @@ inline void
 launch_merge_topk(int metric, int world, int64_t nq, int k, const int64_t* in_ids, const float* in_dist, int64_t* out_ids,
                   float* out_dist, cudaStream_t st) {
     const size_t smem = (size_t)world * k * 12 + 16;
-    static PerDeviceOnce once;
-    once.run([] {
-        cudaFuncSetAttribute((const void*)merge_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    });
-    merge_topk_kernel<<<(unsigned)nq, 256, smem, st>>>(metric, world, nq, k, in_ids, in_dist, out_ids, out_dist);
+    launch<merge_topk_kernel>((unsigned)nq, 256, smem, st, metric, world, nq, k, in_ids, in_dist, out_ids, out_dist);
     KB2_CUDA_CHECK(cudaGetLastError());
 }
 

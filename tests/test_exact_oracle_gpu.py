@@ -200,6 +200,27 @@ def test_flat_translated_data(kb, metric, d, k, custom, filtered):
 
 
 @pytest.mark.parametrize("metric", ["L2", "IP"])
+def test_hnsw_fallback_translated_data(kb, metric):
+    """HNSW's exact fallback ranks by the same norm-expanded keys as FLAT and is certified the same way.  Rows
+    1000 + N(0, 1), reached through both of its triggers: a bitset that keeps about 5 % of the rows, and k >= n / 2."""
+    n, nq, d = 20000, 200, 128
+    rng = np.random.default_rng(12)
+    xb = (1000.0 + rng.standard_normal((n, d))).astype(np.float32)
+    xq = (1000.0 + rng.standard_normal((nq, d))).astype(np.float32)
+    D, B = flat_oracle(xb, xq, metric)
+    mask = rng.random(n) >= 0.05                                        # True = filtered out
+    ix = kb.Index("HNSW", metric, d, {"M": 8, "efConstruction": 40})
+    ix.build(xb)
+    ids, dist = ix.search(xq, 10, bitset=_bits(mask))
+    check_topk(ids, dist, D, B, np.arange(n), metric, valid=~mask, what="HNSW filtered fallback")
+    n2, k2 = 2000, 1000
+    small = kb.Index("HNSW", metric, d, {"M": 8, "efConstruction": 40})
+    small.build(xb[:n2])
+    ids, dist = small.search(xq, k2)
+    check_topk(ids, dist, D[:, :n2], B[:, :n2], np.arange(n2), metric, what="HNSW k >= n/2 fallback")
+
+
+@pytest.mark.parametrize("metric", ["L2", "IP"])
 @pytest.mark.parametrize("keep,k", [(0, 10), (5, 10), (100, 500), (700, 1008)])
 def test_flat_sparse_bitset(kb, metric, keep, k):
     """Bitsets that leave fewer than k rows (padding) or none at all."""
