@@ -430,8 +430,9 @@ class B200IndexNode : public IndexNode {
         return r;
     }
     // AnnIterator (index.h:187-195, index_node.h:1099-1200): one iterator per query yielding (id, distance) best-first.
-    // Backed by batched searches with a doubling k (64, 128, ... up to the selection kernels' 1008): results are a
-    // deterministic prefix-stable order, so the iterator resumes where the previous batch ended.
+    // Backed by batched searches with a doubling k (64, 128, ... up to 16384, the largest k FLAT and IVF searches accept):
+    // results are a deterministic prefix-stable order, so the iterator resumes where the previous batch ended.  (HNSW's
+    // beam search keeps its pool in shared memory: there the iterator ends when a larger beam no longer fits.)
     class SearchIterator : public iterator {
      public:
         SearchIterator(const B200IndexNode* node, std::vector<float> q, Json cfg, PlainBits bits)
@@ -463,7 +464,7 @@ class B200IndexNode : public IndexNode {
         void refill() {
             pos_ = 0;
             const int64_t count = kb2_index_count(node_->h_);
-            const int next_k = (int)std::min<int64_t>(std::min<int64_t>(count, 1008), k_ == 0 ? 64 : 2 * (int64_t)k_);
+            const int next_k = (int)std::min<int64_t>(std::min<int64_t>(count, kMaxIteratorK), k_ == 0 ? 64 : 2 * (int64_t)k_);
             if (next_k <= k_) { exhausted_ = true; return; }
             k_ = next_k;
             ids_.assign(k_, -1);
@@ -472,8 +473,9 @@ class B200IndexNode : public IndexNode {
             c[indexparam::EF] = std::max<int>(k_, c.get<int>(indexparam::EF, 0));
             int rc = kb2_index_search(node_->h_, q_.data(), 1, k_, c.dump().c_str(), bits_.data, bits_.nbits, ids_.data(), dis_.data());
             if (rc) { exhausted_ = true; ids_.clear(); return; }
-            if (k_ >= std::min<int64_t>(count, 1008)) exhausted_ = true;   // nothing larger can be asked for
+            if (k_ >= std::min<int64_t>(count, kMaxIteratorK)) exhausted_ = true;   // nothing larger can be asked for
         }
+        static constexpr int64_t kMaxIteratorK = 16384;
         const B200IndexNode* node_;
         std::vector<float> q_;
         Json cfg_;

@@ -1568,7 +1568,7 @@ struct HnswIndex : IndexBase {
         KB2_CUDA_CHECK(cudaMemsetAsync(d_counter.p, 0, 16, st));
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev0, st));
         if (bf) {
-            KB2_REQUIRE(k <= kMaxK - 16, KB2_INVALID_ARGS, "k out of range (1..1008)");
+            KB2_REQUIRE(k <= kMaxLargeK, KB2_INVALID_ARGS, "k out of range (1..16384)");
             brute_force(dq, nq, k, dbits, d_ids, d_dist);
         } else {
             const Launch L = plan_launch(nq, ef_cap, dbits != nullptr);
@@ -1593,7 +1593,7 @@ struct HnswIndex : IndexBase {
         }
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev1, st));
         // rows with fewer than k results although more valid vectors exist: exact fallback (faiss_hnsw.cc:1464-1478)
-        if (dbits && !bf && !cfg.get_bool("disable_fallback_brute_force", false) && k <= kMaxK - 16) {
+        if (dbits && !bf && !cfg.get_bool("disable_fallback_brute_force", false) && k <= kMaxLargeK) {
             s_short.ensure((size_t)nq + 1);
             KB2_CUDA_CHECK(cudaMemsetAsync(s_short.p, 0, 4, st));
             short_rows_kernel<<<grid1d(nq, 256), 256, 0, st>>>(d_ids, nq, k, n_valid, s_short.p + 1, (uint32_t*)s_short.p);

@@ -5,6 +5,8 @@
 // but hand the WHOLE query batch to the device in one call (like the in-tree GPU precedent,
 // src/common/cuvs/integration/cuvs_knowhere_index.cuh:508-632) instead of nq thread-pool tasks.
 #pragma once
+#include <algorithm>
+#include <functional>
 #include <mutex>
 #include <vector>
 
@@ -15,11 +17,15 @@
 #include "kb2_ivfpq_tc.cuh"
 #include "kb2_ivfflat_tc.cuh"
 #include "kb2_json.h"
+#include "kb2_large_k.cuh"
 
 namespace kb2 {
 
 constexpr int kMaxK = 1024;            // largest k' any selection kernel keeps
 constexpr int kMaxSortEntries = 8192;  // finalize sorts at most this many candidates per query
+constexpr int kMaxLargeK = 16384;      // largest candidate window of the large-k path (DESIGN §4.9)
+// scratch of the large-k path beyond the buffers every search uses: queries are processed in groups that fit it, whatever nq
+constexpr int64_t kLargeKScratch = 1ll << 30;
 
 struct Counters {
     int64_t launches = 0, codes = 0, code_bytes = 0, pairs = 0, h2d = 0, d2h = 0;
@@ -57,7 +63,7 @@ struct IndexBase {
     bool timing = false;
     float last_kernel_ms = 0.f;      // dominant kernel of the last search (IVF_PQ tensor-core engine: the filter kernel)
     float last_stage_ms = 0.f;       // whole list-scan stage of the last search (all engines)
-    int last_engine = 0;             // 0: query-major scan kernels, 1: list-major tensor-core engine
+    int last_engine = 0;             // 0: query-major scan kernels, 1: list-major tensor-core engine, 2: large-k path
     float last_comm_ms = 0.f;        // collectives (+ merge) of the last sharded search
     Comm* comm = nullptr;            // not owned (kb2_index_set_comm)
     virtual void set_comm(Comm* c) { comm = c; }
@@ -85,6 +91,13 @@ struct IndexBase {
     }
     DevBuf<uint8_t> s_typed_raw;
     DevBuf<uint32_t> s_cert;   // dense_knn: [0] max |x|^2 (float bits), [1] uncertified count, [2..] uncertified queries
+    // large-k path (kb2_large_k.cuh): key rows / running best sets, selected candidates, and the finalize's sort buffers
+    DevBuf<uint64_t> s_lk_rows, s_lk_cand;
+    DevBuf<float> s_lk_key;
+    DevBuf<int64_t> s_lk_label, s_lk_label2;
+    DevBuf<int32_t> s_lk_slot, s_lk_slot2, s_lk_order, s_lk_off;
+    DevBuf<uint32_t> s_lk_okey, s_lk_okey2, s_lk_info;
+    DevBuf<uint8_t> s_lk_tmp;
 
     // device buffers a search writes its [nq][k] result to: the caller's, or s_out_* when the caller's are on the host
     void
@@ -306,17 +319,187 @@ launch_finalize(IndexBase& ix, FinalizeParams fp, int64_t nq) {
     KB2_CUDA_CHECK(cudaGetLastError());
 }
 
+// ============================================================================================
+// Large-k path (DESIGN §4.9): windows of K > kMaxK candidates per query.  Key rows -> select_rows_kernel -> large finalize.
+// ============================================================================================
+// large-k scratch per launch row besides the rows its keys come from: K candidates and the finalize's sort buffers
+inline int64_t
+large_k_row_bytes(int K) {
+    return (int64_t)K * 48 + 16;
+}
+// launch rows per group so that `per_row` bytes each stay within kLargeKScratch
+inline int64_t
+large_k_group(int64_t nrows, int64_t per_row) {
+    return std::max<int64_t>(1, std::min<int64_t>(nrows, kLargeKScratch / std::max<int64_t>(per_row, 1)));
+}
+
+// out row b <- the min(K, valid) best entries of input row b (b < rows), unsorted, kEmpty padded
+template <typename T>
+inline void
+large_k_select(IndexBase& ix, const T* in, int64_t ld, int64_t len, uint32_t pos_base, int K, uint64_t* out, int64_t out_ld,
+               int64_t rows) {
+    launch<select_rows_kernel<T>>((unsigned)rows, kSelThreads, 0, ix.stream, in, ld, len, pos_base, K, out, out_ld);
+    ix.last.launches++;
+    KB2_CUDA_CHECK(cudaGetLastError());
+}
+
+// Finalize of `rows` launch rows of K selected candidates each (row b: query fp.qlist[b], or q0 + b): keys (exact from
+// fp.raw / fp.raw16 when fp.rerank), labels, (key, label) order by two stable segmented radix sorts (label, then key),
+// the fp.k_out best written to fp.out_*, and with fp.cert the certification finalize_row applies.
+inline void
+large_k_finalize(IndexBase& ix, const FinalizeParams& fp, const uint64_t* cand, int64_t cand_ld, int K, int64_t rows, int64_t q0) {
+    cudaStream_t st = ix.stream;
+    const int64_t n = rows * K;
+    KB2_REQUIRE(n < (1ll << 31), KB2_INTERNAL_ERROR, "large-k finalize: group too large");
+    ix.s_lk_key.ensure(n);
+    ix.s_lk_label.ensure(n);
+    ix.s_lk_label2.ensure(n);
+    ix.s_lk_slot.ensure(n);
+    ix.s_lk_slot2.ensure(n);
+    ix.s_lk_order.ensure(n);
+    ix.s_lk_okey.ensure(n);
+    ix.s_lk_okey2.ensure(n);
+    ix.s_lk_info.ensure((size_t)rows * 4);
+    ix.s_lk_off.ensure((size_t)rows + 1);
+    LargeFin lf{cand, cand_ld, K, q0, ix.s_lk_key.p, ix.s_lk_label.p, ix.s_lk_slot.p, ix.s_lk_okey.p, ix.s_lk_order.p,
+                ix.s_lk_info.p};
+    KB2_CUDA_CHECK(cudaMemsetAsync(ix.s_lk_info.p, 0, (size_t)rows * 16, st));
+    launch<large_rerank_kernel>(dim3((unsigned)rows, (unsigned)((K + 255) / 256)), 256, (size_t)fp.d * 4 + 16, st, fp, lf);
+    segment_offsets_kernel<<<grid1d(rows + 1, 256), 256, 0, st>>>(ix.s_lk_off.p, rows, K);
+    const int32_t* off = ix.s_lk_off.p;
+    size_t b1 = 0, b2 = 0;
+    cub::DeviceSegmentedRadixSort::SortPairs(nullptr, b1, ix.s_lk_label.p, ix.s_lk_label2.p, ix.s_lk_slot.p, ix.s_lk_slot2.p,
+                                             (int)n, (int)rows, off, off + 1, 0, 64, st);
+    cub::DeviceSegmentedRadixSort::SortPairs(nullptr, b2, ix.s_lk_okey.p, ix.s_lk_okey2.p, ix.s_lk_slot2.p, ix.s_lk_order.p,
+                                             (int)n, (int)rows, off, off + 1, 0, 32, st);
+    ix.s_lk_tmp.ensure(std::max(b1, b2));
+    // stable radix sorts: by label, then by key => (key, label) order, equal pairs in slot order
+    cub::DeviceSegmentedRadixSort::SortPairs(ix.s_lk_tmp.p, b1, ix.s_lk_label.p, ix.s_lk_label2.p, ix.s_lk_slot.p,
+                                             ix.s_lk_slot2.p, (int)n, (int)rows, off, off + 1, 0, 64, st);
+    large_gather_keys_kernel<<<grid1d(n, 256), 256, 0, st>>>(lf, ix.s_lk_slot2.p, n);
+    cub::DeviceSegmentedRadixSort::SortPairs(ix.s_lk_tmp.p, b2, ix.s_lk_okey.p, ix.s_lk_okey2.p, ix.s_lk_slot2.p,
+                                             ix.s_lk_order.p, (int)n, (int)rows, off, off + 1, 0, 32, st);
+    large_emit_kernel<<<grid1d(rows * fp.k_out, 256), 256, 0, st>>>(fp, lf, rows);
+    ix.last.launches += 7;
+    KB2_CUDA_CHECK(cudaGetLastError());
+}
+
+// dense_knn for windows k_out + 16 > kMaxK.  The key chunks of the contraction are those of dense_candidates; each query
+// keeps its K = k_out + 16 best in a running set (best of the first chunk, then best of set + next chunk), which the large
+// finalize re-ranks exactly and certifies.  Uncertified queries are redone from directly accumulated distances: the dense
+// mode of range_scan_kernel writes each one's full key row, and the same selection and finalize run on it.
+inline int64_t
+dense_knn_large(IndexBase& ix, const float* Q, int64_t nq, const float* X, const float* xn, int64_t n, int d, int metric,
+                int k_out, const uint8_t* bitset, int64_t bit_base, const int64_t* labels, int64_t* out_ids, float* out_dist,
+                bool certify, cudaEvent_t ev_cand) {
+    cudaStream_t st = ix.stream;
+    const int K = k_out + 16;
+    FinalizeParams fp{};
+    fp.k_sel = K;
+    fp.k_out = k_out;
+    fp.labels = labels;
+    fp.rerank = 1;
+    fp.raw = X;
+    fp.raw_by_pos = 1;
+    fp.queries = Q;
+    fp.d = d;
+    fp.metric = metric;
+    fp.out_ids = out_ids;
+    fp.out_dist = out_dist;
+    if (certify) {
+        ix.s_cert.ensure((size_t)nq + 2);
+        KB2_CUDA_CHECK(cudaMemsetAsync(ix.s_cert.p, 0, 8, st));
+        pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, st>>>(xn, n, ix.s_cert.p);
+        fp.cert = ix.s_cert.p;
+    }
+    ix.s_qn.ensure(nq);
+    if (metric == KB2_METRIC_L2) {
+        row_norms_kernel<<<grid1d(nq * 32, 256), 256, 0, st>>>(Q, nq, d, ix.s_qn.p);
+        ix.last.launches++;
+    }
+    // per query: two running sets of 2K entries, then the finalize's scratch
+    const int64_t g = large_k_group(nq, (int64_t)K * 32 + large_k_row_bytes(K));
+    const int64_t max_key_elems = 64ll << 20;  // 256 MB of keys, as in dense_candidates
+    int64_t chunk = std::min<int64_t>(n, std::max<int64_t>(1024, max_key_elems / g));
+    if (chunk < n) chunk = std::max<int64_t>(128, chunk / 128 * 128);
+    const int64_t ldk = (chunk + 3) & ~(int64_t)3;
+    ix.s_keys.ensure((size_t)g * ldk);
+    ix.s_lk_rows.ensure((size_t)g * 4 * K);
+    for (int64_t q0 = 0; q0 < nq; q0 += g) {
+        const int64_t rows = std::min(g, nq - q0);
+        uint64_t* A = ix.s_lk_rows.p;
+        uint64_t* B = A + (size_t)g * 2 * K;
+        for (int64_t c0 = 0; c0 < n; c0 += chunk) {
+            const int64_t cols = std::min(chunk, n - c0);
+            launch_gemm_keys(st, 1, metric, Q + q0 * d, X + c0 * d, ix.s_qn.p + q0, xn + c0, (int)rows, (int)cols, d, ix.s_keys.p,
+                             ldk, bitset, nullptr, c0 + bit_base);
+            ix.last.launches++;
+            if (c0 == 0) {
+                large_k_select<float>(ix, ix.s_keys.p, ldk, cols, 0u, K, A, 2 * K, rows);
+            } else {
+                large_k_select<float>(ix, ix.s_keys.p, ldk, cols, (uint32_t)c0, K, A + K, 2 * K, rows);
+                large_k_select<uint64_t>(ix, A, 2 * K, 2 * K, 0u, K, B, 2 * K, rows);
+                std::swap(A, B);
+            }
+        }
+        if (ev_cand && q0 + rows == nq) KB2_CUDA_CHECK(cudaEventRecord(ev_cand, st));
+        large_k_finalize(ix, fp, A, 2 * K, K, rows, q0);
+    }
+    if (!certify) return 0;
+    uint32_t* hc = (uint32_t*)ix.h_counter.p;
+    KB2_CUDA_CHECK(cudaMemcpyAsync(hc, ix.s_cert.p + 1, 4, cudaMemcpyDeviceToHost, st));
+    KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+    const int64_t nredo = hc[0];
+    if (nredo == 0) return 0;
+    const int64_t ldr = round_up(n, 32);
+    const int64_t g2 = large_k_group(nredo, ldr * 8 + large_k_row_bytes(K));
+    ix.s_lk_rows.ensure((size_t)g2 * ldr);
+    ix.s_lk_cand.ensure((size_t)g2 * K);
+    RangeParams rp{};
+    rp.sp.queries = Q;
+    rp.sp.nq = (int)nq;
+    rp.sp.d = d;
+    rp.sp.metric = metric;
+    rp.sp.bitset = bitset;
+    rp.sp.vecs = X;
+    rp.kind = 0;
+    rp.single_len = n;
+    rp.bit_base = bit_base;
+    rp.dense = ix.s_lk_rows.p;
+    rp.dense_ld = ldr;
+    const size_t smem = (size_t)d * 4 + 128;
+    KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "dimension too large for the exact redo scan");
+    const uint32_t* qlist = ix.s_cert.p + 2;
+    fp.cert = nullptr;
+    for (int64_t r0 = 0; r0 < nredo; r0 += g2) {
+        const int64_t rows = std::min(g2, nredo - r0);
+        rp.sp.nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + rows - 1) / rows), std::max<int64_t>(1, n / 1024));
+        rp.qlist = qlist + r0;
+        KB2_CUDA_CHECK(cudaMemsetAsync(ix.s_lk_rows.p, 0xFF, (size_t)rows * ldr * 8, st));
+        launch<range_scan_kernel>((unsigned)(rows * rp.sp.nsplit), kScanThreads, smem, st, rp);
+        ix.last.launches++;
+        KB2_CUDA_CHECK(cudaGetLastError());
+        large_k_select<uint64_t>(ix, ix.s_lk_rows.p, ldr, n, 0u, K, ix.s_lk_cand.p, K, rows);
+        fp.qlist = (const int32_t*)(qlist + r0);
+        large_k_finalize(ix, fp, ix.s_lk_cand.p, K, K, rows, 0);
+    }
+    return nredo;
+}
+
 // Exact dense k-NN of the nq queries Q against the n rows X with norms xn (FLAT, BruteForce, HNSW's exact fallback, the IVF
 // coarse quantizer): candidates from the norm-expanded keys, then finalize re-ranks the k_sel best of each query exactly
 // and writes the k_out best.  `bit_base` is the bitset position of row 0; `labels` (or nullptr: the row) is the reported id.
 // With `certify`, queries whose re-ranked window finalize could not certify (data whose norms are large against the
 // distances: the norm-expanded keys cancel) are searched again with directly accumulated distances, and their rows of the
 // result are finalized again from those candidates.  On ordinary data there are none and this costs one 4-byte copy.
-// `ev_cand`, if given, is recorded once the candidates are queued.  Returns the number of queries redone.
+// `ev_cand`, if given, is recorded once the candidates are queued.  Returns the number of queries redone.  Windows
+// k_out + 16 above kMaxK take the large-k path (dense_knn_large); k_sel is then k_out + 16.
 inline int64_t
 dense_knn(IndexBase& ix, const float* Q, int64_t nq, const float* X, const float* xn, int64_t n, int d, int metric, int k_out,
           int k_sel, const uint8_t* bitset, int64_t bit_base, const int64_t* labels, int64_t* out_ids, float* out_dist,
           bool certify, cudaEvent_t ev_cand = nullptr) {
+    if (k_out + 16 > kMaxK)
+        return dense_knn_large(ix, Q, nq, X, xn, n, d, metric, k_out, bitset, bit_base, labels, out_ids, out_dist, certify, ev_cand);
     cudaStream_t st = ix.stream;
     const DensePlan pl = dense_candidates(ix, Q, nq, X, xn, n, d, metric, k_out + 16, bitset, bit_base);
     if (ev_cand) KB2_CUDA_CHECK(cudaEventRecord(ev_cand, st));
@@ -444,7 +627,7 @@ struct FlatIndex : IndexBase {
            float* out_dist) override {
         const int64_t n = count();
         KB2_REQUIRE(n > 0, KB2_EMPTY_INDEX, "index is empty");
-        KB2_REQUIRE(k > 0 && k <= kMaxK - 16, KB2_INVALID_ARGS, "k out of range (1..1008)");
+        KB2_REQUIRE(k > 0 && k <= kMaxLargeK, KB2_INVALID_ARGS, "k out of range (1..16384)");
         const float* dq = to_device(q, (size_t)nq * dim, s_q);
         const uint8_t* dbits = bitset_to_device(bitset, nbits);
         int64_t* d_ids;
@@ -461,7 +644,7 @@ struct FlatIndex : IndexBase {
         last.code_bytes = n * (int64_t)dim * 4;  // list-major contraction reads the base once per batch
         last.pairs = nq;
         results_out(nq, k, out_ids, out_dist, d_ids, d_dist);
-        last_engine = 0;
+        last_engine = (k + 16 > kMaxK) ? 2 : 0;
         if (timing) {
             KB2_CUDA_CHECK(cudaEventElapsedTime(&last_stage_ms, ev0, ev1));
             last_kernel_ms = last_stage_ms;
@@ -1276,6 +1459,94 @@ struct IvfIndex : IndexBase {
                   s_probe_dis.p + q_lo * nprobe, false);
     }
 
+    // ---------------------------------------------------------------- large-k path (DESIGN §4.9)
+    // Candidate windows k_base > kMaxK: the dense mode of range_scan_kernel writes every probed row's key to its query's
+    // row (slot = rank of the row among the query's probed rows, lists padded to 32), select_rows_kernel keeps the k_base
+    // best, and the large finalize refines them (IVF_PQ with refine), maps labels and orders them.  Queries run in groups
+    // whose rows fit kLargeKScratch.
+    void
+    search_large(const float* dq, int64_t nq, int nprobe, int k, int k_base, bool use_refine, const uint8_t* dbits,
+                 int64_t* d_ids, float* d_dist) {
+        cudaStream_t st = stream;
+        // row length: the nprobe longest lists, each padded to 32 rows
+        std::vector<int64_t> padded(nlist);
+        for (int64_t l = 0; l < nlist; l++) padded[l] = round_up(h_list_len[l], 32);
+        std::partial_sort(padded.begin(), padded.begin() + nprobe, padded.end(), std::greater<int64_t>());
+        int64_t L = 32;
+        for (int j = 0; j < nprobe; j++) L += padded[j];
+        const int K = k_base;
+        const int64_t g = large_k_group(nq, L * 8 + large_k_row_bytes(K));
+        s_lk_rows.ensure((size_t)g * L);
+        s_lk_cand.ensure((size_t)g * K);
+        RangeParams rp{};
+        IvfScanParams& sp = rp.sp;
+        sp.queries = dq;
+        sp.nq = (int)nq;
+        sp.d = dim;
+        sp.metric = metric;
+        sp.bitset = dbits;
+        sp.probe_ids = s_probe_ids.p;
+        sp.probe_dis = s_probe_dis.p;
+        sp.nprobe = nprobe;
+        sp.list_off = list_off.p;
+        sp.list_len = list_len.p;
+        sp.rows = rows.p;
+        sp.vecs = vecs.p;
+        sp.pq_centroids = pqc.p;
+        sp.M = M;
+        sp.dsub = dsub;
+        sp.codes = (const uint4*)codes.p;
+        sp.npad = npad;
+        sp.t1 = t1.p;
+        rp.kind = is_pq ? (G > 0 ? 1 : 2) : 0;
+        rp.G = G;
+        rp.codes_b = codes.p;
+        rp.single_len = -1;
+        rp.dense = s_lk_rows.p;
+        rp.dense_ld = L;
+        rp.scanned = d_counter.p;
+        sp.nsplit = (g < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + g - 1) / g) : 1;
+        const int np_max = (nprobe + sp.nsplit - 1) / sp.nsplit;
+        const size_t smem = (size_t)dim * 4 + 64 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12 + (is_pq ? (size_t)M * 1024 : 0);
+        KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "large-k search: m too large");
+        FinalizeParams fp{};
+        fp.k_sel = K;
+        fp.k_out = k;
+        fp.rows = rows.p;
+        fp.labels = custom_labels ? labels.p : nullptr;
+        fp.rerank = use_refine ? 1 : 0;
+        fp.raw = vecs.p;
+        fp.raw16 = (is_pq && refine_kind) ? vecs16.p : nullptr;
+        fp.raw16_kind = refine_kind;
+        fp.raw_by_pos = 1;
+        fp.queries = dq;
+        fp.d = dim;
+        fp.metric = metric;
+        fp.out_ids = d_ids;
+        fp.out_dist = d_dist;
+        KB2_CUDA_CHECK(cudaMemsetAsync(d_counter.p, 0, 8, st));
+        if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev0, st));
+        for (int64_t q0 = 0; q0 < nq; q0 += g) {
+            const int64_t rws = std::min(g, nq - q0);
+            rp.q0 = q0;
+            KB2_CUDA_CHECK(cudaMemsetAsync(s_lk_rows.p, 0xFF, (size_t)rws * L * 8, st));
+            launch<range_scan_kernel>((unsigned)(rws * sp.nsplit), kScanThreads, smem, st, rp);
+            last.launches++;
+            KB2_CUDA_CHECK(cudaGetLastError());
+            large_k_select<uint64_t>(*this, s_lk_rows.p, L, L, 0u, K, s_lk_cand.p, K, rws);
+            large_k_finalize(*this, fp, s_lk_cand.p, K, K, rws, q0);
+        }
+        if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev1, st));
+        unsigned long long* hc = (unsigned long long*)h_counter.p;
+        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, d_counter.p, 8, cudaMemcpyDeviceToHost, st));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+        last.codes = (int64_t)hc[0];
+        last.code_bytes = last.codes * (is_pq ? (int64_t)M : (int64_t)dim * 4);
+        last.pairs = nq * nprobe;
+        last.survivors = 0;
+        last.flagged = 0;
+    }
+
     // ---------------------------------------------------------------- Search (ivf.cc:887-1168)
     void
     search(const float* q, int64_t nq, int k, const JsonObj& cfg, const uint8_t* bitset, int64_t nbits, int64_t* out_ids,
@@ -1289,8 +1560,9 @@ struct IvfIndex : IndexBase {
         const bool use_refine = is_pq && refine;
         const double refine_k = cfg.get_num("refine_k", 1.0);
         KB2_REQUIRE(refine_k >= 1.0, KB2_OUT_OF_RANGE_IN_JSON, "refine_k must be >= 1");
+        KB2_REQUIRE(k > 0 && (use_refine ? (double)k * refine_k : (double)k) <= (double)kMaxLargeK, KB2_INVALID_ARGS,
+                    "k (x refine_k) out of range (max 16384)");
         const int k_base = use_refine ? (int)((double)k * refine_k) : k;  // K/IndexRefine.cpp:80-83
-        KB2_REQUIRE(k > 0 && k_base <= kMaxK, KB2_INVALID_ARGS, "k (x refine_k) out of range (max 1024)");
         const bool dist = distributed();
         KB2_REQUIRE(!dist || (int64_t)shard_world * k <= kMaxSortEntries, KB2_INVALID_ARGS, "world * k too large for the merge");
 
@@ -1318,6 +1590,19 @@ struct IvfIndex : IndexBase {
             if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev_c1, st));
         } else {
             coarse_probes(dq, 0, nq, nprobe);
+        }
+
+        if (k_base > kMaxK) {
+            KB2_REQUIRE(!dist, KB2_NOT_IMPLEMENTED, "sharded search with k (x refine_k) above 1024");
+            search_large(dq, nq, nprobe, k, k_base, use_refine, dbits, d_ids, d_dist);
+            results_out(nq, k, out_ids, out_dist, d_ids, d_dist);
+            last_engine = 2;
+            if (timing) {
+                KB2_CUDA_CHECK(cudaEventElapsedTime(&last_stage_ms, ev0, ev1));
+                last_kernel_ms = last_stage_ms;
+                last_comm_ms = 0.f;
+            }
+            return;
         }
 
         // ---- visiting order of the queries: sorted by nearest list, so that CTAs resident at the same

@@ -552,4 +552,172 @@ ivfflat_scan_kernel(IvfScanParams p) {
     block_emit_topk(lists, p.K, out, p.kout);
 }
 
+// ============================================================================================
+// Row scan with directly accumulated distances: RangeSearch (kb2_range.cuh) and the dense key rows of the large-k path.
+// ============================================================================================
+struct RangeParams {
+    IvfScanParams sp;
+    int kind;            // 0 vectors [pos][d], 1 PQ rotated groups, 2 PQ plain bytes
+    int G;
+    const uint8_t* codes_b;
+    float radius, range_filter;
+    int has_filter;
+    RangeHit* hits;
+    unsigned long long* count;
+    unsigned long long cap;
+    int64_t single_len;  // FLAT: one pseudo-list [0, single_len) (probe arrays unused)
+    // Dense emission (the large-k path, kb2_large_k.cuh): instead of appending in-range hits, every probed row that is not
+    // filtered writes (key, position) to a fixed slot of its query's row dense[i][*] (i = launch row): FLAT the position
+    // itself, IVF the rank of its 32-row chunk among all the query's probed chunks (probe order) * 32 + lane.  Slots nobody
+    // writes keep what the caller filled them with (kEmpty).  Row i is query qlist[i], or q0 + i without a list.
+    uint64_t* dense;
+    int64_t dense_ld;
+    const uint32_t* qlist;
+    int64_t q0;
+    int64_t bit_base;    // bitset position of row 0 (FLAT shard); only the dense mode reads it
+    unsigned long long* scanned;   // dense mode, optional: rows scanned
+};
+
+__device__ __forceinline__ bool
+in_range(float dist, float radius, float range_filter, int has_filter, int metric) {
+    if (metric == KB2_METRIC_L2) return dist < radius && (!has_filter || dist >= range_filter);
+    return dist > radius && (!has_filter || dist <= range_filter);
+}
+
+static inline bool
+in_range_host(float dist, float radius, float range_filter, bool has_filter, int metric) {
+    if (metric == KB2_METRIC_L2) return dist < radius && (!has_filter || dist >= range_filter);
+    return dist > radius && (!has_filter || dist <= range_filter);
+}
+
+// grid = rows * nsplit (rows = nq, or the dense mode's launch rows).  dynamic smem: query | [M*1024 LUT for PQ] | probes
+__global__ void __launch_bounds__(kScanThreads)
+range_scan_kernel(RangeParams rp) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const IvfScanParams& p = rp.sp;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t qi = blockIdx.x / p.nsplit;
+    const int64_t q = rp.qlist ? (int64_t)rp.qlist[qi] : rp.q0 + qi;
+    const int split = blockIdx.x % p.nsplit;
+    float* s_q = (float*)smem_raw;
+    float* lut = s_q + p.d;
+    const size_t lut_floats = (rp.kind == 0) ? 0 : (size_t)p.M * 256;
+    const int np_max = (rp.single_len >= 0) ? 1 : (p.nprobe + p.nsplit - 1) / p.nsplit;
+    ProbeSmem ps;
+    ps.start = (uint32_t*)(lut + lut_floats);
+    ps.off = ps.start + np_max + 1;
+    ps.len = (int32_t*)(ps.off + np_max);
+    ps.dis0 = (float*)(ps.len + np_max);
+
+    for (int i = threadIdx.x; i < p.d; i += blockDim.x) s_q[i] = p.queries[q * p.d + i];
+    int nchunks;
+    int j0 = 0;
+    uint32_t chunk_base = 0;   // dense IVF rows: chunks of the query's probes before this CTA's first one
+    if (rp.single_len >= 0) {
+        // FLAT: split the row range across the nsplit CTAs in multiples of 32 rows
+        const int64_t per = ((rp.single_len + p.nsplit - 1) / p.nsplit + 31) / 32 * 32;
+        const int64_t b = min((long long)rp.single_len, (long long)split * per);
+        const int64_t e = min((long long)rp.single_len, (long long)(b + per));
+        if (threadIdx.x == 0) {
+            ps.start[0] = 0;
+            ps.off[0] = (uint32_t)b;
+            ps.len[0] = (int32_t)(e - b);
+            ps.dis0[0] = 0.f;
+            ps.start[1] = (uint32_t)((e - b + 31) / 32);
+        }
+        __syncthreads();
+        nchunks = (int)ps.start[1];
+    } else {
+        j0 = min(p.nprobe, split * np_max);
+        const int j1 = min(p.nprobe, j0 + np_max);
+        nchunks = setup_probes(p, q, j0, j1, ps);
+        if (rp.dense) {
+            const int64_t pstride = p.probe_stride ? p.probe_stride : p.nprobe;
+            for (int j = 0; j < j0; j++) {   // every thread the same serial sum (j0 <= nprobe <= 1008)
+                const int64_t l = p.probe_ids[q * pstride + j];
+                if (l >= 0) chunk_base += (uint32_t)((p.list_len[l] + 31) >> 5);
+            }
+        }
+    }
+    if (rp.kind != 0) {
+        const float scale = (p.metric == KB2_METRIC_L2) ? -2.f : -1.f;
+        for (int e = threadIdx.x; e < p.M * 256; e += blockDim.x) {
+            const int m = e >> 8;
+            const float* c = p.pq_centroids + (int64_t)e * p.dsub;
+            float acc = 0.f;
+            for (int t = 0; t < p.dsub; t++) acc = fmaf(s_q[m * p.dsub + t], c[t], acc);
+            lut[e] = acc * scale;
+        }
+    }
+    __syncthreads();
+
+    if (rp.scanned && threadIdx.x == 0) {
+        unsigned long long rows_here = 0;
+        const int np_here = (rp.single_len >= 0) ? 1 : min(p.nprobe, j0 + np_max) - j0;
+        for (int j = 0; j < np_here; j++) rows_here += (unsigned long long)ps.len[j];
+        if (rows_here) atomicAdd(rp.scanned, rows_here);
+    }
+    int cur = 0;
+    for (int c = warp; c < nchunks; c += kScanWarps) {
+        while (c >= (int)ps.start[cur + 1]) cur++;
+        const uint32_t rel0 = ((uint32_t)c - ps.start[cur]) * 32u;
+        const uint32_t pos0 = ps.off[cur] + rel0;
+        const int nrows = min(32, ps.len[cur] - (int)rel0);
+        float mykey = INFINITY;
+        if (rp.kind == 0) {
+            for (int r = 0; r < nrows; r++) {
+                const float* x = p.vecs + (int64_t)(pos0 + r) * p.d;
+                float acc = 0.f;
+                if (p.metric == KB2_METRIC_L2) {
+                    for (int j = lane; j < p.d; j += kWarp) {
+                        const float t = s_q[j] - x[j];
+                        acc = fmaf(t, t, acc);
+                    }
+                } else {
+                    for (int j = lane; j < p.d; j += kWarp) acc = fmaf(s_q[j], x[j], acc);
+                }
+                acc = warp_sum(acc);
+                if (lane == r) mykey = (p.metric == KB2_METRIC_L2) ? acc : -acc;
+            }
+        } else if (lane < nrows) {
+            const uint32_t pos = pos0 + lane;
+            float acc = (p.metric == KB2_METRIC_L2) ? p.t1[pos] : 0.f;
+            if (rp.kind == 1) {
+                for (int g = 0; g < rp.G; g++) {
+                    const uint8_t* cb = (const uint8_t*)(p.codes + (int64_t)g * p.npad + pos);
+                    for (int s = 0; s < 16; s++) acc += lut[(g * 16 + ((s + pos) & 15)) * 256 + cb[s]];
+                }
+            } else {
+                const uint8_t* cb = rp.codes_b + (int64_t)pos * p.M;
+                for (int m = 0; m < p.M; m++) acc += lut[m * 256 + cb[m]];
+            }
+            mykey = ps.dis0[cur] + acc;
+        }
+        if (rp.dense) {
+            if (lane < nrows) {
+                const uint32_t pos = pos0 + lane;
+                const bool ok = !p.bitset || !bit_is_set(p.bitset, p.rows ? (int64_t)p.rows[pos] : rp.bit_base + (int64_t)pos);
+                const int64_t slot = (rp.single_len >= 0) ? (int64_t)pos : ((int64_t)chunk_base + c) * 32 + lane;
+                if (ok) rp.dense[qi * rp.dense_ld + slot] = pack_kp(mykey, pos);
+            }
+        } else if (lane < nrows) {
+            const uint32_t pos = pos0 + lane;
+            bool ok = true;
+            if (p.bitset) ok = !bit_is_set(p.bitset, p.rows ? (int64_t)p.rows[pos] : (int64_t)pos);
+            const float dist = (p.metric == KB2_METRIC_L2) ? mykey : -mykey;
+            if (ok && in_range(dist, rp.radius, rp.range_filter, rp.has_filter, p.metric)) {
+                const unsigned long long slot = atomicAdd(rp.count, 1ull);
+                if (slot < rp.cap) {
+                    RangeHit h;
+                    h.q = (int32_t)q;
+                    h.probe = j0 + cur;
+                    h.pos = pos;
+                    h.dist = dist;
+                    rp.hits[slot] = h;
+                }
+            }
+        }
+    }
+}
+
 }  // namespace kb2

@@ -275,6 +275,80 @@ fin_certify(const FinalizeParams& p, int64_t q, float last, float kth, float qq)
     p.cert[2 + atomicAdd(p.cert + 1, 1u)] = (uint32_t)q;
 }
 
+// Exact key of one candidate from the raw store (the re-rank of finalize_row and of the large-k finalize, kb2_large_k.cuh).
+// fin_vec4(p): rows are read four floats at a time and a candidate is summed by 8 lanes, fin_exact_part8 giving lane
+// `sub`'s share; otherwise by a whole warp, fin_exact_part32 giving lane `lane`'s share.  The caller adds the shares (in
+// the same shuffle order everywhere, so every path gets the same bits) and negates for IP.  r = row of the raw store.
+__device__ __forceinline__ bool
+fin_vec4(const FinalizeParams& p) {
+    return (p.d & 3) == 0 && (p.raw16 ? (reinterpret_cast<uintptr_t>(p.raw16) & 7) == 0
+                                      : (reinterpret_cast<uintptr_t>(p.raw) & 15) == 0);
+}
+__device__ __forceinline__ float
+fin_exact_part8(const FinalizeParams& p, const float4* q4, int64_t r, int sub) {
+    float acc = 0.f;
+    // a 16-bit store (refine_type fp16 / bf16) is decoded to fp32 and summed in the same order as the fp32
+    // store, so it answers exactly like a flat store holding the rounded rows
+    const float4* x4 = p.raw16 ? nullptr : reinterpret_cast<const float4*>(p.raw + r * (int64_t)p.d);
+    const uint2* h4 = p.raw16 ? reinterpret_cast<const uint2*>(p.raw16 + r * (int64_t)p.d) : nullptr;
+    for (int j = sub; j < (p.d >> 2); j += 8) {
+        float4 xv;
+        if (x4) {
+            xv = __ldg(x4 + j);
+        } else {
+            const uint2 h = __ldg(h4 + j);
+            if (p.raw16_kind == 1) {
+                const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&h.x));
+                const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
+                xv = make_float4(a.x, a.y, b.x, b.y);
+            } else {
+                xv = make_float4(__uint_as_float(h.x << 16), __uint_as_float(h.x & 0xffff0000u),
+                                 __uint_as_float(h.y << 16), __uint_as_float(h.y & 0xffff0000u));
+            }
+        }
+        const float4 qv = q4[j];
+        if (p.metric == KB2_METRIC_L2) {
+            float t;
+            t = qv.x - xv.x; acc = fmaf(t, t, acc);
+            t = qv.y - xv.y; acc = fmaf(t, t, acc);
+            t = qv.z - xv.z; acc = fmaf(t, t, acc);
+            t = qv.w - xv.w; acc = fmaf(t, t, acc);
+        } else {
+            acc = fmaf(qv.x, xv.x, acc); acc = fmaf(qv.y, xv.y, acc);
+            acc = fmaf(qv.z, xv.z, acc); acc = fmaf(qv.w, xv.w, acc);
+        }
+    }
+    return acc;
+}
+__device__ __forceinline__ float
+fin_exact_part32(const FinalizeParams& p, const float* s_q, int64_t r, int lane) {
+    float acc = 0.f;
+    if (p.raw16) {
+        const uint16_t* x16 = p.raw16 + r * (int64_t)p.d;
+        for (int j = lane; j < p.d; j += kWarp) {
+            const float xv = (p.raw16_kind == 1) ? __half2float(__ushort_as_half(x16[j]))
+                                                 : __uint_as_float((uint32_t)x16[j] << 16);
+            if (p.metric == KB2_METRIC_L2) {
+                const float t = s_q[j] - xv;
+                acc = fmaf(t, t, acc);
+            } else {
+                acc = fmaf(s_q[j], xv, acc);
+            }
+        }
+    } else {
+        const float* x = p.raw + r * (int64_t)p.d;
+        if (p.metric == KB2_METRIC_L2) {
+            for (int j = lane; j < p.d; j += kWarp) {
+                float t = s_q[j] - x[j];
+                acc = fmaf(t, t, acc);
+            }
+        } else {
+            for (int j = lane; j < p.d; j += kWarp) acc = fmaf(s_q[j], x[j], acc);
+        }
+    }
+    return acc;
+}
+
 // dynamic smem: n_sort*8 + k_sel*(4+8+4) + d*4
 __device__ __forceinline__ void
 finalize_row(FinalizeParams p, const int64_t q) {   // p by value: the variable-length branch edits its copy
@@ -338,9 +412,7 @@ finalize_row(FinalizeParams p, const int64_t q) {   // p by value: the variable-
     if (p.rerank) {
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
         const int nwarps = blockDim.x >> 5;
-        const bool vec4 = (p.d & 3) == 0 && (p.raw16 ? (reinterpret_cast<uintptr_t>(p.raw16) & 7) == 0
-                                                      : (reinterpret_cast<uintptr_t>(p.raw) & 15) == 0);
-        if (vec4) {
+        if (fin_vec4(p)) {
             // four candidates per warp at a time (8 lanes each, 128 B per candidate and step): the re-rank is a chain of
             // dependent random-row round trips (L2 / HBM), so candidates in flight per warp are what sets its duration
             const int sub = lane & 7, grp = lane >> 3;
@@ -351,37 +423,7 @@ finalize_row(FinalizeParams p, const int64_t q) {   // p by value: the variable-
                 float acc = 0.f;
                 if (pos != kNoPos) {
                     const int64_t r = p.raw_by_pos ? (int64_t)pos : (p.rows ? (int64_t)p.rows[pos] : (int64_t)pos);
-                    // a 16-bit store (refine_type fp16 / bf16) is decoded to fp32 and summed in the same order as the fp32
-                    // store, so it answers exactly like a flat store holding the rounded rows
-                    const float4* x4 = p.raw16 ? nullptr : reinterpret_cast<const float4*>(p.raw + r * (int64_t)p.d);
-                    const uint2* h4 = p.raw16 ? reinterpret_cast<const uint2*>(p.raw16 + r * (int64_t)p.d) : nullptr;
-                    for (int j = sub; j < (p.d >> 2); j += 8) {
-                        float4 xv;
-                        if (x4) {
-                            xv = __ldg(x4 + j);
-                        } else {
-                            const uint2 h = __ldg(h4 + j);
-                            if (p.raw16_kind == 1) {
-                                const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&h.x));
-                                const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
-                                xv = make_float4(a.x, a.y, b.x, b.y);
-                            } else {
-                                xv = make_float4(__uint_as_float(h.x << 16), __uint_as_float(h.x & 0xffff0000u),
-                                                 __uint_as_float(h.y << 16), __uint_as_float(h.y & 0xffff0000u));
-                            }
-                        }
-                        const float4 qv = q4[j];
-                        if (p.metric == KB2_METRIC_L2) {
-                            float t;
-                            t = qv.x - xv.x; acc = fmaf(t, t, acc);
-                            t = qv.y - xv.y; acc = fmaf(t, t, acc);
-                            t = qv.z - xv.z; acc = fmaf(t, t, acc);
-                            t = qv.w - xv.w; acc = fmaf(t, t, acc);
-                        } else {
-                            acc = fmaf(qv.x, xv.x, acc); acc = fmaf(qv.y, xv.y, acc);
-                            acc = fmaf(qv.z, xv.z, acc); acc = fmaf(qv.w, xv.w, acc);
-                        }
-                    }
+                    acc = fin_exact_part8(p, q4, r, sub);
                 }
                 acc += __shfl_xor_sync(0xffffffffu, acc, 4);
                 acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -394,30 +436,7 @@ finalize_row(FinalizeParams p, const int64_t q) {   // p by value: the variable-
             uint32_t pos = s_pos[i];
             if (pos == kNoPos) continue;
             int64_t r = p.raw_by_pos ? (int64_t)pos : (p.rows ? (int64_t)p.rows[pos] : (int64_t)pos);
-            float acc = 0.f;
-            if (p.raw16) {
-                const uint16_t* x16 = p.raw16 + r * (int64_t)p.d;
-                for (int j = lane; j < p.d; j += kWarp) {
-                    const float xv = (p.raw16_kind == 1) ? __half2float(__ushort_as_half(x16[j]))
-                                                         : __uint_as_float((uint32_t)x16[j] << 16);
-                    if (p.metric == KB2_METRIC_L2) {
-                        const float t = s_q[j] - xv;
-                        acc = fmaf(t, t, acc);
-                    } else {
-                        acc = fmaf(s_q[j], xv, acc);
-                    }
-                }
-            } else {
-                const float* x = p.raw + r * (int64_t)p.d;
-                if (p.metric == KB2_METRIC_L2) {
-                    for (int j = lane; j < p.d; j += kWarp) {
-                        float t = s_q[j] - x[j];
-                        acc = fmaf(t, t, acc);
-                    }
-                } else {
-                    for (int j = lane; j < p.d; j += kWarp) acc = fmaf(s_q[j], x[j], acc);
-                }
-            }
+            float acc = fin_exact_part32(p, s_q, r, lane);
             acc = warp_sum(acc);
             if (lane == 0) s_key[i] = (p.metric == KB2_METRIC_L2) ? acc : -acc;
         }
