@@ -236,7 +236,8 @@ int kb2_index_enable_kernel_timing(kb2_index_t h, int on);
 int kb2_index_last_kernel_ms(kb2_index_t h, float* out_ms);
 /* out4: [0] device ms of the whole list-scan stage of the last search, [1] device ms of its dominant kernel
  * (== kb2_index_last_kernel_ms), [2] engine that served it: 0 = query-major scan kernels, 1 = list-major
- * tensor-core engine (IVF_PQ m=16 d=128 with large batches; kb2_ivfpq_tc.cuh), [3] device ms of the collectives
+ * tensor-core engine (IVF_PQ m=16 d=128 with large batches; kb2_ivfpq_tc.cuh), 2 = large-k path, 3 = HNSW beam
+ * search with one query per CTA (max(ef, k) too large for the four-queries-per-CTA kernels), [3] device ms of the collectives
  * (+ merge kernel) of a sharded search with a communicator */
 int kb2_index_last_stage_info(kb2_index_t h, float* out4);
 

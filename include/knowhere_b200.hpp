@@ -430,9 +430,9 @@ class B200IndexNode : public IndexNode {
         return r;
     }
     // AnnIterator (index.h:187-195, index_node.h:1099-1200): one iterator per query yielding (id, distance) best-first.
-    // Backed by batched searches with a doubling k (64, 128, ... up to 16384, the largest k FLAT and IVF searches accept):
-    // results are a deterministic prefix-stable order, so the iterator resumes where the previous batch ended.  (HNSW's
-    // beam search keeps its pool in shared memory: there the iterator ends when a larger beam no longer fits.)
+    // Backed by batched searches with a doubling k (64, 128, ... up to 16384, the largest k FLAT, IVF and HNSW searches
+    // accept; on HNSW ef = k): results are a deterministic prefix-stable order, so the iterator resumes where the previous
+    // batch ended.
     class SearchIterator : public iterator {
      public:
         SearchIterator(const B200IndexNode* node, std::vector<float> q, Json cfg, PlainBits bits)

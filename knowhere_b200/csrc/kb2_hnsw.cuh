@@ -14,7 +14,8 @@
 // two rows in flight), and the candidate pool is a sorted array in shared memory updated by
 // warp-cooperative shifts.  The algorithm state after each expansion equals the reference's
 // (same pool capacity max(ef,k), same strict/upper_bound tie rules), so with identical graph and
-// distances the result is identical; distances differ by fp32 summation order only.
+// distances the result is identical; distances differ by fp32 summation order only.  Pools too large for four per CTA
+// (max(ef, k) up to 16384) run hnsw_wide_kernel: one query per CTA, same state after every expansion.
 #pragma once
 #include <omp.h>
 
@@ -823,6 +824,341 @@ hnsw_filtered_kernel(HnswSearchParams p) {
 
 
 // ============================================================================================
+// One query per CTA: hnsw_wide_kernel<METRIC, FILTERED> runs the beams whose pools do not fit the four-warp layout of the
+// two kernels above (DESIGN §4.7), max(ef, k) up to kMaxLargeK.  FILTERED = false is hnsw_search_kernel's traversal,
+// FILTERED = true hnsw_filtered_kernel's top-k traversal (two pools, kAlpha budget).  The state after every expansion is
+// theirs, and so the reference's:
+//   * warp 0 reads the popped node's link row in 32-slot chunks and does the visited test-and-set, the touched-id log
+//     and the kAlpha walk in slot order, exactly as the warp kernels; it lists the evaluated neighbours in slot order;
+//   * every warp then computes keys of whole rows (hnsw_key4 / hnsw_key: the warp kernels' per-row arithmetic, so the
+//     keys are bit-identical);
+//   * the listed neighbours enter the pool in one CTA-wide merge (hnsw_wide_merge), which gives the pool of the one-by-one
+//     upper_bound inserts in slot order;
+//   * filtered: an invalid neighbour at slot j is admitted while its key is below the valid pool's back as it stands after
+//     the valid neighbours of slots < j were inserted (thread 0 replays that back, see below).
+// The valid pool lives in shared memory; the invalid pool, popped from the front, in a per-CTA global scratch of 2 * cap
+// entries addressed through a head offset (compacted when the head passes cap).
+// dynamic smem: 8 control ints | query (dpad floats) | valid pool (cap x (4 + 4)) | candidates (deg x 21 bytes)
+// ============================================================================================
+constexpr int kWideWarps = 8;
+constexpr int kWideThreads = kWideWarps * 32;
+constexpr int kWideItems = 4;   // pool entries each thread moves per step of the merge
+
+struct HnswWideParams {
+    HnswSearchParams s;
+    int deg;              // level-0 link slots per node: bound on the neighbours one expansion evaluates
+    float* inv_dist;      // FILTERED: [grid][2 * ef_cap] invalid pool of each CTA
+    uint32_t* inv_id;
+};
+
+// Merges the candidates t < m with kind[t] == want (keys ck, ids cv, listed in link-slot order) into the sorted pool
+// (dist, id) of `size` entries, keeping the first cap.  This is the pool the reference's one-by-one inserts build
+// (Neighbor.h:46-150): each insert goes at upper_bound(key), i.e. after every equal key already present, earlier
+// candidates of the same expansion included, so the final order is (key; old entries, then candidates in slot order),
+// and dropping the last entry at every step keeps the same first cap entries as truncating once.  The smallest insert
+// position of the sequence is the first position written here.  Returns it (cap if nothing enters).  Called by every
+// thread with the same arguments; starts and ends at a barrier.
+__device__ int
+hnsw_wide_merge(float* dist, uint32_t* id, int& size, int cap, const float* ck, const int32_t* cv, const uint8_t* kind,
+                int want, int m, int* c_dest, float* s_sorted, int* s_ctl) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    if (tid < kWarp) {
+        int nsel = 0, p0 = cap;
+        for (int base = 0; base < m; base += kWarp) {
+            const int t = base + lane;
+            const bool sel = t < m && kind[t] == want;
+            int dest = INT_MAX;
+            if (sel) {
+                const float key = ck[t];
+                int r = 0;   // rank among the selected candidates by (key, slot)
+                for (int u = 0; u < m; u++) r += kind[u] == want && (ck[u] < key || (ck[u] == key && u < t));
+                int lo = 0, hi = size;   // upper_bound(key) in the pool
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (dist[mid] <= key) lo = mid + 1; else hi = mid;
+                }
+                dest = lo + r;
+                s_sorted[r] = key;
+                p0 = min(p0, dest);
+            }
+            if (t < m) c_dest[t] = dest;
+            nsel += __popc(__ballot_sync(0xffffffffu, sel));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) p0 = min(p0, __shfl_xor_sync(0xffffffffu, p0, o));
+        if (lane == 0) { s_ctl[0] = nsel; s_ctl[1] = p0; }
+    }
+    __syncthreads();
+    const int nsel = s_ctl[0], p0 = s_ctl[1];
+    if (p0 < cap) {
+        // entry i >= p0 moves up by the number of candidates with a smaller key; high chunks first, so every destination
+        // has been read before it is written
+        constexpr int kChunk = kWideThreads * kWideItems;
+        for (int hi = min(size, cap); hi > p0; hi -= kChunk) {
+            const int lo = max(p0, hi - kChunk);
+            float dv[kWideItems];
+            uint32_t iv[kWideItems];
+            int to[kWideItems];
+#pragma unroll
+            for (int u = 0; u < kWideItems; u++) {
+                const int i = lo + tid + u * kWideThreads;
+                to[u] = -1;
+                if (i < hi) {
+                    dv[u] = dist[i];
+                    iv[u] = id[i];
+                    int a = 0, b = nsel;   // lower_bound(dv[u]) among the sorted candidate keys
+                    while (a < b) {
+                        const int mid = (a + b) >> 1;
+                        if (s_sorted[mid] < dv[u]) a = mid + 1; else b = mid;
+                    }
+                    if (i + a < cap) to[u] = i + a;
+                }
+            }
+            __syncthreads();
+#pragma unroll
+            for (int u = 0; u < kWideItems; u++)
+                if (to[u] >= 0) { dist[to[u]] = dv[u]; id[to[u]] = iv[u]; }
+            __syncthreads();
+        }
+        for (int t = tid; t < m; t += kWideThreads)
+            if (c_dest[t] < cap) { dist[c_dest[t]] = ck[t]; id[c_dest[t]] = (uint32_t)cv[t]; }
+    }
+    __syncthreads();
+    size = min(size + nsel, cap);
+    return p0;
+}
+
+template <int METRIC, bool FILTERED>
+__global__ void __launch_bounds__(kWideThreads)
+hnsw_wide_kernel(HnswWideParams w) {
+    const HnswSearchParams& p = w.s;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int dpad = (p.d + 3) & ~3;
+    const int cap = p.ef_cap, deg = w.deg;
+    int* s_ctl = (int*)smem_raw;
+    float* s_q = (float*)(smem_raw + 32);
+    float* v_dist = s_q + dpad;
+    uint32_t* v_id = (uint32_t*)(v_dist + cap);   // bit31 = checked
+    int32_t* c_v = (int32_t*)(v_id + cap);        // neighbours evaluated by this expansion, in slot order
+    float* c_key = (float*)(c_v + deg);
+    int* c_dest = (int*)(c_key + deg);
+    float* s_sorted = (float*)(c_dest + deg);
+    float* s_add = s_sorted + deg;
+    uint8_t* c_kind = (uint8_t*)(s_add + deg);     // 0 member, 1 filtered and admitted, 2 filtered and not admitted
+
+    uint32_t* vis = p.visited + (int64_t)blockIdx.x * p.nwords;
+    int32_t* vlog = p.vis_log + (int64_t)blockIdx.x * p.log_cap;
+    float* i_dist = FILTERED ? w.inv_dist + (int64_t)blockIdx.x * 2 * cap : nullptr;
+    uint32_t* i_id = FILTERED ? w.inv_id + (int64_t)blockIdx.x * 2 * cap : nullptr;
+    unsigned long long ndis_tot = 0, nhops_tot = 0;   // thread 0's are the CTA's
+    int logn = 0;                                     // warp 0: touched-id log
+    bool log_overflow = false;
+    float alpha = 1.0f;                               // warp 0: accumulated_alpha
+
+    for (;;) {
+        if (tid == 0) s_ctl[0] = atomicAdd(p.next_query, 1);
+        __syncthreads();
+        const int q = s_ctl[0];
+        if (q >= p.nq) break;
+        for (int j = tid; j < p.d; j += kWideThreads) s_q[j] = p.queries[(int64_t)q * p.d + j];
+        __syncthreads();
+
+        if (warp == 0) {
+            int32_t nearest = p.entry_point;
+            float d_nearest = hnsw_key<METRIC>(p.vecs, p.d, s_q, nearest, lane);
+            hnsw_descend<METRIC>(p, s_q, lane, nearest, d_nearest, ndis_tot, nhops_tot);
+            const bool member = !(FILTERED && bit_is_set(p.bitset, nearest + p.bit_offset));
+            if (lane == 0) {
+                if (member) { v_dist[0] = d_nearest; v_id[0] = (uint32_t)nearest; }
+                else { i_dist[0] = d_nearest; i_id[0] = (uint32_t)nearest; }
+                atomicOr(&vis[nearest >> 5], 1u << (nearest & 31));
+                vlog[0] = nearest;
+                s_ctl[1] = member ? 1 : 0;
+            }
+            logn = 1;
+            log_overflow = false;
+            alpha = 1.0f;
+        }
+        __syncthreads();
+        int v_size = 0, v_cur = 0, i_head = 0, i_size = 0;   // the same in every thread
+        if (s_ctl[1]) v_size = 1; else i_size = 1;
+
+        for (;;) {
+            // ---- pop (Neighbor.h:46-150 / 155-210)
+            bool take_inv = false;
+            if (FILTERED) {
+                const float back = (v_size < cap) ? FLT_MAX : v_dist[cap - 1];
+                const bool has_res = v_cur < v_size, has_cand = i_size > 0;
+                if (!(has_res || (has_cand && i_dist[i_head] < back))) break;
+                take_inv = has_cand && (!has_res || i_dist[i_head] < v_dist[v_cur]);
+            } else if (v_cur >= v_size) {
+                break;
+            }
+            uint32_t cur;
+            int popped = -1;
+            if (take_inv) {
+                cur = i_id[i_head];
+                i_head++;
+                if (--i_size == 0) i_head = 0;
+            } else {
+                cur = v_id[v_cur] & 0x7fffffffu;
+                popped = v_cur++;
+                while (v_cur < v_size && (v_id[v_cur] & 0x80000000u)) v_cur++;
+            }
+            nhops_tot++;
+
+            // ---- warp 0: link row, visited test-and-set, kAlpha walk, in slot order
+            if (warp == 0) {
+                const int64_t begin = p.offsets[cur] + p.cum[0];
+                const int64_t end = p.offsets[cur] + p.cum[1];
+                int m = 0;
+                bool done = false;
+                for (int64_t b = begin; b < end && !done; b += kWarp) {
+                    const int32_t v = (b + lane < end) ? p.neighbors[b + lane] : -1;
+                    const unsigned neg = __ballot_sync(0xffffffffu, v < 0);
+                    const int cnt = neg ? (__ffs(neg) - 1) : kWarp;
+                    if (cnt < kWarp) done = true;
+                    bool fresh = false, member = true;
+                    if (lane < cnt) {
+                        const uint32_t bit = 1u << (v & 31);
+                        const uint32_t old = atomicOr(&vis[v >> 5], bit);
+                        fresh = !(old & bit);
+                        if (FILTERED && fresh) member = !bit_is_set(p.bitset, v + p.bit_offset);
+                    }
+                    const unsigned fm = __ballot_sync(0xffffffffu, fresh);
+                    const int nf = __popc(fm);
+                    if (nf == 0) continue;
+                    if (logn + nf <= p.log_cap) {
+                        if (fresh) vlog[logn + __popc(fm & ((1u << lane) - 1))] = v;
+                    } else {
+                        log_overflow = true;
+                    }
+                    logn += nf;
+                    unsigned inv_m = 0, take_m = fm;
+                    if (FILTERED) {
+                        inv_m = __ballot_sync(0xffffffffu, fresh && !member);
+                        take_m = fm & ~inv_m;
+                        unsigned rem = inv_m;
+                        while (rem) {
+                            const int j = __ffs(rem) - 1;
+                            rem &= rem - 1;
+                            alpha += p.k_alpha;
+                            if (alpha < 1.0f) continue;
+                            alpha -= 1.0f;
+                            take_m |= 1u << j;
+                        }
+                    }
+                    ndis_tot += __popc(take_m);
+                    if ((take_m >> lane) & 1u) {
+                        const int t = m + __popc(take_m & ((1u << lane) - 1));
+                        c_v[t] = v;
+                        c_kind[t] = ((inv_m >> lane) & 1u) ? 1 : 0;
+                    }
+                    m += __popc(take_m);
+                }
+                if (lane == 0) s_ctl[2] = m;
+            }
+            __syncthreads();
+            const int m = s_ctl[2];
+            if (tid == 0 && popped >= 0) v_id[popped] |= 0x80000000u;
+
+            // ---- keys: whole rows per warp, four at a time when every warp has work
+            const int per = (m > kWideWarps && (p.d & 3) == 0) ? 4 : 1;
+            for (int g = warp * per; g < m; g += kWideWarps * per) {
+                if (per == 4 && g + 4 <= m) {
+                    float k0, k1, k2, k3;
+                    hnsw_key4<METRIC>(p.vecs, p.d, s_q, c_v[g], c_v[g + 1], c_v[g + 2], c_v[g + 3], lane, k0, k1, k2, k3);
+                    if (lane == 0) { c_key[g] = k0; c_key[g + 1] = k1; c_key[g + 2] = k2; c_key[g + 3] = k3; }
+                } else {
+                    for (int t = g; t < min(g + per, m); t++) {
+                        const float kt = hnsw_key<METRIC>(p.vecs, p.d, s_q, c_v[t], lane);
+                        if (lane == 0) c_key[t] = kt;
+                    }
+                }
+            }
+            __syncthreads();
+            if (m == 0) continue;
+
+            // ---- filtered: admission of the invalid neighbours.  The back the reference compares against at slot j is
+            //      the cap-th smallest key of the old valid pool plus the valid neighbours of slots < j (a valid neighbour
+            //      that did not enter is not below that back, so counting it changes nothing); thread 0 keeps those keys
+            //      sorted and reads the back off the merged tail.
+            if (FILTERED) {
+                if (tid == 0) {
+                    int ns = 0;
+                    for (int t = 0; t < m; t++) {
+                        const float key = c_key[t];
+                        if (c_kind[t] == 0) {
+                            int j = ns++;
+                            while (j > 0 && s_add[j - 1] > key) { s_add[j] = s_add[j - 1]; j--; }
+                            s_add[j] = key;
+                            continue;
+                        }
+                        float bk = FLT_MAX;
+                        const int over = v_size + ns - cap;   // >= 0: the valid pool is full
+                        if (over >= 0) {
+                            int a = v_size - 1, b = ns - 1;   // drop the `over` largest of the union, then take its largest
+                            for (int s = 0; s < over; s++) {
+                                if (b >= 0 && (a < 0 || s_add[b] >= v_dist[a])) b--; else a--;
+                            }
+                            bk = (b >= 0 && (a < 0 || s_add[b] >= v_dist[a])) ? s_add[b] : v_dist[a];
+                        }
+                        c_kind[t] = key < bk ? 1 : 2;
+                    }
+                }
+                __syncthreads();
+            }
+
+            // ---- merge into the pools
+            const int p0 = hnsw_wide_merge(v_dist, v_id, v_size, cap, c_key, c_v, c_kind, 0, m, c_dest, s_sorted, s_ctl + 4);
+            if (p0 < v_cur) v_cur = p0;
+            if (FILTERED) {
+                if (i_head > cap) {   // room for cap entries past the head: move the pool to the front
+                    for (int i = tid; i < i_size; i += kWideThreads) {   // [head, head + size) and [0, size) are disjoint
+                        i_dist[i] = i_dist[i_head + i];
+                        i_id[i] = i_id[i_head + i];
+                    }
+                    __syncthreads();
+                    i_head = 0;
+                }
+                hnsw_wide_merge(i_dist + i_head, i_id + i_head, i_size, cap, c_key, c_v, c_kind, 1, m, c_dest, s_sorted,
+                                s_ctl + 4);
+            }
+        }
+
+        // ---- results (HnswSearcher.h:414-428; IP sign restored as IndexHNSWWrapper.cc:198-204)
+        const int len = min(v_size, p.k);
+        for (int i = tid; i < p.k; i += kWideThreads) {
+            const int64_t o = (int64_t)q * p.k + i;
+            if (i < len) {
+                const int64_t id = (int64_t)(v_id[i] & 0x7fffffffu);
+                p.out_ids[o] = p.labels ? p.labels[id] : id;
+                p.out_dist[o] = (METRIC == KB2_METRIC_L2) ? v_dist[i] : -v_dist[i];
+            } else {
+                p.out_ids[o] = -1;
+                p.out_dist[o] = (METRIC == KB2_METRIC_L2) ? FLT_MAX : -FLT_MAX;
+            }
+        }
+        // ---- clear the visited bits this query set
+        if (tid == 0) s_ctl[3] = log_overflow ? -1 : logn;
+        __syncthreads();
+        const int nlog = s_ctl[3];
+        if (nlog >= 0) {
+            for (int i = tid; i < nlog; i += kWideThreads) vis[vlog[i] >> 5] = 0u;
+        } else {
+            for (int64_t i = tid; i < p.nwords; i += kWideThreads) vis[i] = 0u;
+        }
+        __syncthreads();
+    }
+    if (p.stats && tid == 0) {
+        atomicAdd(&p.stats[0], ndis_tot);
+        atomicAdd(&p.stats[1], nhops_tot);
+    }
+}
+
+
+// ============================================================================================
 // GPU construction (SURVEY 8f rank 3; reference: K/IndexHNSW.cpp:83-215 hnsw_add_vertices, K/impl/HNSW.cpp:231-300
 // shrink_neighbor_list, :302-420 add_links_starting_from).  The reference inserts one node at a time under per-node locks;
 // here every level is built by BATCHED insertion in the reference's order (levels descending): for a batch of new nodes
@@ -1057,6 +1393,8 @@ struct HnswIndex : IndexBase {
     DevBuf<uint32_t> d_qover;
     DevBuf<int64_t> d_offsets, d_labels;
     DevBuf<uint32_t> d_visited;
+    DevBuf<float> d_inv_dist;      // hnsw_wide_kernel<*, true>: per-CTA invalid pools
+    DevBuf<uint32_t> d_inv_id;
     DevBuf<int> d_next;
     bool uploaded = false;
     int64_t last_ndis = 0, last_nhops = 0;
@@ -1507,6 +1845,49 @@ struct HnswIndex : IndexBase {
         d_vlog.ensure((size_t)(L.total_warps * L.log_cap));
         return L;
     }
+    // does the four-warp layout of hnsw_search_kernel / hnsw_filtered_kernel hold this pool (plan_launch's condition)?
+    bool
+    warp_layout_fits(int ef_cap, bool two_pools) const {
+        const int dpad = (dim + 3) & ~3;
+        return kHnswWarps * ((size_t)dpad * 4 + (size_t)ef_cap * (two_pools ? 16 : 8)) <= (size_t)kMaxDynSmem;
+    }
+    // shared memory of one hnsw_wide_kernel CTA (layout at the kernel)
+    size_t
+    wide_smem(int ef_cap, int dpad) const {
+        return (size_t)round_up(32 + (int64_t)dpad * 4 + (int64_t)ef_cap * 8 + (int64_t)h_cum[1] * 21, 16);
+    }
+    // one query per CTA: one visited bitmap and log per CTA, and for filtered search one invalid pool of 2 * ef_cap entries
+    Launch
+    plan_wide(int64_t nq, int ef_cap, bool filtered) {
+        const int dpad = (dim + 3) & ~3;
+        Launch L;
+        L.smem = wide_smem(ef_cap, dpad);
+        if (ef_cap > kMaxLargeK)
+            throw Error(KB2_OUT_OF_RANGE_IN_JSON, "HNSW: max(ef, k) = " + std::to_string(ef_cap) +
+                                                      " out of range (the graph search keeps at most 16384 candidates)");
+        if (L.smem > (size_t)kMaxDynSmem) {
+            int dmax = 0;
+            while (wide_smem(ef_cap, dmax + 4) <= (size_t)kMaxDynSmem) dmax += 4;
+            throw Error(KB2_OUT_OF_RANGE_IN_JSON, "HNSW: dim " + std::to_string(dim) + " too large for max(ef, k) = " +
+                                                      std::to_string(ef_cap) + " (at most " + std::to_string(dmax) + ")");
+        }
+        const int ctas_per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)kMaxDynSmem / L.smem));
+        L.grid = (int)std::min<int64_t>(nq, (int64_t)num_sms() * ctas_per_sm);
+        L.total_warps = L.grid;
+        L.nwords = (n + 31) / 32;
+        // past nwords touched ids, clearing the whole bitmap is the cheaper of the two
+        L.log_cap = (int)std::min<int64_t>(n, std::max<int64_t>(L.nwords, 1024));
+        if (d_visited.n < (size_t)(L.total_warps * L.nwords)) {
+            d_visited.ensure((size_t)(L.total_warps * L.nwords));
+            KB2_CUDA_CHECK(cudaMemsetAsync(d_visited.p, 0, (size_t)(L.total_warps * L.nwords) * 4, stream));
+        }
+        d_vlog.ensure((size_t)(L.total_warps * L.log_cap));
+        if (filtered) {
+            d_inv_dist.ensure((size_t)L.grid * 2 * ef_cap);
+            d_inv_id.ensure((size_t)L.grid * 2 * ef_cap);
+        }
+        return L;
+    }
     HnswSearchParams
     base_params(const float* dq, int64_t nq, int ef_cap, int k, const Launch& L) {
         HnswSearchParams p{};
@@ -1567,9 +1948,36 @@ struct HnswIndex : IndexBase {
         if (dbits) bf = bf || (double)n_filtered >= (double)n * 0.93 || (double)k >= (double)n_valid * 0.5;
         KB2_CUDA_CHECK(cudaMemsetAsync(d_counter.p, 0, 16, st));
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev0, st));
+        // a pool the four-warp kernels cannot hold runs one query per CTA (a collective search over a communicator keeps the
+        // warp kernels' limit; a shard searched on its own does not)
+        const bool wide = !bf && !dist && !warp_layout_fits(ef_cap, dbits != nullptr);
         if (bf) {
             KB2_REQUIRE(k <= kMaxLargeK, KB2_INVALID_ARGS, "k out of range (1..16384)");
             brute_force(dq, nq, k, dbits, d_ids, d_dist);
+        } else if (wide) {
+            const Launch L = plan_wide(nq, ef_cap, dbits != nullptr);
+            KB2_CUDA_CHECK(cudaMemsetAsync(d_next.p, 0, 4, st));
+            HnswWideParams w{};
+            w.s = base_params(dq, nq, ef_cap, k, L);
+            w.s.out_ids = d_ids;
+            w.s.out_dist = d_dist;
+            w.deg = h_cum[1] - h_cum[0];
+            if (dbits) {
+                w.s.bitset = dbits;
+                w.s.bit_offset = shard_world > 1 ? shard_lo : 0;
+                w.s.k_alpha = (float)((double)n_filtered / (double)n) * 0.7f;   // faiss_hnsw.cc:1425
+                w.inv_dist = d_inv_dist.p;
+                w.inv_id = d_inv_id.p;
+            }
+            with_metric(metric, [&](auto m) {
+                constexpr int MM = decltype(m)::value;
+                if (dbits)
+                    launch<hnsw_wide_kernel<MM, true>>(L.grid, kWideThreads, L.smem, st, w);
+                else
+                    launch<hnsw_wide_kernel<MM, false>>(L.grid, kWideThreads, L.smem, st, w);
+            });
+            last.launches++;
+            KB2_CUDA_CHECK(cudaGetLastError());
         } else {
             const Launch L = plan_launch(nq, ef_cap, dbits != nullptr);
             KB2_CUDA_CHECK(cudaMemsetAsync(d_next.p, 0, 4, st));
@@ -1591,6 +1999,7 @@ struct HnswIndex : IndexBase {
             last.launches++;
             KB2_CUDA_CHECK(cudaGetLastError());
         }
+        last_engine = wide ? 3 : 0;   // set once the search's kernel was launched
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev1, st));
         // rows with fewer than k results although more valid vectors exist: exact fallback (faiss_hnsw.cc:1464-1478)
         if (dbits && !bf && !cfg.get_bool("disable_fallback_brute_force", false) && k <= kMaxLargeK) {

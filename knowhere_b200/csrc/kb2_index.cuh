@@ -63,7 +63,8 @@ struct IndexBase {
     bool timing = false;
     float last_kernel_ms = 0.f;      // dominant kernel of the last search (IVF_PQ tensor-core engine: the filter kernel)
     float last_stage_ms = 0.f;       // whole list-scan stage of the last search (all engines)
-    int last_engine = 0;             // 0: query-major scan kernels, 1: list-major tensor-core engine, 2: large-k path
+    int last_engine = 0;             // 0: query-major scan kernels, 1: list-major tensor-core engine, 2: large-k path,
+                                     // 3: HNSW beam with one query per CTA (hnsw_wide_kernel)
     float last_comm_ms = 0.f;        // collectives (+ merge) of the last sharded search
     Comm* comm = nullptr;            // not owned (kb2_index_set_comm)
     virtual void set_comm(Comm* c) { comm = c; }
