@@ -53,8 +53,12 @@ enum {
     KB2_INTERNAL_ERROR = 27
 };
 
-/* metric ids (reference: include/knowhere/comp/index_param.h metric names "L2","IP","COSINE") */
-enum { KB2_METRIC_L2 = 0, KB2_METRIC_IP = 1, KB2_METRIC_COSINE = 2 };
+/* metric ids (reference: include/knowhere/comp/index_param.h metric names "L2","IP","COSINE"; the MAX_SIM_* emb-list
+ * metrics, index_param.h:280-285, only for kb2_bruteforce_search_emb_list; "MAX_SIM" is MAX_SIM_COSINE) */
+enum {
+    KB2_METRIC_L2 = 0, KB2_METRIC_IP = 1, KB2_METRIC_COSINE = 2,
+    KB2_METRIC_MAX_SIM_L2 = 3, KB2_METRIC_MAX_SIM_IP = 4, KB2_METRIC_MAX_SIM_COSINE = 5
+};
 
 typedef struct kb2_index* kb2_index_t;
 typedef struct kb2_comm* kb2_comm_t;
@@ -199,6 +203,25 @@ int kb2_bruteforce_range_search(const float* base, int64_t nb, int dim, int metr
                                 int64_t nq, float radius, float range_filter, int has_range_filter,
                                 const uint8_t* bitset, int64_t bitset_nbits, int64_t** out_lims,
                                 int64_t** out_ids, float** out_dist, int device, void* cuda_stream);
+
+/* ---- emb-list (multi-vector) exact search: knowhere::BruteForce::Search with a MAX_SIM_* metric and EMB_LIST_OFFSET on
+ * both datasets (src/common/comp/brute_force.cc:258-300,424-584,626-665; include/knowhere/emb_list_utils.h).
+ * Document i is base rows [base_lims[i], base_lims[i+1]), query list j is query rows [query_lims[j], query_lims[j+1]);
+ * rows are dim fp32.  Offsets (n_docs + 1 and n_lists + 1 entries, host or device) start at 0 and do not decrease.
+ *   score(Q, D) = sum over q in Q of max over x in D of <q, x>      KB2_METRIC_MAX_SIM_IP; _COSINE: unit q and x / |x|
+ *   score(Q, D) = sum over q in Q of min over x in D of |q - x|^2   KB2_METRIC_MAX_SIM_L2 (smaller is better)
+ * Result [n_lists][k]: document ids best first, ties by ascending id; out_dist is the score itself (not negated).
+ * Bit i of the bitset filters out document i; a bitset must cover n_docs bits.  An empty document is never returned.
+ * Missing entries have id -1 and distance FLT_MIN (MAX_SIM_IP / _COSINE: std::numeric_limits<float>::min(), as the
+ * reference pads, brute_force.cc:566-581) or FLT_MAX (MAX_SIM_L2).  An empty query list gets a whole row of that padding
+ * (the reference leaves such a row as allocated, brute_force.cc:653-655).  k: 1..16384.  Malformed offsets or sizes:
+ * KB2_INVALID_ARGS; any other metric (MAX_SIM_HAMMING / _JACCARD: no binary vectors here): KB2_INVALID_METRIC_TYPE.
+ * out_stats (nullable) int64[3]: query lists, candidate slots re-ranked exactly, lists scored exactly over every document
+ * (lists the filter could not certify, or every list when dim % 4 != 0).  DESIGN §4.10. */
+int kb2_bruteforce_search_emb_list(const float* base, const int64_t* base_lims, int64_t n_docs, int dim, int metric,
+                                   const float* queries, const int64_t* query_lims, int64_t n_lists, int k,
+                                   const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids, float* out_dist,
+                                   int64_t* out_stats, int device, void* cuda_stream);
 
 /* ---- multi-GPU: one process per GPU, inverted lists sharded (kb2_index_set_shard), collectives over NCCL/NVLink
  * INSIDE the library (SURVEY §8e; the reference has no multi-GPU path: one index per device,

@@ -16,6 +16,7 @@
 // (src/index/index.cc:159-420 wraps node calls in GuardedCall, expected.h:408-430).
 #pragma once
 #include <algorithm>
+#include <cctype>
 #include <cstring>
 #include <functional>
 #include <map>
@@ -36,7 +37,7 @@ enum class Status {
     success = 0, invalid_args = 1, invalid_param_in_json = 2, out_of_range_in_json = 3, type_conflict_in_json = 4,
     invalid_metric_type = 5, empty_index = 6, not_implemented = 7, index_not_trained = 8, index_already_trained = 9,
     faiss_inner_error = 10, hnsw_inner_error = 12, malloc_error = 13, invalid_binary_set = 19,
-    cuda_runtime_error = 22, invalid_index_error = 23, internal_error = 27,
+    cuda_runtime_error = 22, invalid_index_error = 23, internal_error = 27, emb_list_inner_error = 31,
 };
 
 template <typename T>
@@ -65,6 +66,7 @@ constexpr const char* TOPK = "k";
 constexpr const char* METRIC_TYPE = "metric_type";
 constexpr const char* RADIUS = "radius";
 constexpr const char* RANGE_FILTER = "range_filter";
+constexpr const char* EMB_LIST_OFFSET = "EMB_LIST_OFFSET";   // const size_t* [lists + 1] (index_param.h:127)
 }  // namespace meta
 namespace indexparam {
 constexpr const char* NLIST = "nlist";
@@ -82,6 +84,14 @@ namespace metric {
 constexpr const char* L2 = "L2";
 constexpr const char* IP = "IP";
 constexpr const char* COSINE = "COSINE";
+// emb-list metrics (index_param.h:280-285); MAX_SIM is MAX_SIM_COSINE.  HAMMING / JACCARD need binary vectors, which this
+// library does not have: searches with them return invalid_metric_type.
+constexpr const char* MAX_SIM = "MAX_SIM";
+constexpr const char* MAX_SIM_COSINE = "MAX_SIM_COSINE";
+constexpr const char* MAX_SIM_IP = "MAX_SIM_IP";
+constexpr const char* MAX_SIM_L2 = "MAX_SIM_L2";
+constexpr const char* MAX_SIM_HAMMING = "MAX_SIM_HAMMING";
+constexpr const char* MAX_SIM_JACCARD = "MAX_SIM_JACCARD";
 }  // namespace metric
 namespace IndexEnum {
 constexpr const char* INDEX_FAISS_IDMAP = "FLAT";
@@ -171,7 +181,14 @@ class DataSet {
     const int64_t* GetIds() const { return ids_; }
     const float* GetDistance() const { return dist_; }
     const size_t* GetLims() const { return lims_; }
+    // keyed values (dataset.h:423-441); the one key this library reads is meta::EMB_LIST_OFFSET (const size_t*)
+    template <typename T> void Set(const std::string& k, T v) { kv_[k] = (const void*)v; }
+    template <typename T> T Get(const std::string& k) const {
+        auto it = kv_.find(k);
+        return it == kv_.end() ? T() : (T)it->second;
+    }
  private:
+    std::map<std::string, const void*> kv_;
     int64_t rows_ = 0, dim_ = 0;
     const void* tensor_ = nullptr;
     const int64_t* ids_ = nullptr;
@@ -579,15 +596,48 @@ class IndexFactory {
     std::map<std::string, Creator> map_;
 };
 
+// emb-list metric names (emb_list_utils.h:225-263, case-insensitive as IsMetricType): true for every MAX_SIM* name, with
+// `code` the C ABI metric, or -1 for MAX_SIM_HAMMING / MAX_SIM_JACCARD (no binary vectors here)
+inline bool kb2_emb_list_metric(const std::string& name, int& code) {
+    std::string m = name;
+    for (auto& c : m) c = (char)toupper((unsigned char)c);
+    if (m == metric::MAX_SIM || m == metric::MAX_SIM_COSINE) code = KB2_METRIC_MAX_SIM_COSINE;
+    else if (m == metric::MAX_SIM_IP) code = KB2_METRIC_MAX_SIM_IP;
+    else if (m == metric::MAX_SIM_L2) code = KB2_METRIC_MAX_SIM_L2;
+    else if (m == metric::MAX_SIM_HAMMING || m == metric::MAX_SIM_JACCARD) code = -1;
+    else return false;
+    return true;
+}
+// The lists of an EMB_LIST_OFFSET over `rows` rows, as EmbListOffset(lims, rows) reads them (emb_list_utils.h:30-41):
+// offsets up to the first one equal to the row count, so trailing empty lists are dropped.  False when no offset equals it.
+inline bool kb2_emb_list_offsets(const size_t* lims, int64_t rows, std::vector<int64_t>& out) {
+    out.clear();
+    size_t i = 0;
+    for (; (int64_t)lims[i] < rows; i++) out.push_back((int64_t)lims[i]);
+    out.push_back((int64_t)lims[i]);
+    return (int64_t)lims[i] == rows;
+}
+
 // ------------------------------------------------------------------ BruteForce (brute_force.h:26-69)
 class BruteForce {
  public:
     template <typename DataType>
     static expected<DataSetPtr> Search(const DataSetPtr base, const DataSetPtr query, const Json& cfg,
                                        const BitsetView& bitset, void* = nullptr) noexcept {
-        const int64_t nq = query->GetRows();
+        int64_t nq = query->GetRows();
         const int k = cfg.get<int>(meta::TOPK, 0);
         if (k <= 0) return expected<DataSetPtr>::Err(Status::invalid_args, "k must be positive");
+        int code = 0;
+        if (kb2_emb_list_metric(cfg.get_string(meta::METRIC_TYPE, "L2"), code)) {
+            // brute_force.cc:270-281: one result row per query list
+            const size_t* ql = query->Get<const size_t*>(meta::EMB_LIST_OFFSET);
+            if (!ql || !base->Get<const size_t*>(meta::EMB_LIST_OFFSET))
+                return expected<DataSetPtr>::Err(Status::invalid_args, "metric type is emb_list, but missing emb_list offset");
+            std::vector<int64_t> lims;
+            if (!kb2_emb_list_offsets(ql, nq, lims))
+                return expected<DataSetPtr>::Err(Status::invalid_args, "emb_list offsets do not end at the row count");
+            nq = (int64_t)lims.size() - 1;
+        }
         auto ids = std::make_unique<int64_t[]>(nq * k);
         auto dis = std::make_unique<float[]>(nq * k);
         Status s = SearchWithBuf<DataType>(base, query, ids.get(), dis.get(), cfg, bitset);
@@ -597,6 +647,21 @@ class BruteForce {
     template <typename DataType>
     static Status SearchWithBuf(const DataSetPtr base, const DataSetPtr query, int64_t* ids, float* dis, const Json& cfg,
                                 const BitsetView& bitset, void* = nullptr) noexcept {
+        const size_t* bl = base->Get<const size_t*>(meta::EMB_LIST_OFFSET);
+        const size_t* ql = query->Get<const size_t*>(meta::EMB_LIST_OFFSET);
+        int code = 0;
+        if (kb2_emb_list_metric(cfg.get_string(meta::METRIC_TYPE, "L2"), code)) {
+            // brute_force.cc:626-665
+            if (!bl || !ql) return Status::invalid_metric_type;
+            std::vector<int64_t> xl, qlv;
+            if (!kb2_emb_list_offsets(bl, base->GetRows(), xl) || !kb2_emb_list_offsets(ql, query->GetRows(), qlv))
+                return Status::invalid_args;
+            return (Status)kb2_bruteforce_search_emb_list(
+                (const float*)base->GetTensor(), xl.data(), (int64_t)xl.size() - 1, (int)base->GetDim(), code,
+                (const float*)query->GetTensor(), qlv.data(), (int64_t)qlv.size() - 1, cfg.get<int>(meta::TOPK, 0), bitset.data(),
+                (int64_t)bitset.size(), ids, dis, nullptr, 0, nullptr);
+        }
+        if (ql) return Status::invalid_metric_type;   // brute_force.cc:673-676: emb-list query, single-vector metric
         Status st;
         const int metric = kb2_metric_of(cfg, st);
         if (st != Status::success) return st;
@@ -608,6 +673,9 @@ class BruteForce {
     template <typename DataType>
     static expected<DataSetPtr> RangeSearch(const DataSetPtr base, const DataSetPtr query, const Json& cfg,
                                             const BitsetView& bitset, void* = nullptr) noexcept {
+        int code = 0;
+        if (kb2_emb_list_metric(cfg.get_string(meta::METRIC_TYPE, "L2"), code))   // index_node.cc:301-310
+            return expected<DataSetPtr>::Err(Status::emb_list_inner_error, "range search is not supported for emb_list");
         Status st;
         const int metric = kb2_metric_of(cfg, st);
         if (st != Status::success) return expected<DataSetPtr>::Err(st, "bad metric");

@@ -84,6 +84,7 @@ def _declare(L):
     L.kb2_bruteforce_search.argtypes = [vp, i64, i32, i32, vp, i64, i32, vp, i64, vp, vp, i32, vp]
     L.kb2_bruteforce_range_search.argtypes = [vp, i64, i32, i32, vp, i64, f32, f32, i32, vp, i64,
                                               c.POINTER(vp), c.POINTER(vp), c.POINTER(vp), i32, vp]
+    L.kb2_bruteforce_search_emb_list.argtypes = [vp, vp, i64, i32, i32, vp, vp, i64, i32, vp, i64, vp, vp, vp, i32, vp]
     L.kb2_merge_topk.argtypes = [i32, i32, i64, i32, vp, vp, vp, vp, i32, vp]
     if hasattr(L, "kb2_faiss_describe"):
         L.kb2_faiss_describe.argtypes = [vp, c.c_size_t, i32, vp, c.c_size_t]
@@ -433,6 +434,48 @@ def brute_force_search(base, queries, k, metric="L2", bitset=None, device=0, str
     _check(L.kb2_bruteforce_search(_ptr(base), base.shape[0], base.shape[1], _METRICS[metric], _ptr(queries), nq, k,
                                    _ptr(bitset), nbits, _ptr(ids), _ptr(dist), device, ctypes.c_void_p(stream)))
     return ids, dist
+
+
+# emb-list metrics (reference index_param.h:280-285; names are case-insensitive, "MAX_SIM" is MAX_SIM_COSINE).  Names the
+# library has no metric for (MAX_SIM_HAMMING, MAX_SIM_JACCARD) go through as -1, which it rejects as an invalid metric.
+_EMB_METRICS = {"MAX_SIM": 5, "MAX_SIM_COSINE": 5, "MAX_SIM_IP": 4, "MAX_SIM_L2": 3}
+
+
+def brute_force_search_emb_list(base, base_lims, queries, query_lims, k, metric="MAX_SIM", bitset=None, device=0,
+                                stream=0, stats=False):
+    """knowhere::BruteForce::Search over emb-lists with a MAX_SIM metric (reference src/common/comp/brute_force.cc:424-665).
+
+    base: [rows, dim] float32; base_lims: int64 [n_docs + 1], document i = base rows [lims[i], lims[i+1]).  queries /
+    query_lims likewise for the query lists.  Each may be a numpy array or a CUDA tensor.  Returns (ids, dist) of shape
+    [n_lists, k] (CUDA tensors when queries are), ids = document indices best first and dist = the MaxSim score; with
+    stats=True also an int64 array [query lists, candidate slots re-ranked, lists scored exactly over every document]."""
+    L = lib()
+    for lims in (base_lims, query_lims):
+        if _is_torch(lims) and str(lims.dtype) != "torch.int64":
+            raise TypeError("list offsets must be int64")
+    if not _is_torch(base_lims):
+        base_lims = np.ascontiguousarray(base_lims, np.int64)
+    if not _is_torch(query_lims):
+        query_lims = np.ascontiguousarray(query_lims, np.int64)
+    n_docs, n_lists = int(base_lims.shape[0]) - 1, int(query_lims.shape[0]) - 1
+    if base.ndim != 2 or queries.ndim != 2 or queries.shape[1] != base.shape[1]:
+        raise KnowhereError(1, "base and queries must be [rows, dim] with the same dim")
+    if n_docs < 1 or n_lists < 0 or int(base_lims[-1]) != base.shape[0] or int(query_lims[-1]) != queries.shape[0]:
+        raise KnowhereError(1, "list offsets must end at the row count of their dataset")
+    if _is_torch(queries) and queries.is_cuda:
+        import torch
+        ids = torch.empty((n_lists, k), dtype=torch.int64, device=queries.device)
+        dist = torch.empty((n_lists, k), dtype=torch.float32, device=queries.device)
+    else:
+        ids = np.empty((n_lists, k), np.int64)
+        dist = np.empty((n_lists, k), np.float32)
+    st = np.zeros(3, np.int64)
+    nbits = 0 if bitset is None else (bitset.numel() if _is_torch(bitset) else bitset.size) * 8
+    _check(L.kb2_bruteforce_search_emb_list(_ptr(base), _ptr(base_lims), n_docs, base.shape[1],
+                                            _EMB_METRICS.get(str(metric).upper(), -1), _ptr(queries), _ptr(query_lims),
+                                            n_lists, k, _ptr(bitset), nbits, _ptr(ids), _ptr(dist), _ptr(st), device,
+                                            ctypes.c_void_p(stream)))
+    return (ids, dist, st) if stats else (ids, dist)
 
 
 def brute_force_range_search(base, queries, radius, range_filter=None, metric="L2", bitset=None, device=0):

@@ -11,6 +11,7 @@
 #include "kb2_fourcc.h"
 #include "kb2_hnsw.cuh"
 #include "kb2_index.cuh"
+#include "kb2_maxsim.cuh"
 #include "kb2_range.cuh"
 
 using namespace kb2;
@@ -749,6 +750,7 @@ namespace {
 struct BfSlot {
     std::mutex mu;
     std::unique_ptr<FlatIndex> fi;
+    msim::Scratch el;   // emb-list search (kb2_bruteforce_search_emb_list)
 };
 BfSlot g_bf[64];
 
@@ -831,6 +833,72 @@ kb2_bruteforce_range_search(const float* base, int64_t nb, int dim, int metric, 
                            has_range_filter != 0, cfg, bitset, bitset_nbits, out_lims, out_ids, out_dist);
         fi.base.release();
         fi.n_used = 0;
+    });
+}
+
+namespace {
+// host copy of n + 1 list offsets (host or device), checked: they start at 0 and do not decrease
+std::vector<int64_t>
+read_lims(const int64_t* lims, int64_t n, const char* what) {
+    std::vector<int64_t> h((size_t)n + 1);
+    if (is_device_ptr(lims)) KB2_CUDA_CHECK(cudaMemcpy(h.data(), lims, h.size() * 8, cudaMemcpyDeviceToHost));
+    else memcpy(h.data(), lims, h.size() * 8);
+    KB2_REQUIRE(h[0] == 0, KB2_INVALID_ARGS, std::string(what) + " offsets must start at 0");
+    for (int64_t i = 0; i < n; i++)
+        KB2_REQUIRE(h[i + 1] >= h[i], KB2_INVALID_ARGS, std::string(what) + " offsets must not decrease");
+    return h;
+}
+}  // namespace
+
+int
+kb2_bruteforce_search_emb_list(const float* base, const int64_t* base_lims, int64_t n_docs, int dim, int metric,
+                               const float* queries, const int64_t* query_lims, int64_t n_lists, int k,
+                               const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids, float* out_dist,
+                               int64_t* out_stats, int device, void* cuda_stream) {
+    return guarded([&] {
+        KB2_REQUIRE(base && base_lims && queries && query_lims && out_ids && out_dist, KB2_INVALID_ARGS, "null buffer");
+        KB2_REQUIRE(n_docs > 0 && dim > 0 && n_lists >= 0, KB2_INVALID_ARGS, "bad sizes");
+        KB2_REQUIRE(k > 0 && k <= kMaxLargeK, KB2_INVALID_ARGS, "k out of range (1..16384)");
+        KB2_REQUIRE(metric == KB2_METRIC_MAX_SIM_L2 || metric == KB2_METRIC_MAX_SIM_IP || metric == KB2_METRIC_MAX_SIM_COSINE,
+                    KB2_INVALID_METRIC_TYPE, "metric must be MAX_SIM_L2, MAX_SIM_IP or MAX_SIM_COSINE");
+        require_device(device);
+        KB2_REQUIRE(device < 64, KB2_INVALID_ARGS, "bad device ordinal");
+        if (out_stats) out_stats[0] = out_stats[1] = out_stats[2] = 0;
+        const std::vector<int64_t> xl = read_lims(base_lims, n_docs, "base");
+        const std::vector<int64_t> ql = read_lims(query_lims, n_lists, "query");
+        const int64_t nb = xl.back();
+        // positions of the selection entries and TMA row coordinates are 32-bit
+        KB2_REQUIRE(nb > 0 && nb < (1ll << 31) && n_docs < (1ll << 31) && ql.back() < (1ll << 31), KB2_INVALID_ARGS,
+                    "emb-list sizes out of range (base rows 1 .. 2^31 - 1)");
+        KB2_REQUIRE(!bitset || bitset_nbits <= 0 || bitset_nbits >= n_docs, KB2_INVALID_ARGS,
+                    "bitset has fewer bits than the base has documents");
+        if (n_lists == 0) return;
+        const int inner = metric == KB2_METRIC_MAX_SIM_L2 ? KB2_METRIC_L2 : metric == KB2_METRIC_MAX_SIM_IP ? KB2_METRIC_IP
+                                                                                                            : KB2_METRIC_COSINE;
+        BfSlot& slot = g_bf[device];
+        std::lock_guard<std::mutex> lk(slot.mu);
+        FlatIndex& fi = bf_prepare(slot, device, inner, dim, cuda_stream, base, nb);
+        const int64_t nq_rows = ql.back();
+        const float* dq = fi.cosine ? fi.normalized(queries, nq_rows) : fi.to_device(queries, (size_t)nq_rows * dim, fi.s_q);
+        const uint8_t* dbits = nullptr;
+        if (bitset && bitset_nbits > 0) {
+            dbits = bitset;
+            if (!is_device_ptr(bitset)) {
+                const size_t nbytes = (size_t)((n_docs + 7) / 8);
+                slot.el.bits.ensure(nbytes);
+                KB2_CUDA_CHECK(cudaMemcpyAsync(slot.el.bits.p, bitset, nbytes, cudaMemcpyHostToDevice, fi.stream));
+                dbits = slot.el.bits.p;
+            }
+        }
+        int64_t* d_ids;
+        float* d_dist;
+        fi.device_out(n_lists, k, out_ids, out_dist, d_ids, d_dist);
+        int64_t stats[3] = {0, 0, 0};
+        msim::search(fi, slot.el, dq, xl, ql, dim, fi.metric, k, dbits, d_ids, d_dist, stats);
+        fi.results_out(n_lists, k, out_ids, out_dist, d_ids, d_dist);
+        fi.base.release();
+        fi.n_used = 0;
+        if (out_stats) memcpy(out_stats, stats, sizeof(stats));
     });
 }
 

@@ -1085,6 +1085,9 @@ struct IvfIndex : IndexBase {
         s_pair_base.ensure((size_t)npairs);
         KB2_CUDA_CHECK(cudaMemsetAsync(s_lcount.p, 0, (size_t)2 * nlist * 4, ps));
         KB2_CUDA_CHECK(cudaMemsetAsync(s_plan_out.p + 4, 0, 4, ps));
+        // pairs on empty lists (or on other shards' lists) get no slot, so the tail of the pair array stays unwritten: mark it
+        // as no query (-1) for gather_split_queries_kernel, which reads every entry below npairs
+        KB2_CUDA_CHECK(cudaMemsetAsync(s_pair_q.p, 0xFF, (size_t)npairs * 4, ps));
         lm::count_pairs_kernel<<<grid1d(npairs, 256), 256, 0, ps>>>(probe_ids, npairs, list_len.p, s_lcount.p);
         int32_t* items = s_items.p;   // list | q0 | nq
         lm::plan_kernel<<<1, 1024, 0, ps>>>(s_lcount.p, (int)nlist, item_cap, s_lstart.p, items, items + max_items,

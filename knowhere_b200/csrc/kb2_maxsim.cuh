@@ -1,0 +1,581 @@
+// kb2_maxsim.cuh — BruteForce search over emb-lists (multi-vector rows) with the MAX_SIM metrics (DESIGN §4.10).
+//
+//   score(Q, D) = sum over q in Q of ( max over x in D of <q, x> )        MAX_SIM_IP, MAX_SIM / MAX_SIM_COSINE (unit rows)
+//   score(Q, D) = sum over q in Q of ( min over x in D of |q - x|^2 )     MAX_SIM_L2 (smaller is better)
+//
+// Reference: src/common/comp/brute_force.cc:424-584 (one thread per query list builds the |Q| x |D| distance block of every
+// document, then get_sum_max_sim), include/knowhere/emb_list_utils.h:28-107,154-176.
+//
+// Internally every score is a key, smaller is better: the sum over the query tokens of min over x of (-<q, x>) for IP,
+// of |q - x|^2 for L2.  Three stages per chunk of query lists:
+//   1. maxsim_filter_kernel: persistent, sm_90a.  The 3xTF32 wgmma contraction of gemm_keys_tc_kernel with query tokens on
+//      M and base tokens on N; its epilogue takes each query token's extremum over every document of the base tile and sums
+//      them over the tokens of each query list.  It writes one approximate key per (query list, document) to S, never the
+//      token-by-token distances.
+//   2. select_rows_kernel keeps the K = k + 16 best of each S row; maxsim_exact_kernel recomputes their keys in fp32 on the
+//      CUDA cores in a fixed order; a segmented radix sort orders them by (key, document); maxsim_emit_kernel writes the k
+//      best and certifies the list against the filter's error bound (maxsim_bound).
+//   3. Lists that could not be certified are redone with exact keys for every document (maxsim_exact_kernel over all
+//      documents), selected and emitted again.  dim % 4 != 0 (no TMA) takes that exact all-documents path for every list.
+#pragma once
+#include "kb2_index.cuh"
+
+namespace kb2 {
+namespace msim {
+
+constexpr int BM = tc::BM;        // query tokens per block: two consumer warpgroups of 64 rows
+constexpr int BN = tc::BN;        // base rows per tile
+constexpr int MAXD = 32;          // documents per work item
+constexpr int STAGES = 3;
+constexpr size_t SMEM_BYTES = (size_t)STAGES * tc::STAGE_BYTES + (size_t)MAXD * BM * 4 + 2 * MAXD * 4 + 2 * STAGES * 8 + 1024;
+
+// A work item: base rows [row0, row0 + 128 * ntiles) holding the whole documents [doc0, doc0 + ndocs).  Either several
+// documents in one tile, or one document longer than a tile over ntiles consecutive tiles.
+struct Item {
+    int32_t row0, ntiles, doc0, ndocs;
+};
+
+struct FilterParams {
+    const Item* items;
+    int nitems;
+    const int64_t* xlims;      // [n_docs + 1] base list offsets
+    const int64_t* qlims;      // [n_lists + 1] query list offsets
+    const int32_t* row_list;   // [query rows] list of each query row
+    const float* qn;           // |q|^2 per query row (L2)
+    const float* xn;           // |x|^2 per base row (L2)
+    int64_t r0, r1;            // query rows of the chunk (whole lists)
+    int64_t l0;                // first list of the chunk: S row 0
+    int d;
+    const uint8_t* bitset;     // bit i: document i filtered out (its S entry stays +inf)
+    float* S;                  // [lists of the chunk][lds] approximate keys
+    int64_t lds;
+};
+
+// grid = persistent (min(#SMs, items)), block = tc::THREADS (two consumer warpgroups + the TMA producer warp), dynamic
+// smem SMEM_BYTES.  Each CTA walks the items blockIdx.x, + gridDim.x, ...; for each item it walks the query blocks of the
+// chunk in order, and for each block the item's tiles.  A tile's TMA box and the query box stay resident in L2 across the
+// blocks, so the base is read from HBM once per chunk.  Per tile, thread rows keep their extremum over the columns of each
+// document (one quad of lanes holds an accumulator row: a pass over the thread's columns and two shuffles), folded into
+// R[doc][row] across the tiles of a long document.  After the last tile the tokens of each query list are summed over the
+// rows in order; a list that continues into the next block carries its partial sums in `carry` (double-buffered by block
+// parity).  Every S entry is written once, by one thread: the result does not depend on scheduling.
+template <int METRIC>
+__global__ void __launch_bounds__(tc::THREADS, 1)
+maxsim_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                     const FilterParams p) {
+    using namespace tc;
+    extern __shared__ unsigned char smem_dyn[];
+    const uint32_t raw = smem_u32(smem_dyn);
+    const uint32_t base = (raw + 1023u) & ~1023u;
+    unsigned char* base_ptr = smem_dyn + (base - raw);
+    float* R = reinterpret_cast<float*>(base_ptr + STAGES * STAGE_BYTES);   // [MAXD][BM]
+    float* carry = R + MAXD * BM;                                           // [2][MAXD]
+    const uint32_t bars = base + STAGES * STAGE_BYTES + (uint32_t)(MAXD * BM + 2 * MAXD) * 4u;
+    auto bar_full = [&](int s) { return bars + 8u * s; };
+    auto bar_empty = [&](int s) { return bars + 8u * (STAGES + s); };
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nkb = (p.d + BK - 1) / BK;
+    const int64_t nqb = (p.r1 - p.r0 + BM - 1) / BM;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < STAGES; s++) {
+            mbar_init(bar_full(s), 1);
+            mbar_init(bar_empty(s), CONS_THREADS);
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == PRODUCER_WARP) {
+        if (lane == 0) {
+            uint32_t it = 0;
+            for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+                const Item w = p.items[item];
+                for (int64_t qb = 0; qb < nqb; qb++)
+                    for (int t = 0; t < w.ntiles; t++)
+                        for (int kb = 0; kb < nkb; kb++, it++) {
+                            const int s = (int)(it % STAGES);
+                            const uint32_t ph = (it / STAGES) & 1u;
+                            mbar_wait(bar_empty(s), ph ^ 1u);
+                            const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
+                            mbar_expect_tx(bar_full(s), 2 * TILE_BYTES);
+                            tma_load_2d(st, &tmap_q, kb * BK, (int)(p.r0 + qb * BM), bar_full(s));
+                            tma_load_2d(st + TILE_BYTES, &tmap_x, kb * BK, w.row0 + t * BN, bar_full(s));
+                        }
+            }
+        }
+        return;
+    }
+    const int t = threadIdx.x;   // 0..255
+    const int wg = t >> 7;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // block rows of this thread: rl (acc i = 0) and rl + 8 (i = 1)
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] = 0.f;
+    uint32_t it = 0;
+    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+        const Item w = p.items[item];
+        for (int64_t qb = 0; qb < nqb; qb++) {
+            const int64_t b0 = p.r0 + qb * BM;
+            float qq0 = 0.f, qq1 = 0.f;
+            if (METRIC == KB2_METRIC_L2) {
+                if (b0 + rl < p.r1) qq0 = p.qn[b0 + rl];
+                if (b0 + rl + 8 < p.r1) qq1 = p.qn[b0 + rl + 8];
+            }
+            for (int tile = 0; tile < w.ntiles; tile++) {
+                for (int kb = 0; kb < nkb; kb++, it++) {
+                    const int s = (int)(it % STAGES);
+                    const uint32_t ph = (it / STAGES) & 1u;
+                    mbar_wait(bar_full(s), ph);
+                    float4* hi = reinterpret_cast<float4*>(base_ptr + (size_t)s * STAGE_BYTES);
+                    float4* lo = reinterpret_cast<float4*>(base_ptr + (size_t)s * STAGE_BYTES + 2 * TILE_BYTES);
+#pragma unroll 4
+                    for (int i = t; i < 2 * TILE_BYTES / 16; i += CONS_THREADS) {
+                        float4 v = hi[i];
+                        float4 h, l;
+                        h.x = tf32_rn(v.x); l.x = tf32_rn(v.x - h.x);
+                        h.y = tf32_rn(v.y); l.y = tf32_rn(v.y - h.y);
+                        h.z = tf32_rn(v.z); l.z = tf32_rn(v.z - h.z);
+                        h.w = tf32_rn(v.w); l.w = tf32_rn(v.w - h.w);
+                        hi[i] = h;
+                        lo[i] = l;
+                    }
+                    fence_proxy_async();
+                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    const uint32_t st = base + (uint32_t)s * STAGE_BYTES;
+                    const uint32_t a_off = (uint32_t)wg * 64u * 128u;
+                    fence_operand(acc);
+                    wgmma_fence();
+#pragma unroll
+                    for (int kk = 0; kk < BK / 8; kk++) {
+                        const uint32_t ko = (uint32_t)kk * 32u;
+                        const uint64_t a_hi = make_desc(st + a_off + ko);
+                        const uint64_t b_hi = make_desc(st + TILE_BYTES + ko);
+                        const uint64_t a_lo = make_desc(st + 2 * TILE_BYTES + a_off + ko);
+                        const uint64_t b_lo = make_desc(st + 3 * TILE_BYTES + ko);
+                        wgmma_tf32_n128(acc, a_hi, b_hi, (kb > 0 || kk > 0) ? 1u : 0u);
+                        wgmma_tf32_n128(acc, a_hi, b_lo, 1u);
+                        wgmma_tf32_n128(acc, a_lo, b_hi, 1u);
+                    }
+                    wgmma_commit();
+                    fence_operand(acc);
+                    // the previous stage's wgmmas have retired once at most one group is pending: release its slot
+                    wgmma_wait<1>();
+                    if (kb > 0) mbar_arrive(bar_empty((int)((it - 1) % STAGES)));
+                }
+                wgmma_wait<0>();
+                fence_operand(acc);
+                mbar_arrive(bar_empty((int)((it - 1) % STAGES)));
+                // ---- epilogue of the tile: per document, each row's extremum over the document's columns in this tile
+                const int64_t trow0 = (int64_t)w.row0 + (int64_t)tile * BN;
+                for (int dd = 0; dd < w.ndocs; dd++) {
+                    const int64_t lo_c = p.xlims[w.doc0 + dd] - trow0, hi_c = p.xlims[w.doc0 + dd + 1] - trow0;
+                    const int a = lo_c > 0 ? (int)lo_c : 0, b = hi_c < BN ? (int)hi_c : BN;
+                    float m0 = INFINITY, m1 = INFINITY;
+                    if (a < b) {
+#pragma unroll
+                        for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+                            for (int c = 0; c < 2; c++) {
+                                const int col = j * 8 + 2 * (lane & 3) + c;
+                                if (col >= a && col < b) {
+                                    float k0, k1;
+                                    if (METRIC == KB2_METRIC_L2) {
+                                        const float xx = __ldg(p.xn + trow0 + col);
+                                        k0 = qq0 + xx - 2.f * acc[4 * j + c];
+                                        k1 = qq1 + xx - 2.f * acc[4 * j + 2 + c];
+                                    } else {
+                                        k0 = -acc[4 * j + c];
+                                        k1 = -acc[4 * j + 2 + c];
+                                    }
+                                    m0 = fminf(m0, k0);
+                                    m1 = fminf(m1, k1);
+                                }
+                            }
+                        }
+                    }
+                    m0 = fminf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+                    m0 = fminf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+                    m1 = fminf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+                    m1 = fminf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+                    if ((lane & 3) == 0) {
+                        float* Rd = R + dd * BM;
+                        if (tile == 0) {
+                            Rd[rl] = m0;
+                            Rd[rl + 8] = m1;
+                        } else {
+                            Rd[rl] = fminf(Rd[rl], m0);
+                            Rd[rl + 8] = fminf(Rd[rl + 8], m1);
+                        }
+                    }
+                }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");   // R complete for this block
+            // ---- sum over the tokens of each query list (segments of the block's rows), in row order
+            const int cur = (int)(qb & 1);
+            for (int task = t; task < BM * w.ndocs; task += CONS_THREADS) {
+                const int dd = task / BM, r = task % BM;
+                const int64_t g = b0 + r;
+                if (g >= p.r1) continue;
+                const int lst = p.row_list[g];
+                if (r > 0 && p.row_list[g - 1] == lst) continue;   // not the first row of its segment
+                const int64_t lbeg = p.qlims[lst], lend = p.qlims[lst + 1];
+                float sum = (r == 0 && lbeg < b0) ? carry[(cur ^ 1) * MAXD + dd] : 0.f;
+                const int rend = lend - b0 < BM ? (int)(lend - b0) : BM;
+                for (int rr = r; rr < rend; rr++) sum += R[dd * BM + rr];
+                if (lend > b0 + BM) {
+                    carry[cur * MAXD + dd] = sum;
+                } else {
+                    const int64_t doc = (int64_t)w.doc0 + dd;
+                    if (!(p.bitset && bit_is_set(p.bitset, doc))) p.S[(lst - p.l0) * p.lds + doc] = sum;
+                }
+            }
+            // the next R / carry writes come after the first bar.sync of the next tile's contraction
+        }
+    }
+}
+
+// Exact key of (query list, document) pairs in fp32 on the CUDA cores, in the order of get_sum_max_sim: for each query
+// token in order, the extremum over the document's vectors in order (each distance an fmaf chain over the dimensions in
+// order), summed over the tokens in order.  One warp per pair; lane l owns tokens l, l + 32, ...
+//   candidates mode (cand != nullptr): pair (b, j) is the document of entry j of candidate row b (kEmpty stays kEmpty);
+//     out_cand[b][j] = (exact key, document).
+//   all-documents mode: pair (b, j) is document j; out_all[b][j] = exact key, +inf for an empty or filtered document.
+// Row b is query list qlist[b], or l0 + b.  grid = ceil(rows * per_row / 8), block 256.
+struct ExactParams {
+    const float* Q;
+    const int64_t* qlims;
+    const float* X;
+    const int64_t* xlims;
+    int d;
+    const uint8_t* bitset;
+    int64_t l0;
+    const uint32_t* qlist;
+    const uint64_t* cand;
+    uint64_t* out_cand;
+    float* out_all;
+    int64_t lda;
+    int64_t per_row;   // K (candidates) or n_docs (all documents)
+    int64_t npairs;
+};
+
+template <int METRIC, bool VEC4>
+__global__ void __launch_bounds__(256)
+maxsim_exact_kernel(const ExactParams p) {
+    const int lane = threadIdx.x & 31;
+    const int64_t pair = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (pair >= p.npairs) return;
+    const int64_t b = pair / p.per_row, j = pair % p.per_row;
+    const int64_t lst = p.qlist ? (int64_t)p.qlist[b] : p.l0 + b;
+    int64_t doc = j;
+    if (p.cand) {
+        const uint64_t e = p.cand[b * p.per_row + j];
+        if (e == kEmpty) {
+            if (lane == 0) p.out_cand[b * p.per_row + j] = kEmpty;
+            return;
+        }
+        doc = unpack_pos(e);
+    }
+    const int64_t qa = p.qlims[lst], qe = p.qlims[lst + 1];
+    const int64_t xa = p.xlims[doc], xe = p.xlims[doc + 1];
+    float total = INFINITY;
+    if (qa < qe && xa < xe && !(p.bitset && bit_is_set(p.bitset, doc))) {
+        total = 0.f;
+        for (int64_t t0 = qa; t0 < qe; t0 += kWarp) {
+            const int64_t tq = t0 + lane;
+            float ext = INFINITY;
+            if (tq < qe) {
+                const float* q = p.Q + tq * p.d;
+                for (int64_t x = xa; x < xe; x++) {
+                    const float* xr = p.X + x * p.d;
+                    float acc = 0.f;
+                    if (VEC4) {
+                        const float4* q4 = reinterpret_cast<const float4*>(q);
+                        const float4* x4 = reinterpret_cast<const float4*>(xr);
+                        for (int i = 0; i < (p.d >> 2); i++) {
+                            const float4 qv = __ldg(q4 + i), xv = __ldg(x4 + i);
+                            if (METRIC == KB2_METRIC_L2) {
+                                float df;
+                                df = qv.x - xv.x; acc = fmaf(df, df, acc);
+                                df = qv.y - xv.y; acc = fmaf(df, df, acc);
+                                df = qv.z - xv.z; acc = fmaf(df, df, acc);
+                                df = qv.w - xv.w; acc = fmaf(df, df, acc);
+                            } else {
+                                acc = fmaf(qv.x, xv.x, acc);
+                                acc = fmaf(qv.y, xv.y, acc);
+                                acc = fmaf(qv.z, xv.z, acc);
+                                acc = fmaf(qv.w, xv.w, acc);
+                            }
+                        }
+                    } else {
+                        for (int i = 0; i < p.d; i++) {
+                            const float qv = __ldg(q + i), xv = __ldg(xr + i);
+                            if (METRIC == KB2_METRIC_L2) {
+                                const float df = qv - xv;
+                                acc = fmaf(df, df, acc);
+                            } else {
+                                acc = fmaf(qv, xv, acc);
+                            }
+                        }
+                    }
+                    ext = fminf(ext, (METRIC == KB2_METRIC_L2) ? acc : -acc);
+                }
+            }
+#pragma unroll
+            for (int l = 0; l < kWarp; l++) {
+                const float v = __shfl_sync(0xffffffffu, ext, l);
+                if (t0 + l < qe) total += v;
+            }
+        }
+    }
+    if (lane != 0) return;
+    if (p.cand) p.out_cand[b * p.per_row + j] = pack_kp(total, (uint32_t)doc);
+    else p.out_all[b * p.lda + j] = total;
+}
+
+// Error bound of the filter's key of list Q against any document, from its tokens' norms and M^2 = max |x|^2 over the
+// base (DESIGN §4.10):  E = sum_t rel(d) a_t + |Q| 2^-22 sum_t a_t,  a_t = |q_t| M (IP, COSINE) or |q_t|^2 + M^2 (L2).
+// rel(d) = fin_cert_rel(d) bounds one approximate distance against its exact value as for FLAT (kb2_topk.cuh); the
+// extremum over a document is then off by at most the same, and the second term covers the fp32 sums over the tokens
+// (filter and exact kernel both: each extremum is at most 2 a_t in magnitude).
+__device__ __forceinline__ float
+maxsim_bound(float sum_a, int64_t ntok, int d) {
+    return fin_cert_rel(d) * sum_a + (float)ntok * 0x1p-22f * sum_a;
+}
+
+// Row b of a chunk (list qlist[b], or l0 + b): the k best of its K sorted (exact key, document) entries, padded with -1 and
+// the reference's values (brute_force.cc:566-581: FLT_MIN when larger is better, FLT_MAX for L2).  With `approx` (the
+// filter's selection of the row), the list is certified: when the filter kept K entries, its k-th exact key must beat the
+// largest approximate key kept by more than the bound, or the list is appended to cert[2..] (count in cert[1]) for the
+// exact all-documents redo.  grid = rows, block 256.
+struct EmitParams {
+    const uint64_t* sorted;   // [rows][K]
+    const uint64_t* approx;   // [rows][K] or nullptr
+    int K, k;
+    const float* Q;
+    const int64_t* qlims;
+    int d;
+    uint32_t* cert;           // [0] max |x|^2 (float bits), [1] count, [2..] lists to redo
+    int64_t l0;
+    const uint32_t* qlist;
+    int64_t* out_ids;
+    float* out_dist;
+};
+
+template <int METRIC>
+__global__ void __launch_bounds__(256)
+maxsim_emit_kernel(const EmitParams p) {
+    __shared__ uint32_t s_cnt, s_max;
+    __shared__ float s_a[8];
+    const int64_t b = blockIdx.x;
+    const int64_t lst = p.qlist ? (int64_t)p.qlist[b] : p.l0 + b;
+    const uint64_t* row = p.sorted + b * p.K;
+    for (int r = threadIdx.x; r < p.k; r += blockDim.x) {
+        const uint64_t e = row[r];
+        const int64_t o = lst * p.k + r;
+        if (e == kEmpty) {
+            p.out_ids[o] = -1;
+            p.out_dist[o] = (METRIC == KB2_METRIC_L2) ? FLT_MAX : FLT_MIN;
+        } else {
+            const float key = unpack_key(e);
+            p.out_ids[o] = (int64_t)unpack_pos(e);
+            p.out_dist[o] = (METRIC == KB2_METRIC_L2) ? key : -key;
+        }
+    }
+    if (!p.approx) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) { s_cnt = 0; s_max = 0; }
+    __syncthreads();
+    uint32_t cnt = 0, mx = 0;
+    for (int j = threadIdx.x; j < p.K; j += blockDim.x) {
+        const uint64_t e = p.approx[b * p.K + j];
+        if (e != kEmpty) { cnt++; mx = max(mx, (uint32_t)(e >> 32)); }
+    }
+    atomicAdd(&s_cnt, cnt);
+    atomicMax(&s_max, mx);
+    const float M2 = __uint_as_float(p.cert[0]);
+    const int64_t qa = p.qlims[lst], qe = p.qlims[lst + 1];
+    float a = 0.f;
+    for (int64_t tq = qa + warp; tq < qe; tq += 8) {
+        float s = 0.f;
+        for (int i = lane; i < p.d; i += kWarp) s = fmaf(p.Q[tq * p.d + i], p.Q[tq * p.d + i], s);
+        s = warp_sum(s);
+        a += (METRIC == KB2_METRIC_L2) ? s + M2 : sqrtf(s * M2);
+    }
+    if (lane == 0) s_a[warp] = a;
+    __syncthreads();
+    if (threadIdx.x != 0 || s_cnt < (uint32_t)p.K) return;   // fewer than K documents scored: nothing was cut
+    float sum_a = 0.f;
+    for (int w = 0; w < 8; w++) sum_a += s_a[w];
+    const float E = maxsim_bound(sum_a * 1.0001f, qe - qa, p.d);
+    const float kth = unpack_key(row[p.k - 1]);
+    const float last = ord2f(s_max);
+    if (kth <= last - E) return;
+    p.cert[2 + atomicAdd(p.cert + 1, 1u)] = (uint32_t)lst;
+}
+
+// Scratch of one emb-list search, reused across calls (per-device BruteForce slot).
+struct Scratch {
+    DevBuf<int64_t> xlims, qlims;
+    DevBuf<int32_t> row_list, seg_off;
+    DevBuf<Item> items;
+    DevBuf<uint64_t> cand, exact, sorted;
+    DevBuf<uint8_t> bits, sort_tmp;
+};
+
+// Work items from the base offsets: consecutive documents packed greedily into one 128-row tile (at most MAXD of them),
+// and each document longer than a tile alone over consecutive tiles.  Empty documents are never scored.
+inline std::vector<Item>
+plan_items(const std::vector<int64_t>& xl) {
+    std::vector<Item> items;
+    const int64_t n_docs = (int64_t)xl.size() - 1;
+    bool open = false;
+    Item cur{};
+    int64_t used = 0;
+    auto close = [&] {
+        if (open) items.push_back(cur);
+        open = false;
+    };
+    for (int64_t j = 0; j < n_docs; j++) {
+        const int64_t len = xl[j + 1] - xl[j];
+        if (len > BN) {
+            close();
+            items.push_back(Item{(int32_t)xl[j], (int32_t)((len + BN - 1) / BN), (int32_t)j, 1});
+            continue;
+        }
+        if (open && (used + len > BN || cur.ndocs == MAXD)) close();
+        if (!open) {
+            if (len == 0) continue;
+            cur = Item{(int32_t)xl[j], 1, (int32_t)j, 0};
+            used = 0;
+            open = true;
+        }
+        cur.ndocs++;
+        used += len;
+    }
+    close();
+    return items;
+}
+
+// The search.  fi holds the base (fi.base, fi.norms = |x|^2, rows normalised for COSINE) and the stream; dq: device query
+// rows (normalised for COSINE); xl / ql: validated host offsets; dbits: device bitset over documents or nullptr; d_ids /
+// d_dist: device [n_lists][k].  metric: KB2_METRIC_L2 or KB2_METRIC_IP.  stats: lists, candidate slots re-ranked, lists
+// scored exactly over all documents.
+inline void
+search(FlatIndex& fi, Scratch& sc, const float* dq, const std::vector<int64_t>& xl, const std::vector<int64_t>& ql, int d,
+       int metric, int k, const uint8_t* dbits, int64_t* d_ids, float* d_dist, int64_t stats[3]) {
+    cudaStream_t st = fi.stream;
+    const int64_t n_docs = (int64_t)xl.size() - 1, n_lists = (int64_t)ql.size() - 1;
+    const int64_t nb = xl.back(), nq_rows = ql.back();
+    const float* X = fi.base.p;
+    const float* xn = fi.norms.p;
+    sc.xlims.ensure(xl.size());
+    sc.qlims.ensure(ql.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.xlims.p, xl.data(), xl.size() * 8, cudaMemcpyHostToDevice, st));
+    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.qlims.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice, st));
+    std::vector<int32_t> row_list((size_t)std::max<int64_t>(nq_rows, 1));
+    for (int64_t l = 0; l < n_lists; l++)
+        for (int64_t r = ql[l]; r < ql[l + 1]; r++) row_list[r] = (int32_t)l;
+    sc.row_list.ensure(row_list.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.row_list.p, row_list.data(), row_list.size() * 4, cudaMemcpyHostToDevice, st));
+    fi.s_qn.ensure(std::max<int64_t>(nq_rows, 1));
+    if (metric == KB2_METRIC_L2 && nq_rows > 0)
+        row_norms_kernel<<<grid1d(nq_rows * 32, 256), 256, 0, st>>>(dq, nq_rows, d, fi.s_qn.p);
+    fi.s_cert.ensure((size_t)n_lists + 2);
+    KB2_CUDA_CHECK(cudaMemsetAsync(fi.s_cert.p, 0, 8, st));
+    pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, st>>>(xn, nb, fi.s_cert.p);
+
+    CUtensorMap tq, tx;
+    const bool use_tc = nq_rows > 0 && tc::make_tmap(&tq, dq, nq_rows, d) && tc::make_tmap(&tx, X, nb, d);
+    std::vector<Item> items;
+    if (use_tc) {
+        items = plan_items(xl);
+        sc.items.ensure(std::max<size_t>(items.size(), 1));
+        if (!items.empty())
+            KB2_CUDA_CHECK(cudaMemcpyAsync(sc.items.p, items.data(), items.size() * sizeof(Item), cudaMemcpyHostToDevice, st));
+    }
+    const int K = k + 16;
+    const int64_t lds = round_up(n_docs, 4);
+    // lists per chunk: S within the 256 MB key budget of dense_candidates, candidates within the large-k scratch
+    const int64_t L = std::max<int64_t>(1, std::min<int64_t>({n_lists, (64ll << 20) / lds, large_k_group(n_lists, (int64_t)K * 24 + 16)}));
+    fi.s_keys.ensure((size_t)L * lds);
+    sc.cand.ensure((size_t)L * K);
+    sc.exact.ensure((size_t)L * K);
+    sc.sorted.ensure((size_t)L * K);
+    sc.seg_off.ensure((size_t)L + 1);
+    segment_offsets_kernel<<<grid1d(L + 1, 256), 256, 0, st>>>(sc.seg_off.p, L, K);
+    size_t tmp_bytes = 0;
+    cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, sc.exact.p, sc.sorted.p, (int)(L * K), (int)L, sc.seg_off.p,
+                                            sc.seg_off.p + 1, 0, 64, st);
+    sc.sort_tmp.ensure(tmp_bytes);
+    const bool vec4 = (d & 3) == 0 && (reinterpret_cast<uintptr_t>(dq) & 15) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
+
+    auto exact = [&](const uint64_t* cand, int64_t rows, int64_t l0, const uint32_t* qlist) {
+        ExactParams ep{dq, sc.qlims.p, X, sc.xlims.p, d, dbits, l0, qlist, cand, sc.exact.p, fi.s_keys.p, lds,
+                       cand ? (int64_t)K : n_docs, 0};
+        ep.npairs = rows * ep.per_row;
+        if (ep.npairs == 0) return;
+        const unsigned grid = (unsigned)((ep.npairs + 7) / 8);
+        with_metric(metric, [&](auto m) {
+            if (vec4) maxsim_exact_kernel<decltype(m)::value, true><<<grid, 256, 0, st>>>(ep);
+            else maxsim_exact_kernel<decltype(m)::value, false><<<grid, 256, 0, st>>>(ep);
+        });
+        fi.last.launches++;
+        KB2_CUDA_CHECK(cudaGetLastError());
+    };
+    // sort the K entries of each row by (key, document) and emit the rows
+    auto sort_emit = [&](const uint64_t* in, int64_t rows, int64_t l0, const uint32_t* qlist, const uint64_t* approx) {
+        size_t bytes = tmp_bytes;
+        KB2_CUDA_CHECK(cub::DeviceSegmentedRadixSort::SortKeys(sc.sort_tmp.p, bytes, in, sc.sorted.p, (int)(rows * K), (int)rows,
+                                                               sc.seg_off.p, sc.seg_off.p + 1, 0, 64, st));
+        EmitParams pp{sc.sorted.p, approx, K, k, dq, sc.qlims.p, d, fi.s_cert.p, l0, qlist, d_ids, d_dist};
+        with_metric(metric, [&](auto m) { maxsim_emit_kernel<decltype(m)::value><<<(unsigned)rows, 256, 0, st>>>(pp); });
+        fi.last.launches += 2;
+        KB2_CUDA_CHECK(cudaGetLastError());
+    };
+    // exact keys of every document for `rows` lists -> their K best -> sorted, emitted
+    auto exact_all = [&](int64_t rows, int64_t l0, const uint32_t* qlist) {
+        exact(nullptr, rows, l0, qlist);
+        large_k_select<float>(fi, fi.s_keys.p, lds, n_docs, 0u, K, sc.cand.p, K, rows);
+        sort_emit(sc.cand.p, rows, l0, qlist, nullptr);
+    };
+
+    int64_t n_exact = 0;
+    for (int64_t l0 = 0; l0 < n_lists; l0 += L) {
+        const int64_t rows = std::min(L, n_lists - l0);
+        if (!use_tc) {
+            exact_all(rows, l0, nullptr);
+            n_exact += rows;
+            continue;
+        }
+        pqtc::fill_f32_kernel<<<grid1d(rows * lds, 256), 256, 0, st>>>(fi.s_keys.p, rows * lds, INFINITY);
+        FilterParams fp{sc.items.p, (int)items.size(), sc.xlims.p, sc.qlims.p, sc.row_list.p, fi.s_qn.p, xn,
+                        ql[l0], ql[l0 + rows], l0, d, dbits, fi.s_keys.p, lds};
+        if (fp.r1 > fp.r0 && fp.nitems > 0) {
+            const unsigned grid = (unsigned)std::min<int64_t>(num_sms(), fp.nitems);
+            with_metric(metric, [&](auto m) {
+                launch<maxsim_filter_kernel<decltype(m)::value>>(grid, tc::THREADS, SMEM_BYTES, st, tq, tx, fp);
+            });
+            fi.last.launches++;
+            KB2_CUDA_CHECK(cudaGetLastError());
+        }
+        large_k_select<float>(fi, fi.s_keys.p, lds, n_docs, 0u, K, sc.cand.p, K, rows);
+        exact(sc.cand.p, rows, l0, nullptr);
+        sort_emit(sc.exact.p, rows, l0, nullptr, sc.cand.p);
+        stats[1] += rows * K;
+    }
+    int64_t nredo = 0;
+    if (use_tc && n_lists > 0) {
+        uint32_t* hc = (uint32_t*)fi.h_counter.p;
+        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, fi.s_cert.p + 1, 4, cudaMemcpyDeviceToHost, st));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+        nredo = hc[0];
+        for (int64_t r0 = 0; r0 < nredo; r0 += L) exact_all(std::min(L, nredo - r0), 0, fi.s_cert.p + 2 + r0);
+    }
+    stats[0] += n_lists;
+    stats[2] += n_exact + nredo;
+}
+
+}  // namespace msim
+}  // namespace kb2
