@@ -86,6 +86,11 @@ def _declare(L):
                                               c.POINTER(vp), c.POINTER(vp), c.POINTER(vp), i32, vp]
     L.kb2_bruteforce_search_emb_list.argtypes = [vp, vp, i64, i32, i32, vp, vp, i64, i32, vp, i64, vp, vp, vp, i32, vp]
     L.kb2_merge_topk.argtypes = [i32, i32, i64, i32, vp, vp, vp, vp, i32, vp]
+    L.kb2_index_set_emb_list.argtypes = [vp, vp, i64, i32]
+    L.kb2_index_emb_list_offsets.argtypes = [vp, vp, vp]
+    L.kb2_index_search_emb_list.argtypes = [vp, vp, vp, i64, i32, c.c_char_p, vp, i64, vp, vp, vp]
+    L.kb2_index_emb_list_stage_ms.argtypes = [vp, vp]
+    L.kb2_debug_maxsim_pairs.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, i32, vp, vp, i32]
     if hasattr(L, "kb2_faiss_describe"):
         L.kb2_faiss_describe.argtypes = [vp, c.c_size_t, i32, vp, c.c_size_t]
         L.kb2_faiss_rewrite.argtypes = [vp, c.c_size_t, i32, c.POINTER(vp), c.POINTER(c.c_size_t)]
@@ -334,6 +339,49 @@ class Index:
         _check(self.L.kb2_index_get_meta(self.h, ctypes.cast(buf, ctypes.c_void_p), 1024))
         return json.loads(buf.value.decode())
 
+    # -- emb-lists (multi-vector documents) on HNSW / IVF_FLAT: the reference's TokenANN strategy (DESIGN §4.11)
+    def set_emb_list(self, lims, metric):
+        """attach document offsets (int64 [n_docs + 1], ending at count()) and the MAX_SIM metric that pairs with the
+        index metric (MAX_SIM_L2 - L2, MAX_SIM_IP - IP, MAX_SIM / MAX_SIM_COSINE - COSINE)"""
+        lims = lims if _is_torch(lims) else np.ascontiguousarray(lims, np.int64)
+        _check(self.L.kb2_index_set_emb_list(self.h, _ptr(lims), int(lims.shape[0]) - 1,
+                                             _EMB_METRICS.get(str(metric).upper(), -1)))
+
+    def emb_list_offsets(self):
+        n = ctypes.c_int64()
+        _check(self.L.kb2_index_emb_list_offsets(self.h, ctypes.byref(n), None))
+        lims = np.empty(n.value + 1, np.int64)
+        _check(self.L.kb2_index_emb_list_offsets(self.h, ctypes.byref(n), _ptr(lims)))
+        return lims
+
+    def search_emb_list(self, q, q_lims, k, config=None, bitset=None, stats=False):
+        """q: [rows, dim] float32 query tokens, q_lims: int64 [n_lists + 1] (numpy or CUDA tensors).  Returns (ids, dist)
+        [n_lists, k] (CUDA tensors when q is), documents best first; with stats=True also int64 [query lists,
+        candidates re-ranked, token x row distances].  config: retrieval_ann_ratio (default 3) and the base search keys;
+        bitset: one bit per document."""
+        if not _is_torch(q_lims):
+            q_lims = np.ascontiguousarray(q_lims, np.int64)
+        n_lists = int(q_lims.shape[0]) - 1
+        if _is_torch(q) and q.is_cuda:
+            import torch
+            ids = torch.empty((n_lists, k), dtype=torch.int64, device=q.device)
+            dist = torch.empty((n_lists, k), dtype=torch.float32, device=q.device)
+        else:
+            ids = np.empty((n_lists, k), np.int64)
+            dist = np.empty((n_lists, k), np.float32)
+        st = np.zeros(3, np.int64)
+        nbits = 0 if bitset is None else (bitset.numel() if _is_torch(bitset) else bitset.size) * 8
+        _check(self.L.kb2_index_search_emb_list(self.h, _ptr(q), _ptr(q_lims), n_lists, k, _cfg(config), _ptr(bitset),
+                                                nbits, _ptr(ids), _ptr(dist), _ptr(st)))
+        return (ids, dist, st) if stats else (ids, dist)
+
+    def emb_list_stage_ms(self):
+        """device ms of the last search_emb_list's stages (with enable_kernel_timing): stage 1, candidates, re-rank,
+        select"""
+        v = np.zeros(4, np.float32)
+        _check(self.L.kb2_index_emb_list_stage_ms(self.h, _ptr(v)))
+        return dict(stage1=float(v[0]), candidates=float(v[1]), rerank=float(v[2]), select=float(v[3]))
+
     # -- introspection for bench.py
     def last_counters(self):
         c = np.zeros(8, np.int64)
@@ -476,6 +524,22 @@ def brute_force_search_emb_list(base, base_lims, queries, query_lims, k, metric=
                                             n_lists, k, _ptr(bitset), nbits, _ptr(ids), _ptr(dist), _ptr(st), device,
                                             ctypes.c_void_p(stream)))
     return (ids, dist, st) if stats else (ids, dist)
+
+
+def debug_maxsim_pairs(queries, query_lims, base, base_lims, pair_lims, pair_docs, metric="L2", use_rerank=True,
+                       device=0):
+    """validation hook (kb2_debug_maxsim_pairs): exact MaxSim scores of the (list, document) pairs pair_docs[pair_lims[l]
+    : pair_lims[l+1]] by the index re-rank kernel or the BruteForce one.  queries / base / pair_docs (int32): CUDA
+    tensors; offsets: numpy int64.  Returns (scores CUDA tensor [pairs], kernel ms)."""
+    import torch
+    L = lib()
+    ql, xl, pl = (np.ascontiguousarray(a, np.int64) for a in (query_lims, base_lims, pair_lims))
+    out = torch.empty(max(int(pl[-1]), 1), dtype=torch.float32, device=queries.device)
+    ms = ctypes.c_float()
+    _check(L.kb2_debug_maxsim_pairs(_ptr(queries), _ptr(ql), len(ql) - 1, _ptr(base), _ptr(xl), len(xl) - 1,
+                                    base.shape[1], _METRICS[metric], _ptr(pl), _ptr(pair_docs), 1 if use_rerank else 0,
+                                    _ptr(out), ctypes.byref(ms), device))
+    return out[:int(pl[-1])], ms.value
 
 
 def brute_force_range_search(base, queries, radius, range_filter=None, metric="L2", bitset=None, device=0):

@@ -258,6 +258,7 @@ kb2_index_train_typed(kb2_index_t h, const void* x, int dtype, int64_t n) {
         std::lock_guard<std::mutex> lk(ix->mu);
         KB2_CUDA_CHECK(cudaSetDevice(ix->device));
         KB2_REQUIRE(x != nullptr || n == 0, KB2_INVALID_ARGS, "null training data");
+        KB2_REQUIRE(!ix->emb_list, KB2_NOT_IMPLEMENTED, "Train on an emb-list index");
         ix->wait_caller_work();
         const float* xf = widen_to_f32(ix, x, dtype, n * ix->dim);
         ix->train(ix->cosine ? ix->normalized(xf, n) : xf, n);
@@ -275,6 +276,7 @@ kb2_index_add_typed(kb2_index_t h, const void* x, int dtype, int64_t n, const in
         std::lock_guard<std::mutex> lk(ix->mu);
         KB2_CUDA_CHECK(cudaSetDevice(ix->device));
         KB2_REQUIRE(x != nullptr || n == 0, KB2_INVALID_ARGS, "null data");
+        KB2_REQUIRE(!ix->emb_list, KB2_NOT_IMPLEMENTED, "AddEmbList is not implemented: rows cannot be added to an emb-list index");
         ix->wait_caller_work();
         const float* xf = widen_to_f32(ix, x, dtype, n * ix->dim);
         ix->add(ix->cosine ? ix->normalized(xf, n) : xf, n, ids);
@@ -293,6 +295,7 @@ kb2_index_search_typed(kb2_index_t h, const void* queries, int dtype, int64_t nq
         std::lock_guard<std::mutex> lk(ix->mu);
         KB2_CUDA_CHECK(cudaSetDevice(ix->device));
         KB2_REQUIRE(nq >= 0 && k > 0, KB2_INVALID_ARGS, "bad nq / k");
+        KB2_REQUIRE(!ix->emb_list, KB2_EMB_LIST_INNER_ERROR, "emb-list index: search with query list offsets (kb2_index_search_emb_list)");
         if (nq == 0) return;
         KB2_REQUIRE(queries && out_ids && out_dist, KB2_INVALID_ARGS, "null buffer");
         KB2_REQUIRE(is_device_ptr(out_ids) == is_device_ptr(out_dist), KB2_INVALID_ARGS,
@@ -320,6 +323,7 @@ kb2_index_range_search(kb2_index_t h, const float* queries, int64_t nq, float ra
         std::lock_guard<std::mutex> lk(ix->mu);
         KB2_CUDA_CHECK(cudaSetDevice(ix->device));
         KB2_REQUIRE(out_lims && out_ids && out_dist, KB2_INVALID_ARGS, "null output");
+        KB2_REQUIRE(!ix->emb_list, KB2_EMB_LIST_INNER_ERROR, "RangeSearch is not supported on an emb-list index");
         JsonObj cfg = JsonObj::parse(json);
         KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
         ix->last = Counters{};
@@ -373,6 +377,7 @@ kb2_ivf_import_begin(kb2_index_t h, int64_t nlist, const float* centroids, const
         auto* iv = ix_as<IvfIndex>(h, "IVF");
         std::lock_guard<std::mutex> lk(iv->mu);
         KB2_CUDA_CHECK(cudaSetDevice(iv->device));
+        KB2_REQUIRE(!iv->emb_list, KB2_NOT_IMPLEMENTED, "import into an emb-list index");
         iv->import_begin(nlist, centroids, pq_centroids);
     });
 }
@@ -381,6 +386,7 @@ kb2_ivf_import_list(kb2_index_t h, int64_t list_no, int64_t list_size, const int
     return guarded([&] {
         auto* iv = ix_as<IvfIndex>(h, "IVF");
         std::lock_guard<std::mutex> lk(iv->mu);
+        KB2_REQUIRE(!iv->emb_list, KB2_NOT_IMPLEMENTED, "import into an emb-list index");
         if (list_size > 0) iv->import_list(list_no, list_size, ids, codes);
     });
 }
@@ -390,6 +396,7 @@ kb2_ivf_import_finish(kb2_index_t h, const float* raw, int64_t n_raw) {
         auto* iv = ix_as<IvfIndex>(h, "IVF");
         std::lock_guard<std::mutex> lk(iv->mu);
         KB2_CUDA_CHECK(cudaSetDevice(iv->device));
+        KB2_REQUIRE(!iv->emb_list, KB2_NOT_IMPLEMENTED, "import into an emb-list index");
         iv->import_finish(raw, n_raw);
     });
 }
@@ -443,6 +450,8 @@ kb2_hnsw_import(kb2_index_t h, int64_t n, const float* vectors, const int32_t* l
         auto* hn = ix_as<HnswIndex>(h, "HNSW");
         std::lock_guard<std::mutex> lk(hn->mu);
         KB2_CUDA_CHECK(cudaSetDevice(hn->device));
+        // the attached document offsets and doc_of_row describe the current rows
+        KB2_REQUIRE(!hn->emb_list, KB2_NOT_IMPLEMENTED, "import into an emb-list index");
         hn->import_graph(n, vectors, levels, offsets, neighbors, cum_nneighbor, n_cum, entry_point, max_level);
     });
 }
@@ -899,6 +908,182 @@ kb2_bruteforce_search_emb_list(const float* base, const int64_t* base_lims, int6
         fi.base.release();
         fi.n_used = 0;
         if (out_stats) memcpy(out_stats, stats, sizeof(stats));
+    });
+}
+
+// ---------------------------------------------------------------- emb-list search on an index (TokenANN)
+int
+kb2_index_set_emb_list(kb2_index_t h, const int64_t* lims, int64_t n_docs, int metric) {
+    return guarded([&] {
+        IndexBase* ix = ix_of(h);
+        std::lock_guard<std::mutex> lk(ix->mu);
+        KB2_CUDA_CHECK(cudaSetDevice(ix->device));
+        KB2_REQUIRE(lims != nullptr && n_docs >= 1, KB2_INVALID_ARGS, "emb-list offsets: null, or no document");
+        set_emb_list(*ix, read_lims(lims, n_docs, "document"), metric);
+    });
+}
+int
+kb2_index_emb_list_offsets(kb2_index_t h, int64_t* n_docs, int64_t* lims) {
+    return guarded([&] {
+        IndexBase* ix = ix_of(h);
+        std::lock_guard<std::mutex> lk(ix->mu);
+        KB2_REQUIRE(n_docs != nullptr, KB2_INVALID_ARGS, "null argument");
+        KB2_REQUIRE(ix->emb_list != nullptr, KB2_INVALID_ARGS, "the index has no emb-list offsets");
+        *n_docs = ix->emb_list->n_docs();
+        if (lims) memcpy(lims, ix->emb_list->lims.data(), ix->emb_list->lims.size() * 8);
+    });
+}
+int
+kb2_index_search_emb_list(kb2_index_t h, const float* queries, const int64_t* query_lims, int64_t n_lists, int k,
+                          const char* json, const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids, float* out_dist,
+                          int64_t* out_stats) {
+    return guarded([&] {
+        IndexBase* ix = ix_of(h);
+        std::lock_guard<std::mutex> lk(ix->mu);
+        KB2_CUDA_CHECK(cudaSetDevice(ix->device));
+        // index_node.cc:275-297: a query with list offsets needs an emb-list index
+        KB2_REQUIRE(ix->emb_list != nullptr, KB2_EMB_LIST_INNER_ERROR, "the index has no emb-list offsets (kb2_index_set_emb_list)");
+        KB2_REQUIRE(query_lims && out_ids && out_dist && n_lists >= 0, KB2_INVALID_ARGS, "null buffer or bad list count");
+        KB2_REQUIRE(k > 0 && k <= kMaxLargeK, KB2_INVALID_ARGS, "k out of range (1..16384)");
+        KB2_REQUIRE(is_device_ptr(out_ids) == is_device_ptr(out_dist), KB2_INVALID_ARGS,
+                    "out_ids and out_dist must both be host or both be device buffers");
+        JsonObj cfg = JsonObj::parse(json);
+        KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
+        if (out_stats) out_stats[0] = out_stats[1] = out_stats[2] = 0;
+        const std::vector<int64_t> ql = read_lims(query_lims, n_lists, "query");
+        KB2_REQUIRE(ql.back() < (1ll << 31), KB2_INVALID_ARGS, "emb-list sizes out of range (query rows < 2^31)");
+        KB2_REQUIRE(queries || ql.back() == 0, KB2_INVALID_ARGS, "null queries");
+        ix->last = Counters{};
+        ix->wait_caller_work();
+        int64_t stats[3] = {0, 0, 0};
+        search_emb_list(*ix, queries, ql, k, cfg, bitset, bitset_nbits, out_ids, out_dist, stats);
+        if (out_stats) memcpy(out_stats, stats, sizeof(stats));
+    });
+}
+int
+kb2_index_emb_list_stage_ms(kb2_index_t h, float* out4) {
+    return guarded([&] {
+        IndexBase* ix = ix_of(h);
+        std::lock_guard<std::mutex> lk(ix->mu);
+        KB2_REQUIRE(out4 != nullptr && ix->emb_list != nullptr, KB2_INVALID_ARGS, "null argument or no emb-list offsets");
+        memcpy(out4, ix->emb_list->stage_ms, sizeof(ix->emb_list->stage_ms));
+    });
+}
+
+namespace {
+__global__ void
+pairs_to_scores_kernel(const uint64_t* e, int64_t n, int metric, float* out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float key = unpack_key(e[i]);
+    out[i] = metric == KB2_METRIC_L2 ? key : -key;
+}
+__global__ void
+pairs_pad_kernel(const int64_t* pl, const int32_t* docs, int64_t n_lists, int64_t K, uint64_t* cand) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_lists * K) return;
+    const int64_t l = i / K, j = i % K;
+    cand[i] = pl[l] + j < pl[l + 1] ? (uint64_t)(uint32_t)docs[pl[l] + j] : kEmpty;
+}
+// documents -> candidate entries; flags[0] = 1 when a document is outside [0, n_docs)
+__global__ void
+pairs_widen_kernel(const int32_t* docs, int64_t n, int64_t n_docs, uint64_t* cand, int* flags) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int32_t d = docs[i];
+    if (d < 0 || d >= n_docs) flags[0] = 1;
+    cand[i] = (uint64_t)(uint32_t)(d < 0 || d >= n_docs ? 0 : d);
+}
+__global__ void
+pairs_unpad_kernel(const int64_t* pl, const uint64_t* in, int64_t n_lists, int64_t K, uint64_t* out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_lists * K) return;
+    const int64_t l = i / K, j = i % K;
+    if (pl[l] + j < pl[l + 1]) out[pl[l] + j] = in[i];
+}
+}  // namespace
+
+int
+kb2_debug_maxsim_pairs(const float* queries, const int64_t* query_lims, int64_t n_lists, const float* base,
+                       const int64_t* base_lims, int64_t n_docs, int dim, int metric, const int64_t* pair_lims,
+                       const int32_t* pair_docs, int use_rerank, float* out_scores, float* out_ms, int device) {
+    return guarded([&] {
+        require_device(device);
+        KB2_REQUIRE(queries && base && pair_docs && out_scores && query_lims && base_lims && pair_lims, KB2_INVALID_ARGS, "null buffer");
+        KB2_REQUIRE(is_device_ptr(queries) && is_device_ptr(base) && is_device_ptr(pair_docs) && is_device_ptr(out_scores),
+                    KB2_INVALID_ARGS, "debug_maxsim_pairs takes device rows, documents and scores");
+        KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP, KB2_INVALID_METRIC_TYPE, "metric must be L2 or IP");
+        KB2_REQUIRE(n_lists >= 1 && n_docs >= 1 && dim > 0, KB2_INVALID_ARGS, "bad sizes");
+        const std::vector<int64_t> ql = read_lims(query_lims, n_lists, "query");
+        const std::vector<int64_t> xl = read_lims(base_lims, n_docs, "base");
+        const std::vector<int64_t> pl = read_lims(pair_lims, n_lists, "pair");
+        const int64_t np = pl.back();
+        int64_t K = 1;
+        for (int64_t l = 0; l < n_lists; l++) K = std::max(K, pl[l + 1] - pl[l]);
+        DevBuf<int64_t> dql, dxl, dpl;
+        DevBuf<uint64_t> cand, out, tmp;
+        DevBuf<msim::RerankItem> items;
+        DevBuf<int32_t> cnt, off;
+        DevBuf<unsigned long long> stats;
+        dql.ensure(ql.size());
+        dxl.ensure(xl.size());
+        dpl.ensure(pl.size());
+        KB2_CUDA_CHECK(cudaMemcpy(dql.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice));
+        KB2_CUDA_CHECK(cudaMemcpy(dxl.p, xl.data(), xl.size() * 8, cudaMemcpyHostToDevice));
+        KB2_CUDA_CHECK(cudaMemcpy(dpl.p, pl.data(), pl.size() * 8, cudaMemcpyHostToDevice));
+        out.ensure(std::max<int64_t>(np, 1));
+        // the documents must be valid before either kernel reads their offsets
+        tmp.ensure(std::max<int64_t>(np, 1));
+        DevBuf<int> flags;
+        flags.ensure(1);
+        KB2_CUDA_CHECK(cudaMemset(flags.p, 0, 4));
+        if (np) pairs_widen_kernel<<<grid1d(np, 256), 256>>>(pair_docs, np, n_docs, tmp.p, flags.p);
+        int bad = 0;
+        KB2_CUDA_CHECK(cudaMemcpy(&bad, flags.p, 4, cudaMemcpyDeviceToHost));
+        KB2_REQUIRE(!bad, KB2_INVALID_ARGS, "pair documents must lie in [0, n_docs)");
+        cudaEvent_t e0, e1;
+        KB2_CUDA_CHECK(cudaEventCreate(&e0));
+        KB2_CUDA_CHECK(cudaEventCreate(&e1));
+        const bool vec4 = (dim & 3) == 0 && (reinterpret_cast<uintptr_t>(queries) & 15) == 0 && (reinterpret_cast<uintptr_t>(base) & 15) == 0;
+        if (use_rerank) {
+            // the candidate CSR is the pair CSR (tmp: documents in the low 32 bits)
+            cnt.ensure(n_lists + 1);
+            off.ensure(n_lists + 1);
+            stats.ensure(2);
+            KB2_CUDA_CHECK(cudaMemset(stats.p, 0, 16));
+            msim::rerank_plan_kernel<<<grid1d(n_lists, 128), 128>>>(dpl.p, tmp.p, dxl.p, dql.p, 0, n_lists, cnt.p, nullptr, nullptr, stats.p);
+            std::vector<int32_t> hcnt(n_lists), hoff(n_lists + 1, 0);
+            KB2_CUDA_CHECK(cudaMemcpy(hcnt.data(), cnt.p, n_lists * 4, cudaMemcpyDeviceToHost));
+            for (int64_t l = 0; l < n_lists; l++) hoff[l + 1] = hoff[l] + hcnt[l];
+            KB2_CUDA_CHECK(cudaMemcpy(off.p, hoff.data(), (n_lists + 1) * 4, cudaMemcpyHostToDevice));
+            items.ensure(std::max<int32_t>(hoff[n_lists], 1));
+            msim::rerank_plan_kernel<<<grid1d(n_lists, 128), 128>>>(dpl.p, tmp.p, dxl.p, dql.p, 0, n_lists, nullptr, off.p, items.p, nullptr);
+            const msim::RerankParams rp{queries, dql.p, base, nullptr, dxl.p, dim, 0, items.p, tmp.p, out.p};
+            KB2_CUDA_CHECK(cudaEventRecord(e0));
+            if (hoff[n_lists] > 0)
+                with_metric(metric, [&](auto m) { msim::launch_rerank<decltype(m)::value>(vec4, (unsigned)hoff[n_lists], 0, rp); });
+            KB2_CUDA_CHECK(cudaEventRecord(e1));
+        } else {
+            cand.ensure((size_t)n_lists * K);
+            pairs_pad_kernel<<<grid1d(n_lists * K, 256), 256>>>(dpl.p, pair_docs, n_lists, K, cand.p);
+            tmp.ensure((size_t)n_lists * K);
+            msim::ExactParams ep{queries, dql.p, base, dxl.p, dim, nullptr, 0, nullptr, cand.p, tmp.p, nullptr, 0, K, n_lists * K};
+            KB2_CUDA_CHECK(cudaEventRecord(e0));
+            with_metric(metric, [&](auto m) {
+                if (vec4) msim::maxsim_exact_kernel<decltype(m)::value, true><<<(unsigned)((ep.npairs + 7) / 8), 256>>>(ep);
+                else msim::maxsim_exact_kernel<decltype(m)::value, false><<<(unsigned)((ep.npairs + 7) / 8), 256>>>(ep);
+            });
+            KB2_CUDA_CHECK(cudaEventRecord(e1));
+            pairs_unpad_kernel<<<grid1d(n_lists * K, 256), 256>>>(dpl.p, tmp.p, n_lists, K, out.p);
+        }
+        KB2_CUDA_CHECK(cudaGetLastError());
+        if (np) pairs_to_scores_kernel<<<grid1d(np, 256), 256>>>(out.p, np, metric, out_scores);
+        KB2_CUDA_CHECK(cudaDeviceSynchronize());
+        float ms = 0.f;
+        KB2_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+        cudaEventDestroy(e0);
+        cudaEventDestroy(e1);
+        if (out_ms) *out_ms = ms;
     });
 }
 

@@ -1,0 +1,331 @@
+// kb2_emb_list_index.cuh — emb-list (multi-vector) search on an HNSW or IVF_FLAT index with the MAX_SIM metrics: the
+// reference's TokenANN strategy (src/index/emb_list/emb_list_strategy_token_ann.cc:51-175,
+// emb_list_strategy.cc:45-117, index_node.cc:275-324,453-507).  DESIGN §4.11.
+//
+// The base index holds every row of every document; the document offsets are attached afterwards (set_emb_list), and
+// doc_of_row maps each row to its document on the device.  A search runs over chunks of whole query lists:
+//   0. (bitset) row_bits_kernel expands the document bitset into a row bitset, so the base search, its kAlpha and its
+//      brute-force thresholds all see row counts, as the reference does;
+//   1. stage 1: the handle's own search() of every query token with k = vec_topk = min(max(int(k * ratio), 1), rows);
+//      HNSW checks ef >= k against the list-level k and searches with max(ef, vec_topk);
+//   2. candidates: cand_keys_kernel maps each stage-1 id to (list << 32) | document, one radix sort and one unique pass
+//      compact them, and cand_off_kernel finds each list's run: a CSR of distinct documents per list, ascending;
+//   3. re-rank: rerank_plan_kernel packs each list's candidates into work items and msim::maxsim_rerank_kernel computes
+//      their exact MaxSim keys, bit-identical to the BruteForce re-rank (kb2_maxsim.cuh);
+//   4. select: a segmented radix sort orders each list's (key, document) entries and el_emit_kernel writes the k best,
+//      padded with id -1 and -FLT_MAX (larger is better) or FLT_MAX (MAX_SIM_L2), as emb_list_strategy.cc:111-114.
+// Ties in the score are ordered by ascending document id (the reference's order follows unordered_set iteration).
+#pragma once
+#include <cub/cub.cuh>
+
+#include "kb2_hnsw.cuh"
+#include "kb2_maxsim.cuh"
+
+namespace kb2 {
+
+constexpr uint32_t kEmbListTag = 0x54534c45;   // "ELST": emb-list section of a "KB2I" blob (kb2_range.cuh)
+// 36 bytes of stage-1 and candidate scratch per (token, vec_topk) entry: at most this many entries per chunk of lists
+constexpr int64_t kEmbListChunkEntries = 8ll << 20;
+
+struct EmbListState {
+    int metric = KB2_METRIC_MAX_SIM_L2;   // KB2_METRIC_MAX_SIM_*
+    std::vector<int64_t> lims;            // [n_docs + 1] document offsets (host)
+    DevBuf<int64_t> d_lims;
+    DevBuf<int32_t> doc_of_row;
+    // per-search scratch (grow-only)
+    DevBuf<float> q, s1_dist;
+    DevBuf<int64_t> qlims, s1_ids, cand_off;
+    DevBuf<int32_t> row_list, item_cnt, item_off;
+    DevBuf<uint64_t> keys, keys_sorted, cand, cand_key, cand_sorted;
+    DevBuf<msim::RerankItem> items;
+    DevBuf<uint8_t> doc_bits, row_bits, tmp;
+    DevBuf<unsigned long long> counters;   // [0] candidate pairs, [1] token x row distances, [2] unique count
+    cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    float stage_ms[4] = {0.f, 0.f, 0.f, 0.f};   // last search: stage 1, candidates, re-rank, select (with timing on)
+    int64_t n_docs() const { return (int64_t)lims.size() - 1; }
+    ~EmbListState() {
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+    }
+};
+
+__global__ void
+doc_of_row_kernel(const int64_t* lims, int64_t n_docs, int32_t* doc_of_row) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_docs) return;
+    for (int64_t r = lims[j]; r < lims[j + 1]; r++) doc_of_row[r] = (int32_t)j;
+}
+
+// byte b of the row bitset: bit i set when the document of row 8b + i is filtered out
+__global__ void
+row_bits_kernel(const uint8_t* doc_bits, const int32_t* doc_of_row, int64_t n, uint8_t* row_bits) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b * 8 >= n) return;
+    uint32_t v = 0;
+    for (int i = 0; i < 8 && b * 8 + i < n; i++)
+        if (bit_is_set(doc_bits, doc_of_row[b * 8 + i])) v |= 1u << i;
+    row_bits[b] = (uint8_t)v;
+}
+
+// entry e = (token, slot) of the stage-1 result -> (list of the token - l0) << 32 | document; kEmpty for id -1
+__global__ void
+cand_keys_kernel(const int64_t* ids, int64_t n, int vec_topk, const int32_t* row_list, int64_t r0, int64_t l0,
+                 const int32_t* doc_of_row, uint64_t* keys) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const int64_t id = ids[e];
+    keys[e] = id < 0 ? kEmpty
+                     : ((uint64_t)(row_list[r0 + e / vec_topk] - l0) << 32) | (uint64_t)(uint32_t)doc_of_row[id];
+}
+
+// off[l] = first of the nu sorted distinct keys with list >= l (the kEmpty sentinel sorts after every list)
+__global__ void
+cand_off_kernel(const uint64_t* ukeys, const unsigned long long* nu, int64_t nlists, int64_t* off) {
+    const int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (l > nlists) return;
+    const uint64_t key = (uint64_t)l << 32;
+    int64_t lo = 0, hi = (int64_t)*nu;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (ukeys[mid] < key) lo = mid + 1;
+        else hi = mid;
+    }
+    off[l] = lo;
+}
+
+template <int METRIC>
+__global__ void
+el_emit_kernel(const uint64_t* sorted, const int64_t* off, int64_t nlists, int k, int64_t l0, int64_t* out_ids,
+               float* out_dist) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= nlists * k) return;
+    const int64_t l = e / k, r = e % k;
+    const int64_t o = (l0 + l) * k + r;
+    if (r < off[l + 1] - off[l]) {
+        const uint64_t v = sorted[off[l] + r];
+        const float key = unpack_key(v);
+        out_ids[o] = (int64_t)unpack_pos(v);
+        out_dist[o] = (METRIC == KB2_METRIC_L2) ? key : -key;
+    } else {
+        out_ids[o] = -1;
+        out_dist[o] = (METRIC == KB2_METRIC_L2) ? FLT_MAX : -FLT_MAX;
+    }
+}
+
+// metric of the base index that an emb-list metric pairs with (MAX_SIM_L2 - L2, MAX_SIM_IP - IP, MAX_SIM_COSINE - COSINE)
+inline bool
+emb_list_metric_pairs(const IndexBase& ix, int metric) {
+    if (metric == KB2_METRIC_MAX_SIM_L2) return ix.metric == KB2_METRIC_L2;
+    if (metric == KB2_METRIC_MAX_SIM_IP) return ix.metric == KB2_METRIC_IP && !ix.cosine;
+    if (metric == KB2_METRIC_MAX_SIM_COSINE) return ix.cosine;
+    return false;
+}
+
+// Attach validated host offsets (lims.back() == ix.count()) to an HNSW or IVF_FLAT index.
+inline void
+set_emb_list(IndexBase& ix, std::vector<int64_t> lims, int metric) {
+    auto* iv = dynamic_cast<IvfIndex*>(&ix);
+    auto* hn = dynamic_cast<HnswIndex*>(&ix);
+    KB2_REQUIRE((iv && !iv->is_pq) || hn, KB2_INVALID_METRIC_TYPE, "emb-lists are supported on HNSW and IVF_FLAT only");
+    KB2_REQUIRE(metric == KB2_METRIC_MAX_SIM_L2 || metric == KB2_METRIC_MAX_SIM_IP || metric == KB2_METRIC_MAX_SIM_COSINE,
+                KB2_INVALID_METRIC_TYPE, "metric must be MAX_SIM_L2, MAX_SIM_IP or MAX_SIM_COSINE");
+    KB2_REQUIRE(emb_list_metric_pairs(ix, metric), KB2_INVALID_METRIC_TYPE,
+                "the emb-list metric does not match the index metric (MAX_SIM_L2: L2, MAX_SIM_IP: IP, MAX_SIM_COSINE: COSINE)");
+    KB2_REQUIRE(ix.shard_world == 1, KB2_NOT_IMPLEMENTED, "emb-lists on a sharded index");
+    KB2_REQUIRE(!(iv && iv->custom_labels) && !(hn && hn->custom_labels), KB2_NOT_IMPLEMENTED, "emb-lists with custom ids");
+    const int64_t n = ix.count();
+    KB2_REQUIRE(lims.size() >= 2 && lims.back() == n, KB2_INVALID_ARGS, "document offsets must end at the index's row count");
+    KB2_REQUIRE(n > 0 && n < (1ll << 31) && (int64_t)lims.size() - 1 < (1ll << 31), KB2_INVALID_ARGS,
+                "emb-list sizes out of range (rows 1 .. 2^31 - 1)");
+    if (iv) iv->seal();
+    auto el = std::make_shared<EmbListState>();
+    el->metric = metric;
+    el->lims = std::move(lims);
+    const int64_t nd = el->n_docs();
+    el->d_lims.ensure(nd + 1);
+    el->doc_of_row.ensure(n);
+    KB2_CUDA_CHECK(cudaMemcpyAsync(el->d_lims.p, el->lims.data(), (nd + 1) * 8, cudaMemcpyHostToDevice, ix.stream));
+    doc_of_row_kernel<<<grid1d(nd, 256), 256, 0, ix.stream>>>(el->d_lims.p, nd, el->doc_of_row.p);
+    KB2_CUDA_CHECK(cudaGetLastError());
+    for (cudaEvent_t& e : el->ev) KB2_CUDA_CHECK(cudaEventCreate(&e));
+    el->counters.ensure(4);
+    KB2_CUDA_CHECK(cudaStreamSynchronize(ix.stream));
+    ix.emb_list = std::move(el);
+}
+
+// The search.  queries: host or device rows, ql: validated host offsets of the query lists; out_*: [lists][k], host or
+// device.  stats: query lists, (list, document) candidates re-ranked, token x row distances computed.
+inline void
+search_emb_list(IndexBase& ix, const float* queries, const std::vector<int64_t>& ql, int k, const JsonObj& cfg,
+                const uint8_t* bitset, int64_t nbits, int64_t* out_ids, float* out_dist, int64_t stats[3]) {
+    EmbListState& el = *ix.emb_list;
+    cudaStream_t st = ix.stream;
+    auto* iv = dynamic_cast<IvfIndex*>(&ix);
+    auto* hn = dynamic_cast<HnswIndex*>(&ix);
+    const int64_t n = ix.count(), n_docs = el.n_docs(), n_lists = (int64_t)ql.size() - 1, nq_rows = ql.back();
+    const int d = ix.dim;
+    // doc_of_row and the offsets were built for the rows the index held when they were attached
+    KB2_REQUIRE(el.lims.back() == n, KB2_EMB_LIST_INNER_ERROR, "the index's rows no longer match its emb-list offsets");
+    const double ratio_in = cfg.get_num("retrieval_ann_ratio", 3.0);
+    const float ratio = (float)ratio_in;
+    KB2_REQUIRE(ratio > 0.f, KB2_EMB_LIST_INNER_ERROR, "retrieval_ann_ratio could not be less than or equal to 0");
+    // emb_list_strategy_token_ann.cc:87-88: int32(k * ratio) in fp32, at least 1, at most the index's rows
+    const float prod = (float)k * ratio;
+    const int64_t want = prod >= 2147483648.f ? (int64_t)INT32_MAX : (int64_t)(int32_t)prod;
+    const int vec_topk = (int)std::min<int64_t>(std::max<int64_t>(want, 1), n);
+    JsonObj base = cfg;
+    if (hn) {
+        // base_hnsw_config.h:60-72 checks ef against the list-level k; the base search keeps max(ef, vec_topk)
+        const int64_t ef = cfg.get_int("ef", std::max(k, 16));
+        KB2_REQUIRE(ef >= k, KB2_OUT_OF_RANGE_IN_JSON, "ef(" + std::to_string(ef) + ") should be larger than k(" + std::to_string(k) + ")");
+        base.kv["ef"] = std::to_string(std::max<int64_t>(ef, vec_topk));
+    }
+    for (float& v : el.stage_ms) v = 0.f;
+    if (n_lists == 0) return;
+
+    // query rows on the device (normalised once for COSINE), list offsets and the list of every row
+    const float* dq = nullptr;
+    if (nq_rows > 0) {
+        el.q.ensure((size_t)nq_rows * d);
+        const float* src = ix.cosine ? ix.normalized(queries, nq_rows) : queries;
+        KB2_CUDA_CHECK(cudaMemcpyAsync(el.q.p, src, (size_t)nq_rows * d * 4, cudaMemcpyDefault, st));
+        dq = el.q.p;
+    }
+    el.qlims.ensure(ql.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(el.qlims.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice, st));
+    std::vector<int32_t> row_list((size_t)std::max<int64_t>(nq_rows, 1));
+    for (int64_t l = 0; l < n_lists; l++)
+        for (int64_t r = ql[l]; r < ql[l + 1]; r++) row_list[r] = (int32_t)l;
+    el.row_list.ensure(row_list.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(el.row_list.p, row_list.data(), row_list.size() * 4, cudaMemcpyHostToDevice, st));
+
+    // the document bitset as a row bitset
+    const uint8_t* rbits = nullptr;
+    if (bitset && nbits > 0) {
+        KB2_REQUIRE(nbits >= n_docs, KB2_INVALID_ARGS, "bitset has fewer bits than the index has documents");
+        const uint8_t* dbits = bitset;
+        if (!is_device_ptr(bitset)) {
+            el.doc_bits.ensure((size_t)((n_docs + 7) / 8));
+            KB2_CUDA_CHECK(cudaMemcpyAsync(el.doc_bits.p, bitset, (size_t)((n_docs + 7) / 8), cudaMemcpyHostToDevice, st));
+            dbits = el.doc_bits.p;
+        }
+        el.row_bits.ensure((size_t)((n + 7) / 8));
+        row_bits_kernel<<<grid1d((n + 7) / 8, 256), 256, 0, st>>>(dbits, el.doc_of_row.p, n, el.row_bits.p);
+        KB2_CUDA_CHECK(cudaGetLastError());
+        rbits = el.row_bits.p;
+    }
+
+    int64_t* d_ids;
+    float* d_dist;
+    ix.device_out(n_lists, k, out_ids, out_dist, d_ids, d_dist);
+    const float* X = hn ? (hn->upload(), hn->d_vecs.p) : iv->vecs.p;
+    const int32_t* pos = iv ? iv->pos_of_row.p : nullptr;
+    const bool vec4 = (d & 3) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
+    KB2_CUDA_CHECK(cudaMemsetAsync(el.counters.p, 0, 2 * sizeof(unsigned long long), st));
+    unsigned long long* hc = (unsigned long long*)ix.h_counter.p + 12;   // [0] items, [1] candidates
+
+    for (int64_t l0 = 0; l0 < n_lists;) {
+        // whole lists, stage-1 entries within the scratch budget (at least one list)
+        int64_t l1 = l0 + 1;
+        while (l1 < n_lists && (ql[l1 + 1] - ql[l0]) * vec_topk <= kEmbListChunkEntries) l1++;
+        const int64_t L = l1 - l0, r0 = ql[l0], nt = ql[l1] - r0;
+        const int64_t ne = nt * vec_topk;
+        KB2_REQUIRE(ne < (1ll << 31), KB2_INVALID_ARGS, "emb-list search: one query list's tokens x vec_topk exceed 2^31 - 1");
+        el.cand_off.ensure(L + 1);
+        if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[0], st));
+        int64_t nu = 0;
+        if (nt > 0) {
+            // 1. stage 1 over the chunk's tokens
+            el.s1_ids.ensure(ne);
+            el.s1_dist.ensure(ne);
+            ix.search(dq + r0 * d, nt, vec_topk, base, rbits, rbits ? n : 0, el.s1_ids.p, el.s1_dist.p);
+            if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[1], st));
+            // 2. distinct (list, document) candidates
+            el.keys.ensure(ne);
+            el.keys_sorted.ensure(ne);
+            el.cand.ensure(ne);
+            cand_keys_kernel<<<grid1d(ne, 256), 256, 0, st>>>(el.s1_ids.p, ne, vec_topk, el.row_list.p, r0, l0,
+                                                              el.doc_of_row.p, el.keys.p);
+            // list bits up to the first that no list of the chunk sets: kEmpty (all ones) still sorts last
+            int end_bit = 33;
+            while ((1ll << (end_bit - 32)) <= L) end_bit++;
+            size_t b1 = 0, b2 = 0;
+            cub::DeviceRadixSort::SortKeys(nullptr, b1, el.keys.p, el.keys_sorted.p, (int)ne, 0, end_bit, st);
+            cub::DeviceSelect::Unique(nullptr, b2, el.keys_sorted.p, el.cand.p, el.counters.p + 2, (int)ne, st);
+            el.tmp.ensure(std::max(b1, b2));
+            b1 = el.tmp.n;
+            KB2_CUDA_CHECK(cub::DeviceRadixSort::SortKeys(el.tmp.p, b1, el.keys.p, el.keys_sorted.p, (int)ne, 0, end_bit, st));
+            b2 = el.tmp.n;
+            KB2_CUDA_CHECK(cub::DeviceSelect::Unique(el.tmp.p, b2, el.keys_sorted.p, el.cand.p, el.counters.p + 2, (int)ne, st));
+            cand_off_kernel<<<grid1d(L + 1, 256), 256, 0, st>>>(el.cand.p, el.counters.p + 2, L, el.cand_off.p);
+            // items of every list
+            el.item_cnt.ensure(L + 1);
+            el.item_off.ensure(L + 1);
+            KB2_CUDA_CHECK(cudaMemsetAsync(el.item_cnt.p + L, 0, 4, st));
+            msim::rerank_plan_kernel<<<grid1d(L, 128), 128, 0, st>>>(el.cand_off.p, el.cand.p, el.d_lims.p, el.qlims.p, l0, L,
+                                                                     el.item_cnt.p, nullptr, nullptr, el.counters.p);
+            size_t b3 = 0;
+            cub::DeviceScan::ExclusiveSum(nullptr, b3, el.item_cnt.p, el.item_off.p, (int)(L + 1), st);
+            el.tmp.ensure(b3);
+            b3 = el.tmp.n;
+            KB2_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(el.tmp.p, b3, el.item_cnt.p, el.item_off.p, (int)(L + 1), st));
+            KB2_CUDA_CHECK(cudaMemcpyAsync(hc, el.item_off.p + L, 4, cudaMemcpyDeviceToHost, st));
+            KB2_CUDA_CHECK(cudaMemcpyAsync(hc + 1, el.cand_off.p + L, 8, cudaMemcpyDeviceToHost, st));
+            KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+            const int64_t nitems = (int64_t)*(const int32_t*)hc;
+            nu = (int64_t)hc[1];
+            el.items.ensure(std::max<int64_t>(nitems, 1));
+            msim::rerank_plan_kernel<<<grid1d(L, 128), 128, 0, st>>>(el.cand_off.p, el.cand.p, el.d_lims.p, el.qlims.p, l0, L,
+                                                                     nullptr, el.item_off.p, el.items.p, nullptr);
+            KB2_CUDA_CHECK(cudaGetLastError());
+            if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[2], st));
+            // 3. exact keys of every candidate
+            el.cand_key.ensure(std::max<int64_t>(nu, 1));
+            el.cand_sorted.ensure(std::max<int64_t>(nu, 1));
+            if (nitems > 0) {
+                const msim::RerankParams rp{dq, el.qlims.p, X, pos, el.d_lims.p, d, l0, el.items.p, el.cand.p, el.cand_key.p};
+                with_metric(ix.metric, [&](auto m) { msim::launch_rerank<decltype(m)::value>(vec4, (unsigned)nitems, st, rp); });
+                KB2_CUDA_CHECK(cudaGetLastError());
+            }
+            if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[3], st));
+            // 4. each list's candidates in (key, document) order
+            if (nu > 0) {
+                size_t b4 = 0;
+                cub::DeviceSegmentedRadixSort::SortKeys(nullptr, b4, el.cand_key.p, el.cand_sorted.p, (int)nu, (int)L,
+                                                        el.cand_off.p, el.cand_off.p + 1, 0, 64, st);
+                el.tmp.ensure(b4);
+                b4 = el.tmp.n;
+                KB2_CUDA_CHECK(cub::DeviceSegmentedRadixSort::SortKeys(el.tmp.p, b4, el.cand_key.p, el.cand_sorted.p, (int)nu,
+                                                                       (int)L, el.cand_off.p, el.cand_off.p + 1, 0, 64, st));
+            }
+            ix.last.launches += 7;
+        } else {
+            KB2_CUDA_CHECK(cudaMemsetAsync(el.cand_off.p, 0, (L + 1) * 8, st));
+            el.cand_sorted.ensure(1);
+            for (int i = 1; i < 4; i++)
+                if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[i], st));
+        }
+        with_metric(ix.metric, [&](auto m) {
+            el_emit_kernel<decltype(m)::value><<<grid1d(L * k, 256), 256, 0, st>>>(el.cand_sorted.p, el.cand_off.p, L, k, l0, d_ids,
+                                                                                  d_dist);
+        });
+        KB2_CUDA_CHECK(cudaGetLastError());
+        if (ix.timing) {
+            KB2_CUDA_CHECK(cudaEventRecord(el.ev[4], st));
+            KB2_CUDA_CHECK(cudaEventSynchronize(el.ev[4]));
+            for (int i = 0; i < 4; i++) {
+                float ms = 0.f;
+                KB2_CUDA_CHECK(cudaEventElapsedTime(&ms, el.ev[i], el.ev[i + 1]));
+                el.stage_ms[i] += ms;
+            }
+        }
+        l0 = l1;
+    }
+    KB2_CUDA_CHECK(cudaMemcpyAsync(hc, el.counters.p, 16, cudaMemcpyDeviceToHost, st));
+    ix.results_out(n_lists, k, out_ids, out_dist, d_ids, d_dist);
+    stats[0] = n_lists;
+    stats[1] = (int64_t)hc[0];
+    stats[2] = (int64_t)hc[1];
+}
+
+}  // namespace kb2

@@ -499,7 +499,8 @@ hnsw_search_kernel(HnswSearchParams p) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dpad = (p.d + 3) & ~3;
     const int cap = p.ef_cap;
-    const size_t per_warp = (size_t)dpad * 4 + (size_t)cap * (FILTERED ? 16 : 8);
+    // 16-byte aligned per-warp regions: the query row is read as float4 (an odd ef would misalign every other warp's)
+    const size_t per_warp = ((size_t)dpad * 4 + (size_t)cap * (FILTERED ? 16 : 8) + 15) & ~(size_t)15;
     unsigned char* mine = smem_raw + (size_t)warp * per_warp;
     float* s_q = (float*)mine;
     float* v_dist = (float*)(mine + (size_t)dpad * 4);
@@ -1625,7 +1626,7 @@ struct HnswIndex : IndexBase {
     size_t
     warp_smem(int ef_cap, bool two_pools) const {
         const int dpad = (dim + 3) & ~3;
-        return kHnswWarps * ((size_t)dpad * 4 + (size_t)ef_cap * (two_pools ? 16 : 8));
+        return kHnswWarps * (size_t)round_up((int64_t)dpad * 4 + (int64_t)ef_cap * (two_pools ? 16 : 8), 16);
     }
     // grow the per-warp (per-CTA) visited bitmaps, zeroed, and touched-id logs to what L needs
     void

@@ -7,6 +7,7 @@
 #pragma once
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -50,9 +51,12 @@ dev_append(DevBuf<T>& buf, size_t& used, const T* src, size_t count, cudaStream_
     used += count;
 }
 
+struct EmbListState;   // kb2_emb_list_index.cuh
+
 // ============================================================================================
 struct IndexBase {
     std::string type;
+    std::shared_ptr<EmbListState> emb_list;   // document offsets of an emb-list index (kb2_index_set_emb_list), or null
     int metric = KB2_METRIC_L2, dim = 0, device = 0;
     bool cosine = false;   // COSINE: metric == IP over vectors normalised on entry (see kb2_index_create)
     cudaStream_t stream = nullptr;

@@ -577,5 +577,254 @@ search(FlatIndex& fi, Scratch& sc, const float* dq, const std::vector<int64_t>& 
     stats[2] += n_exact + nredo;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Exact re-rank of gathered candidates (index-level emb-list search, kb2_emb_list_index.cuh; DESIGN §4.11).
+//
+// A work item is one query list and a run of its candidate documents: up to RR_MAXD whole documents of at most RR_TR
+// rows in all, or one longer document alone.  One CTA per item.  The list's tokens are taken RR_TQ at a time; for each
+// token block the item's rows are taken RR_TR at a time, and the (token x row) block is contracted like an SGEMM over
+// RR_DK-dimension stages (cp.async 16-byte copies into a double-buffered shared tile when rows are float4-aligned).
+// Each thread owns a 4 x 4 (token x row) register tile and runs every one of its distances as the fmaf chain over
+// dimensions 0..d-1 of maxsim_exact_kernel, so each distance has the same bits; the per-(token, document) extremum is
+// order-free (fminf over the same values), and after each token block one thread per document adds the block's extrema
+// to its running sum in token order, as maxsim_exact_kernel does.  The scores are therefore bit-identical to the
+// BruteForce re-rank.  Rows are read in place (HNSW) or at pos[row] (IVF_FLAT's list-order store).
+constexpr int RR_TQ = 32;
+constexpr int RR_TR = 128;
+constexpr int RR_DK = 32;
+constexpr int RR_LD = RR_DK + 4;   // row stride of the stage tiles: a warp's 8 tokens / 4 rows fall on distinct banks
+constexpr int RR_MAXD = 32;
+constexpr int RR_THREADS = 256;
+constexpr size_t RR_SMEM = (size_t)(2 * (RR_TQ + RR_TR) * RR_LD + RR_TQ * RR_TR + RR_TQ * RR_MAXD + RR_MAXD) * 4 +
+                           (size_t)(2 * RR_TR + RR_MAXD + 1) * 4;
+
+struct RerankItem {
+    int32_t list;    // query list, relative to RerankParams::l0
+    int32_t c0;      // first candidate (index into cand)
+    int32_t ndocs;   // candidates cand[c0 .. c0 + ndocs)
+    int32_t nrows;   // their rows in all
+};
+
+struct RerankParams {
+    const float* Q;             // query rows
+    const int64_t* qlims;       // [lists + 1]
+    const float* X;             // stored rows
+    const int32_t* pos;         // row -> position in X, or nullptr (row r at X + r * d)
+    const int64_t* xlims;       // [n_docs + 1]
+    int d;
+    int64_t l0;
+    const RerankItem* items;
+    const uint64_t* cand;       // low 32 bits: document
+    uint64_t* out;              // [candidates] pack_kp(exact key, document)
+};
+
+__device__ __forceinline__ void
+cp_async16(void* smem, const void* gmem, int src_bytes) {
+    const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(src_bytes) : "memory");
+}
+
+template <int METRIC, bool VEC4>
+__global__ void __launch_bounds__(RR_THREADS)
+maxsim_rerank_kernel(const RerankParams p) {
+    extern __shared__ __align__(16) unsigned char rr_smem[];
+    float* sQ = reinterpret_cast<float*>(rr_smem);   // [2][RR_TQ][RR_LD]
+    float* sX = sQ + 2 * RR_TQ * RR_LD;               // [2][RR_TR][RR_LD]
+    float* sK = sX + 2 * RR_TR * RR_LD;               // [RR_TQ][RR_TR] keys of the current (token block, row tile)
+    float* sE = sK + RR_TQ * RR_TR;                   // [RR_TQ][RR_MAXD] extremum per (token, document)
+    float* sT = sE + RR_TQ * RR_MAXD;                 // [RR_MAXD] running token sums
+    int32_t* sRow = reinterpret_cast<int32_t*>(sT + RR_MAXD);   // [RR_TR] position of each tile row in X, -1 past the end
+    int32_t* sSlot = sRow + RR_TR;                               // [RR_TR] document slot of each tile row
+    int32_t* sBeg = sSlot + RR_TR;                               // [RR_MAXD + 1] first item row of each document
+
+    const RerankItem it = p.items[blockIdx.x];
+    const int64_t lst = p.l0 + it.list;
+    const int64_t qa = p.qlims[lst], qe = p.qlims[lst + 1];
+    const int d = p.d;
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const int tg = lane & 7, rg = warp * 4 + (lane >> 3);   // this thread: tokens tg + 8i, rows rg + 32j (i, j < 4)
+    if (t == 0) {
+        int acc = 0;
+        for (int s = 0; s < it.ndocs; s++) {
+            sBeg[s] = acc;
+            const int64_t doc = (int64_t)(uint32_t)p.cand[it.c0 + s];
+            acc += (int)(p.xlims[doc + 1] - p.xlims[doc]);
+        }
+        sBeg[it.ndocs] = acc;
+    }
+    if (t < it.ndocs) sT[t] = 0.f;
+    __syncthreads();
+
+    const int ntiles = (it.nrows + RR_TR - 1) / RR_TR;
+    const int nkc = (d + RR_DK - 1) / RR_DK;
+    for (int64_t t0 = qa; t0 < qe; t0 += RR_TQ) {
+        const int nt = qe - t0 < RR_TQ ? (int)(qe - t0) : RR_TQ;
+        for (int tile = 0; tile < ntiles; tile++) {
+            const int r0 = tile * RR_TR;
+            if (t < RR_TR) {
+                const int r = r0 + t;
+                int32_t ps = -1, slot = 0;
+                if (r < it.nrows) {
+                    while (sBeg[slot + 1] <= r) slot++;
+                    const int64_t doc = (int64_t)(uint32_t)p.cand[it.c0 + slot];
+                    const int64_t row = p.xlims[doc] + (r - sBeg[slot]);
+                    ps = p.pos ? p.pos[row] : (int32_t)row;
+                }
+                sRow[t] = ps;
+                sSlot[t] = slot;
+            }
+            __syncthreads();
+            // stage kc of dimensions [kc * RR_DK, +RR_DK) into buffer b; zero past d, past the list and past the item
+            auto load = [&](int kc, int b) {
+                float* q = sQ + b * RR_TQ * RR_LD;
+                float* x = sX + b * RR_TR * RR_LD;
+                const int k0 = kc * RR_DK;
+                if (VEC4) {
+                    {
+                        const int tok = t >> 3, c = (t & 7) * 4;
+                        const bool ok = tok < nt && k0 + c < d;
+                        cp_async16(q + tok * RR_LD + c, ok ? p.Q + (t0 + tok) * d + k0 + c : p.Q, ok ? 16 : 0);
+                    }
+#pragma unroll
+                    for (int i = 0; i < RR_TR * RR_DK / 4 / RR_THREADS; i++) {
+                        const int e = t + i * RR_THREADS;
+                        const int r = e >> 3, c = (e & 7) * 4;
+                        const int32_t ps = sRow[r];
+                        const bool ok = ps >= 0 && k0 + c < d;
+                        cp_async16(x + r * RR_LD + c, ok ? p.X + (int64_t)ps * d + k0 + c : p.X, ok ? 16 : 0);
+                    }
+                    asm volatile("cp.async.commit_group;" ::: "memory");
+                } else {
+                    for (int e = t; e < RR_TQ * RR_DK; e += RR_THREADS) {
+                        const int tok = e / RR_DK, c = e % RR_DK;
+                        q[tok * RR_LD + c] = (tok < nt && k0 + c < d) ? p.Q[(t0 + tok) * d + k0 + c] : 0.f;
+                    }
+                    for (int e = t; e < RR_TR * RR_DK; e += RR_THREADS) {
+                        const int r = e / RR_DK, c = e % RR_DK;
+                        const int32_t ps = sRow[r];
+                        x[r * RR_LD + c] = (ps >= 0 && k0 + c < d) ? p.X[(int64_t)ps * d + k0 + c] : 0.f;
+                    }
+                }
+            };
+            float acc[4][4];
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
+            load(0, 0);
+            for (int kc = 0; kc < nkc; kc++) {
+                if (kc + 1 < nkc) {
+                    load(kc + 1, (kc + 1) & 1);
+                    if (VEC4) asm volatile("cp.async.wait_group 1;" ::: "memory");
+                } else if (VEC4) {
+                    asm volatile("cp.async.wait_group 0;" ::: "memory");
+                }
+                __syncthreads();
+                const float* q = sQ + (kc & 1) * RR_TQ * RR_LD;
+                const float* x = sX + (kc & 1) * RR_TR * RR_LD;
+                // zero-padded dimensions past d leave every chain unchanged: fmaf(0, 0, acc) == acc (acc is never -0)
+#pragma unroll 8
+                for (int kk = 0; kk < RR_DK; kk++) {
+                    float qv[4], xv[4];
+#pragma unroll
+                    for (int i = 0; i < 4; i++) qv[i] = q[(tg + 8 * i) * RR_LD + kk];
+#pragma unroll
+                    for (int j = 0; j < 4; j++) xv[j] = x[(rg + 32 * j) * RR_LD + kk];
+#pragma unroll
+                    for (int i = 0; i < 4; i++)
+#pragma unroll
+                        for (int j = 0; j < 4; j++) {
+                            if (METRIC == KB2_METRIC_L2) {
+                                const float df = qv[i] - xv[j];
+                                acc[i][j] = fmaf(df, df, acc[i][j]);
+                            } else {
+                                acc[i][j] = fmaf(qv[i], xv[j], acc[i][j]);
+                            }
+                        }
+                }
+                __syncthreads();
+            }
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++)
+                    sK[(tg + 8 * i) * RR_TR + rg + 32 * j] = (METRIC == KB2_METRIC_L2) ? acc[i][j] : -acc[i][j];
+            __syncthreads();
+            // extremum of each (token, document) over the document's rows in this tile, folded over the tiles
+            for (int task = t; task < RR_TQ * it.ndocs; task += RR_THREADS) {
+                const int s = task / RR_TQ, tok = task % RR_TQ;
+                if (tok >= nt) continue;
+                const int a = max(sBeg[s], r0) - r0, b = min(sBeg[s + 1], r0 + RR_TR) - r0;
+                if (a >= b) continue;
+                float m = INFINITY;
+                for (int r = a; r < b; r++) m = fminf(m, sK[tok * RR_TR + r]);
+                float* e = sE + tok * RR_MAXD + s;
+                *e = sBeg[s] >= r0 ? m : fminf(*e, m);
+            }
+            __syncthreads();
+        }
+        // sum of the block's extrema, in token order, onto each document's running sum
+        if (t < it.ndocs) {
+            float tot = sT[t];
+            for (int tok = 0; tok < nt; tok++) tot += sE[tok * RR_MAXD + t];
+            sT[t] = tot;
+        }
+        __syncthreads();
+    }
+    // an empty query list or document scores +inf, as in maxsim_exact_kernel
+    if (t < it.ndocs)
+        p.out[it.c0 + t] = pack_kp(qe > qa && sBeg[t + 1] > sBeg[t] ? sT[t] : INFINITY, (uint32_t)p.cand[it.c0 + t]);
+}
+
+template <int METRIC>
+inline void
+launch_rerank(bool vec4, unsigned nitems, cudaStream_t st, const RerankParams& rp) {
+    if (vec4) launch<maxsim_rerank_kernel<METRIC, true>>(nitems, RR_THREADS, RR_SMEM, st, rp);
+    else launch<maxsim_rerank_kernel<METRIC, false>>(nitems, RR_THREADS, RR_SMEM, st, rp);
+}
+
+// Items of the candidates of each list (cand_off: [lists + 1] CSR over the candidates, each list's documents in
+// ascending order).  One thread per list packs its documents greedily: consecutive documents while they hold at most
+// RR_TR rows and RR_MAXD documents, a longer document alone.  Pass 1 (items == nullptr) counts each list's items into
+// cnt[l] and adds the list's (document, |Q| x |D|) totals to stats[0..1]; pass 2 writes them at off[l].
+__global__ void
+rerank_plan_kernel(const int64_t* cand_off, const uint64_t* cand, const int64_t* xlims, const int64_t* qlims, int64_t l0,
+                   int64_t nlists, int32_t* cnt, const int32_t* off, RerankItem* items, unsigned long long* stats) {
+    const int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (l >= nlists) return;
+    const int64_t c0 = cand_off[l], c1 = cand_off[l + 1];
+    int n = 0;
+    int64_t o = items ? off[l] : 0;
+    unsigned long long rows_all = 0;
+    RerankItem cur{(int32_t)l, 0, 0, 0};
+    auto close = [&] {
+        if (cur.ndocs == 0) return;
+        if (items) items[o++] = cur;
+        n++;
+        cur.ndocs = 0;
+    };
+    for (int64_t c = c0; c < c1; c++) {
+        const int64_t doc = (int64_t)(uint32_t)cand[c];
+        const int len = (int)(xlims[doc + 1] - xlims[doc]);
+        rows_all += (unsigned long long)len;
+        if (cur.ndocs > 0 && (len > RR_TR || cur.nrows + len > RR_TR || cur.ndocs == RR_MAXD)) close();
+        if (cur.ndocs == 0) {
+            cur.c0 = (int32_t)c;
+            cur.nrows = 0;
+        }
+        cur.ndocs++;
+        cur.nrows += len;
+        if (len > RR_TR) close();
+    }
+    close();
+    if (!items) {
+        cnt[l] = n;
+        if (c1 > c0) {
+            atomicAdd(stats, (unsigned long long)(c1 - c0));
+            atomicAdd(stats + 1, rows_all * (unsigned long long)(qlims[l0 + l + 1] - qlims[l0 + l]));
+        }
+    }
+}
+
 }  // namespace msim
 }  // namespace kb2

@@ -9,6 +9,7 @@
 #include <memory>
 
 #include "kb2_blob.h"
+#include "kb2_emb_list_index.cuh"
 #include "kb2_hnsw.cuh"
 #include "kb2_index.cuh"
 
@@ -283,6 +284,13 @@ serialize_index(IndexBase& ix, std::vector<uint8_t>& blob) {
     } else {
         throw Error(KB2_NOT_IMPLEMENTED, "serialize: unknown index class");
     }
+    // optional trailing section of an emb-list index: "ELST", the MAX_SIM metric, n_docs, offsets[n_docs + 1]
+    if (ix.emb_list) {
+        w.put<uint32_t>(kEmbListTag);
+        w.put<int32_t>(ix.emb_list->metric);
+        w.put<int64_t>(ix.emb_list->n_docs());
+        w.put_bytes(ix.emb_list->lims.data(), ix.emb_list->lims.size() * 8);
+    }
 }
 
 inline std::unique_ptr<IndexBase>
@@ -369,6 +377,17 @@ deserialize_index(const uint8_t* blob, size_t size, int device) {
         throw Error(KB2_INVALID_BINARY_SET, "unknown index type in blob");
     }
     ix->cosine = cosine;   // stored vectors are already normalised; queries will be
+    if (r.o < r.n) {
+        KB2_REQUIRE(r.get<uint32_t>() == kEmbListTag, KB2_INVALID_BINARY_SET, "unknown section after the index in blob");
+        const int el_metric = r.get<int32_t>();
+        const int64_t nd = r.get<int64_t>();
+        KB2_REQUIRE(nd >= 1 && (uint64_t)nd < (r.n - r.o) / 8, KB2_INVALID_BINARY_SET, "bad emb-list document count in blob");
+        std::vector<int64_t> lims((size_t)nd + 1);
+        memcpy(lims.data(), r.get_bytes(lims.size() * 8), lims.size() * 8);
+        KB2_REQUIRE(lims[0] == 0, KB2_INVALID_BINARY_SET, "bad emb-list offsets in blob");
+        for (int64_t i = 0; i < nd; i++) KB2_REQUIRE(lims[i + 1] >= lims[i], KB2_INVALID_BINARY_SET, "bad emb-list offsets in blob");
+        set_emb_list(*ix, std::move(lims), el_metric);
+    }
     return ix;
 }
 
