@@ -495,11 +495,14 @@ class B200IndexNode : public IndexNode {
     bool HasRawData(const std::string&) const override { return h_ && kb2_index_has_raw_data(h_); }
     // Serialize: ONE binary named after the index type holding the faiss fourcc stream, exactly what the reference's
     // nodes write (flat.cc:323-343, ivf.cc:1717-1741, faiss_hnsw.cc:188-217), so the reference's CPU nodes can load it.
-    // Indexes the wire format cannot express (COSINE keeps unit vectors only; custom ids) fall back to the "KB2I" container.
+    // Indexes the wire format cannot express (COSINE keeps unit vectors only; custom ids; GPU_CAGRA) use the "KB2I" container.
     Status Serialize(BinarySet& bs) const override {
         if (!h_) return Status::empty_index;
         uint8_t* p = nullptr; size_t n = 0;
-        int rc = kb2_index_serialize_faiss(h_, &p, &n);
+        // GPU_CAGRA keeps its own type and build parameters in the container (its graph as an HNSW stream is
+        // kb2_index_serialize_faiss, for the reference's CPU HNSW node)
+        const bool cagra = type_ == "GPU_CAGRA" || type_ == "GPU_CUVS_CAGRA";
+        int rc = cagra ? KB2_NOT_IMPLEMENTED : kb2_index_serialize_faiss(h_, &p, &n);
         if (rc == KB2_NOT_IMPLEMENTED) rc = kb2_index_serialize(h_, &p, &n);
         if (rc) return (Status)rc;
         std::shared_ptr<uint8_t[]> buf(new uint8_t[n]);
@@ -660,6 +663,8 @@ class B200IndexNode : public IndexNode {
     };
     expected<std::vector<IteratorPtr>> AnnIterator(const DataSetPtr ds, const Json& cfg, const BitsetView& bitset) const override {
         if (!h_) return expected<std::vector<IteratorPtr>>::Err(Status::empty_index, "index not loaded");
+        if (type_ == "GPU_CAGRA" || type_ == "GPU_CUVS_CAGRA")   // as the reference's GPU nodes (gpu_cuvs.h)
+            return expected<std::vector<IteratorPtr>>::Err(Status::not_implemented, "AnnIterator is not supported on GPU_CAGRA");
         int code = 0;
         if (kb2_emb_list_metric(cfg.get_string(meta::METRIC_TYPE, "L2"), code))   // index_node.cc:312-324
             return expected<std::vector<IteratorPtr>>::Err(Status::emb_list_inner_error, "ann iterator is not supported for emb_list");
@@ -744,7 +749,7 @@ class IndexFactory {
     const IndexFactory& Register(const std::string& name, Creator c) { map_[name] = std::move(c); return *this; }
  private:
     IndexFactory() {
-        for (const char* n : {"FLAT", "IVF_FLAT", "IVF_PQ", "HNSW"}) {
+        for (const char* n : {"FLAT", "IVF_FLAT", "IVF_PQ", "HNSW", "GPU_CAGRA", "GPU_CUVS_CAGRA"}) {
             const std::string name = n;
             map_[name] = [name](const int32_t&, const void*) {
                 return Index<IndexNode>(std::static_pointer_cast<IndexNode>(std::make_shared<B200IndexNode>(name)));

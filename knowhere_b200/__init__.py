@@ -395,7 +395,7 @@ class Index:
     def last_stage_info(self):
         v = np.zeros(4, np.float32)
         _check(self.L.kb2_index_last_stage_info(self.h, _ptr(v)))
-        return dict(stage_ms=float(v[0]), kernel_ms=float(v[1]), engine=("scan", "tc", "large_k", "hnsw_wide")[int(round(v[2]))], comm_ms=float(v[3]))
+        return dict(stage_ms=float(v[0]), kernel_ms=float(v[1]), engine=("scan", "tc", "large_k", "hnsw_wide", "cagra")[int(round(v[2]))], comm_ms=float(v[3]))
 
     def last_kernel_ms(self):
         v = ctypes.c_float()

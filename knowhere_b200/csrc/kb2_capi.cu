@@ -8,6 +8,7 @@
 #include <cstring>
 #include <memory>
 
+#include "kb2_cagra.cuh"
 #include "kb2_fourcc.h"
 #include "kb2_hnsw.cuh"
 #include "kb2_index.cuh"
@@ -173,6 +174,16 @@ kb2_index_create(const char* index_type, int metric, int dim, const char* json_c
             hn->M = (int)cfg.get_int("M", 30);
             hn->efConstruction = (int)cfg.get_int("efConstruction", 360);
             KB2_REQUIRE(hn->M >= 2 && hn->M <= 2048, KB2_OUT_OF_RANGE_IN_JSON, "M out of range");
+        } else if (t == "GPU_CAGRA" || t == "GPU_CUVS_CAGRA") {
+            // gpu_cuvs_cagra_config.h; build_algo, nn_descent_niter, cache_dataset_on_device and adapt_for_cpu are
+            // accepted and have no effect (the intermediate graph is always the exact k-NN graph)
+            auto* cg = new CagraIndex();
+            ix.reset(cg);
+            cg->igd = (int)cfg.get_int("intermediate_graph_degree", 128);
+            cg->gd = (int)cfg.get_int("graph_degree", 64);
+            KB2_REQUIRE(cg->igd >= 1 && cg->igd <= kCagraMaxIgd, KB2_OUT_OF_RANGE_IN_JSON, "intermediate_graph_degree out of range (1..1007)");
+            KB2_REQUIRE(cg->gd >= 1 && cg->gd <= kCagraMaxGd && cg->gd <= cg->igd, KB2_OUT_OF_RANGE_IN_JSON,
+                        "graph_degree out of range (1..256, and at most intermediate_graph_degree)");
         } else {
             throw Error(KB2_INVALID_ARGS, "unknown index type " + t);
         }
@@ -211,6 +222,7 @@ kb2_index_set_shard(kb2_index_t h, int rank, int world) {
         IndexBase* ix = ix_of(h);
         KB2_REQUIRE(world >= 1 && rank >= 0 && rank < world, KB2_INVALID_ARGS, "bad shard rank/world");
         KB2_REQUIRE(ix->count() == 0, KB2_INVALID_ARGS, "set_shard must precede add/import");
+        KB2_REQUIRE(world == 1 || !dynamic_cast<CagraIndex*>(ix), KB2_NOT_IMPLEMENTED, "GPU_CAGRA: sharding is not implemented");
         ix->shard_rank = rank;
         ix->shard_world = world;
     });
@@ -450,6 +462,7 @@ kb2_hnsw_import(kb2_index_t h, int64_t n, const float* vectors, const int32_t* l
         auto* hn = ix_as<HnswIndex>(h, "HNSW");
         std::lock_guard<std::mutex> lk(hn->mu);
         KB2_CUDA_CHECK(cudaSetDevice(hn->device));
+        KB2_REQUIRE(!dynamic_cast<CagraIndex*>(hn), KB2_NOT_IMPLEMENTED, "GPU_CAGRA builds its own graph: import into an HNSW handle");
         // the attached document offsets and doc_of_row describe the current rows
         KB2_REQUIRE(!hn->emb_list, KB2_NOT_IMPLEMENTED, "import into an emb-list index");
         hn->import_graph(n, vectors, levels, offsets, neighbors, cum_nneighbor, n_cum, entry_point, max_level);
@@ -619,6 +632,18 @@ index_to_faiss(IndexBase& ix, FaissIndexData& o) {
             KB2_CUDA_CHECK(cudaStreamSynchronize(iv->stream));
             o.k_factor = 1.f;
         }
+    } else if (auto* cg = dynamic_cast<CagraIndex*>(&ix)) {
+        // the graph as a one-level HNSW (what the reference's CPU HNSW node loads: build on the GPU, serve on the CPU)
+        o.kind = "HNSW";
+        o.xb = cg->h_vecs;
+        o.levels = cg->h_levels;
+        o.neighbors = cg->h_neighbors;
+        o.offsets.assign(cg->h_offsets.begin(), cg->h_offsets.end());
+        o.entry_point = cg->entry_point;
+        o.max_level = cg->max_level;
+        o.efConstruction = cg->igd;
+        o.cum = cg->h_cum;
+        o.assign_probas.assign(1, 1.0);
     } else if (auto* hn = dynamic_cast<HnswIndex*>(&ix)) {
         KB2_REQUIRE(!hn->custom_labels, KB2_NOT_IMPLEMENTED, "faiss stream: HNSW with custom ids");
         o.xb = hn->h_vecs;
@@ -742,6 +767,10 @@ kb2_index_get_meta(kb2_index_t h, char* json_out, size_t cap) {
         if (auto* iv = dynamic_cast<IvfIndex*>(ix)) {
             s += ", \"nlist\": " + std::to_string(iv->nlist);
             if (iv->is_pq) s += ", \"m\": " + std::to_string(iv->M) + ", \"nbits\": " + std::to_string(iv->nbits) + ", \"refine\": " + (iv->refine ? "true" : "false");
+        } else if (auto* cg = dynamic_cast<CagraIndex*>(ix)) {
+            s += ", \"intermediate_graph_degree\": " + std::to_string(cg->igd) + ", \"graph_degree\": " + std::to_string(cg->gd) +
+                 ", \"degree\": " + std::to_string(cg->degree()) + ", \"build_ms\": [" + std::to_string(cg->build_ms[0]) + ", " +
+                 std::to_string(cg->build_ms[1]) + ", " + std::to_string(cg->build_ms[2]) + "]";
         } else if (auto* hn = dynamic_cast<HnswIndex*>(ix)) {
             s += ", \"M\": " + std::to_string(hn->M) + ", \"efConstruction\": " + std::to_string(hn->efConstruction) +
                  ", \"max_level\": " + std::to_string(hn->max_level) + ", \"entry_point\": " + std::to_string(hn->entry_point);

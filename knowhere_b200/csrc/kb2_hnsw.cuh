@@ -1035,19 +1035,21 @@ hnsw_select_kernel(HnswBuildParams p) {
 }
 
 // reverse links: for every selected neighbour s of the new node q, add q to s's row (under s's lock); a full row is
-// re-selected among its members + q with the heuristic, centre s.  dynamic smem per warp: 2 * d floats + 3 * 64 words
+// re-selected among its members + q with the heuristic, centre s.  dynamic smem per warp: 2 * d floats + 3 * kLinkSlots
+// words (a full row of 2M = 64 members plus q is 65 candidates)
+constexpr int kLinkSlots = 72;
 template <int METRIC>
 __global__ void __launch_bounds__(kBuildWarps * 32)
 hnsw_link_kernel(HnswBuildParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dpad = (p.d + 3) & ~3;
-    unsigned char* mine = smem_raw + (size_t)warp * ((size_t)dpad * 8 + 768);
+    unsigned char* mine = smem_raw + (size_t)warp * ((size_t)dpad * 8 + 3 * kLinkSlots * 4);
     float* s_s = (float*)mine;                       // vector of the centre s
     float* s_c = s_s + dpad;                         // vector of the candidate being tested
-    int32_t* s_id = (int32_t*)(s_c + dpad);          // [64] candidate ids (sorted by key to s)
-    float* s_key = (float*)(s_id + 64);              // [64]
-    int32_t* s_sel = (int32_t*)(s_key + 64);         // [64] kept ids
+    int32_t* s_id = (int32_t*)(s_c + dpad);          // [kLinkSlots] candidate ids (sorted by key to s)
+    float* s_key = (float*)(s_id + kLinkSlots);      // [kLinkSlots]
+    int32_t* s_sel = (int32_t*)(s_key + kLinkSlots); // [kLinkSlots] kept ids
     const int w = blockIdx.x * kBuildWarps + warp;
     if (w >= p.nb) return;
     const int32_t q = p.batch[w];
@@ -1477,7 +1479,7 @@ struct HnswIndex : IndexBase {
         d_next.ensure(1);
         const int dpad = (dim + 3) & ~3;
         const size_t smem_sel = (size_t)kBuildWarps * ((size_t)dpad * 4 + 256);
-        const size_t smem_link = (size_t)kBuildWarps * ((size_t)dpad * 8 + 768);
+        const size_t smem_link = (size_t)kBuildWarps * ((size_t)dpad * 8 + 3 * kLinkSlots * 4);
         KB2_REQUIRE(smem_link <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "HNSW GPU build: dim too large");
         int64_t level_count[64] = {0};   // nodes with (levels - 1) >= L
         for (int L = 0; L <= max_level && L < 64; L++) {

@@ -9,6 +9,7 @@
 #include <memory>
 
 #include "kb2_blob.h"
+#include "kb2_cagra.cuh"
 #include "kb2_emb_list_index.cuh"
 #include "kb2_hnsw.cuh"
 #include "kb2_index.cuh"
@@ -24,6 +25,7 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
     IvfIndex* iv = dynamic_cast<IvfIndex*>(&ix);
     HnswIndex* hn = dynamic_cast<HnswIndex*>(&ix);
     KB2_REQUIRE(fi || iv || hn, KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
+    KB2_REQUIRE(!dynamic_cast<CagraIndex*>(&ix), KB2_NOT_IMPLEMENTED, "RangeSearch is not implemented on GPU_CAGRA");
     KB2_REQUIRE(ix.count() > 0, KB2_EMPTY_INDEX, "index is empty");
     if (nq == 0) {
         *out_lims = (int64_t*)calloc(1, sizeof(int64_t));
@@ -279,6 +281,8 @@ serialize_index(IndexBase& ix, std::vector<uint8_t>& blob) {
                 w.put_bytes(rv.data(), rv.size() * 4);
             }
         }
+    } else if (auto* cg = dynamic_cast<CagraIndex*>(&ix)) {
+        cg->serialize(w);
     } else if (auto* hn = dynamic_cast<HnswIndex*>(&ix)) {
         hn->serialize(w);
     } else {
@@ -367,6 +371,12 @@ deserialize_index(const uint8_t* blob, size_t size, int device) {
         }
         const bool with_raw = iv->is_pq && iv->refine;
         iv->import_finish(with_raw ? raw_rows.data() : nullptr, with_raw ? (int64_t)(raw_rows.size() / dim) : 0, true);
+    } else if (type == "GPU_CAGRA" || type == "GPU_CUVS_CAGRA") {
+        auto* cg = new CagraIndex();
+        ix.reset(cg);
+        cg->type = type; cg->metric = metric; cg->dim = dim; cg->device = device;
+        cg->init_common();
+        cg->deserialize(r);
     } else if (type == "HNSW") {
         auto* hn = new HnswIndex();
         ix.reset(hn);
