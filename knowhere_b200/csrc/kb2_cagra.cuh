@@ -583,21 +583,62 @@ struct CagraIndex : HnswIndex {
         if (timing) KB2_CUDA_CHECK(cudaEventElapsedTime(&last_kernel_ms, ev0, ev1));
     }
 
+    // gpu_cuvs_cagra_config.h; build_algo, nn_descent_niter, cache_dataset_on_device and adapt_for_cpu are accepted and have
+    // no effect (the intermediate graph is always the exact k-NN graph)
     void
-    serialize(BlobWriter& w) {
+    configure(const JsonObj& cfg) override {
+        igd = (int)cfg.get_int("intermediate_graph_degree", 128);
+        gd = (int)cfg.get_int("graph_degree", 64);
+        KB2_REQUIRE(igd >= 1 && igd <= kCagraMaxIgd, KB2_OUT_OF_RANGE_IN_JSON, "intermediate_graph_degree out of range (1..1007)");
+        KB2_REQUIRE(gd >= 1 && gd <= kCagraMaxGd && gd <= igd, KB2_OUT_OF_RANGE_IN_JSON,
+                    "graph_degree out of range (1..256, and at most intermediate_graph_degree)");
+    }
+
+    void
+    save(BlobWriter& w) override {
         w.put<int32_t>(igd);
         w.put<int32_t>(gd);
-        HnswIndex::serialize(w);
+        HnswIndex::save(w);
     }
     void
-    deserialize(BlobReader& r) {
+    load(BlobReader& r) override {
         igd = r.get<int32_t>();
         gd = r.get<int32_t>();
-        HnswIndex::deserialize(r);
+        HnswIndex::load(r);
         KB2_REQUIRE(max_level == 0 && h_cum.size() == 2 && !custom_labels, KB2_INVALID_BINARY_SET, "GPU_CAGRA: bad graph in blob");
         for (int64_t i = 0; i < n; i++)
             KB2_REQUIRE(h_offsets[i] == i * h_cum[1], KB2_INVALID_BINARY_SET, "GPU_CAGRA: bad graph in blob");
     }
+
+    // the graph as a one-level HNSW (what the reference's CPU HNSW node loads: build on the GPU, serve on the CPU)
+    void
+    to_faiss(FaissIndexData& o) override {
+        o.kind = "HNSW";
+        o.xb = h_vecs;
+        o.levels = h_levels;
+        o.neighbors = h_neighbors;
+        o.offsets.assign(h_offsets.begin(), h_offsets.end());
+        o.entry_point = entry_point;
+        o.max_level = max_level;
+        o.efConstruction = igd;
+        o.cum = h_cum;
+        o.assign_probas.assign(1, 1.0);
+    }
+
+    void
+    append_meta(std::string& s) const override {
+        s += ", \"intermediate_graph_degree\": " + std::to_string(igd) + ", \"graph_degree\": " + std::to_string(gd) +
+             ", \"degree\": " + std::to_string(degree()) + ", \"build_ms\": [" + std::to_string(build_ms[0]) + ", " +
+             std::to_string(build_ms[1]) + ", " + std::to_string(build_ms[2]) + "]";
+    }
+
+    void
+    refuse(Op op) const override {
+        KB2_REQUIRE(op != kShard, KB2_NOT_IMPLEMENTED, "GPU_CAGRA: sharding is not implemented");
+        KB2_REQUIRE(op != kHnswImport, KB2_NOT_IMPLEMENTED, "GPU_CAGRA builds its own graph: import into an HNSW handle");
+        KB2_REQUIRE(op != kRangeSearch, KB2_NOT_IMPLEMENTED, "RangeSearch is not implemented on GPU_CAGRA");
+    }
+    bool takes_emb_list() const override { return false; }
 };
 
 }  // namespace kb2

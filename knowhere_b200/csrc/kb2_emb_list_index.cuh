@@ -126,7 +126,7 @@ inline void
 set_emb_list(IndexBase& ix, std::vector<int64_t> lims, int metric) {
     auto* iv = dynamic_cast<IvfIndex*>(&ix);
     auto* hn = dynamic_cast<HnswIndex*>(&ix);
-    KB2_REQUIRE((iv && !iv->is_pq) || (hn && hn->type == "HNSW"), KB2_INVALID_METRIC_TYPE, "emb-lists are supported on HNSW and IVF_FLAT only");
+    KB2_REQUIRE(ix.takes_emb_list(), KB2_INVALID_METRIC_TYPE, "emb-lists are supported on HNSW and IVF_FLAT only");
     KB2_REQUIRE(metric == KB2_METRIC_MAX_SIM_L2 || metric == KB2_METRIC_MAX_SIM_IP || metric == KB2_METRIC_MAX_SIM_COSINE,
                 KB2_INVALID_METRIC_TYPE, "metric must be MAX_SIM_L2, MAX_SIM_IP or MAX_SIM_COSINE");
     KB2_REQUIRE(emb_list_metric_pairs(ix, metric), KB2_INVALID_METRIC_TYPE,

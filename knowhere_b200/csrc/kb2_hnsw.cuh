@@ -1933,7 +1933,14 @@ struct HnswIndex : IndexBase {
     }
 
     void
-    serialize(BlobWriter& w) {
+    configure(const JsonObj& cfg) override {
+        M = (int)cfg.get_int("M", 30);
+        efConstruction = (int)cfg.get_int("efConstruction", 360);
+        KB2_REQUIRE(M >= 2 && M <= 2048, KB2_OUT_OF_RANGE_IN_JSON, "M out of range");
+    }
+
+    void
+    save(BlobWriter& w) override {
         w.put<int32_t>(M);
         w.put<int32_t>(efConstruction);
         w.put<int64_t>(n);
@@ -1949,7 +1956,7 @@ struct HnswIndex : IndexBase {
         if (custom_labels) w.put_bytes(h_labels.data(), h_labels.size() * 8);
     }
     void
-    deserialize(BlobReader& r) {
+    load(BlobReader& r) override {
         M = r.get<int32_t>();
         efConstruction = r.get<int32_t>();
         n = r.get<int64_t>();
@@ -1977,6 +1984,59 @@ struct HnswIndex : IndexBase {
         validate_graph();
         uploaded = false;
     }
+
+    void
+    to_faiss(FaissIndexData& o) override {
+        KB2_REQUIRE(!custom_labels, KB2_NOT_IMPLEMENTED, "faiss stream: HNSW with custom ids");
+        o.xb = h_vecs;
+        o.levels = h_levels;
+        o.neighbors = h_neighbors;
+        o.offsets.assign(h_offsets.begin(), h_offsets.end());
+        o.entry_point = entry_point;
+        o.max_level = max_level;
+        o.efConstruction = efConstruction;
+        // K/impl/HNSW.cpp:78-89 set_default_probas(M, 1 / ln M): the full level table, of which h_cum is a prefix
+        const double mult = 1.0 / std::log((double)M);
+        int nn = 0;
+        o.cum.assign(1, 0);
+        for (int level = 0;; level++) {
+            const double proba = std::exp(-level / mult) * (1 - std::exp(-1 / mult));
+            if (proba < 1e-9) break;
+            o.assign_probas.push_back(proba);
+            nn += level == 0 ? M * 2 : M;
+            o.cum.push_back(nn);
+        }
+        KB2_REQUIRE(o.cum.size() >= h_cum.size(), KB2_INTERNAL_ERROR, "HNSW level table shorter than the graph's");
+        for (size_t i = 0; i < h_cum.size(); i++)
+            KB2_REQUIRE(o.cum[i] == h_cum[i], KB2_NOT_IMPLEMENTED, "faiss stream: non-default HNSW link counts");
+    }
+    void
+    from_faiss(const FaissIndexData& o) override {
+        M = o.cum.size() >= 2 ? o.cum[1] / 2 : 16;
+        efConstruction = o.efConstruction;
+        std::vector<int64_t> off(o.offsets.begin(), o.offsets.end());
+        std::vector<float> normed;
+        const float* xb = o.xb.data();
+        if (o.cosine) {   // the reference keeps raw rows + norms (IHN9); this core keeps unit rows
+            normed = o.xb;
+            for (int64_t i = 0; i < o.ntotal; i++) {
+                double s2 = 0;
+                for (int j = 0; j < o.d; j++) s2 += (double)normed[i * o.d + j] * normed[i * o.d + j];
+                const float inv = s2 > 0 ? (float)(1.0 / std::sqrt(s2)) : 1.f;
+                for (int j = 0; j < o.d; j++) normed[i * o.d + j] *= inv;
+            }
+            xb = normed.data();
+        }
+        import_graph(o.ntotal, xb, o.levels.data(), off.data(), o.neighbors.data(), o.cum.data(), (int)o.cum.size(), o.entry_point,
+                     o.max_level);
+    }
+
+    void
+    append_meta(std::string& s) const override {
+        s += ", \"M\": " + std::to_string(M) + ", \"efConstruction\": " + std::to_string(efConstruction) +
+             ", \"max_level\": " + std::to_string(max_level) + ", \"entry_point\": " + std::to_string(entry_point);
+    }
+    bool takes_emb_list() const override { return true; }
 };
 
 }  // namespace kb2

@@ -1,4 +1,4 @@
-// kb2_index.cuh — host-side index objects behind the C ABI (FLAT, IVF_FLAT, IVF_PQ).
+// kb2_index.cuh — host-side index objects behind the C ABI (the IndexBase interface, FLAT, IVF_FLAT, IVF_PQ).
 // They play the role of the reference's IndexNode implementations
 //   FlatIndexNode  src/index/flat/flat.cc:33-427
 //   IvfIndexNode   src/index/ivf/ivf.cc:68-1972   (IVF_FLAT + IVF_PQ branches)
@@ -13,6 +13,7 @@
 
 #include "kb2_build.cuh"
 #include "kb2_comm.h"
+#include "kb2_fourcc.h"
 #include "kb2_gemm_tc.cuh"
 #include "kb2_ivf.cuh"
 #include "kb2_ivfpq_tc.cuh"
@@ -151,6 +152,16 @@ struct IndexBase {
         KB2_CUDA_CHECK(cudaEventRecord(ev_in, cudaStreamLegacy));
         KB2_CUDA_CHECK(cudaStreamWaitEvent(stream, ev_in, 0));
     }
+    // a new index: type, metric (COSINE: IP over rows normalised on entry), dim and device, then its stream and events
+    void
+    init(const std::string& t, int m, int d, int dev) {
+        type = t;
+        cosine = (m == KB2_METRIC_COSINE);
+        metric = cosine ? KB2_METRIC_IP : m;
+        dim = d;
+        device = dev;
+        init_common();
+    }
     void
     init_common() {
         KB2_CUDA_CHECK(cudaSetDevice(device));
@@ -222,6 +233,21 @@ struct IndexBase {
     virtual void get_vectors(const int64_t* ids, int64_t n, float* out) {
         throw Error(KB2_NOT_IMPLEMENTED, "GetVectorByIds not supported by this index");
     }
+
+    // build keys of kb2_index_create
+    virtual void configure(const JsonObj&) {}
+    // the type's section of the KB2I container (kb2_range.cuh writes the framing around it)
+    virtual void save(BlobWriter& w) = 0;
+    virtual void load(BlobReader& r) = 0;
+    // the faiss fourcc stream (the reference's BinarySet payload): fields beyond the common header
+    virtual void to_faiss(FaissIndexData&) { throw Error(KB2_NOT_IMPLEMENTED, "faiss stream: unknown index class"); }
+    virtual void from_faiss(const FaissIndexData&) { throw Error(KB2_NOT_IMPLEMENTED, "faiss stream: unsupported index kind"); }
+    // the type's fields of GetIndexMeta, appended to the common JSON prefix
+    virtual void append_meta(std::string&) const {}
+    // operations a type may leave out: refuse() throws the type's status and message where the operation starts
+    enum Op { kShard, kHnswImport, kRangeSearch };
+    virtual void refuse(Op) const {}
+    virtual bool takes_emb_list() const { return false; }   // kb2_index_set_emb_list
 };
 
 // ============================================================================================
@@ -670,6 +696,45 @@ struct FlatIndex : IndexBase {
             KB2_CUDA_CHECK(cudaMemcpyAsync(out + i * dim, base.p + h[i] * dim, (size_t)dim * 4, cudaMemcpyDefault, stream));
         }
         KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
+    }
+
+    void
+    save(BlobWriter& w) override {
+        const int64_t n = count();
+        w.put<int64_t>(n);
+        w.put<int32_t>(custom_labels ? 1 : 0);
+        std::vector<float> h((size_t)n * dim);
+        if (n) KB2_CUDA_CHECK(cudaMemcpy(h.data(), base.p, h.size() * 4, cudaMemcpyDeviceToHost));
+        w.put_bytes(h.data(), h.size() * 4);
+        if (custom_labels) {
+            std::vector<int64_t> l(n);
+            if (n) KB2_CUDA_CHECK(cudaMemcpy(l.data(), labels.p, n * 8, cudaMemcpyDeviceToHost));
+            w.put_bytes(l.data(), n * 8);
+        }
+    }
+    void
+    load(BlobReader& r) override {
+        const int64_t n = r.get<int64_t>();
+        KB2_REQUIRE(n >= 0 && (uint64_t)n <= r.n / ((size_t)dim * 4), KB2_INVALID_BINARY_SET, "bad row count in blob");
+        const int custom = r.get<int32_t>();
+        const float* data = (const float*)r.get_bytes((size_t)n * dim * 4);
+        const int64_t* l = custom ? (const int64_t*)r.get_bytes((size_t)n * 8) : nullptr;
+        // blob memory may be unaligned: stage through vectors
+        std::vector<float> hd((size_t)n * dim);
+        memcpy(hd.data(), data, hd.size() * 4);
+        std::vector<int64_t> hl;
+        if (custom) { hl.resize(n); memcpy(hl.data(), l, n * 8); }
+        add(hd.data(), n, custom ? hl.data() : nullptr);
+    }
+    void
+    to_faiss(FaissIndexData& o) override {
+        KB2_REQUIRE(!custom_labels, KB2_NOT_IMPLEMENTED, "faiss stream: FLAT with custom ids");
+        o.xb.resize((size_t)o.ntotal * o.d);
+        if (o.ntotal) KB2_CUDA_CHECK(cudaMemcpy(o.xb.data(), base.p, o.xb.size() * 4, cudaMemcpyDeviceToHost));
+    }
+    void
+    from_faiss(const FaissIndexData& o) override {
+        if (o.ntotal) add(o.cosine ? normalized(o.xb.data(), o.ntotal) : o.xb.data(), o.ntotal, nullptr);
     }
 };
 
@@ -1895,6 +1960,162 @@ struct IvfIndex : IndexBase {
             KB2_CUDA_CHECK(cudaMemcpy(cds, codes.p + (size_t)off * M, (size_t)len * M, cudaMemcpyDeviceToHost));
         }
     }
+
+    void
+    configure(const JsonObj& cfg) override {
+        nlist = cfg.get_int("nlist", 128);
+        KB2_REQUIRE(nlist >= 1 && nlist <= 65536 * 16, KB2_OUT_OF_RANGE_IN_JSON, "nlist out of range");
+        if (!is_pq) return;
+        KB2_REQUIRE(cfg.has("m"), KB2_INVALID_PARAM_IN_JSON, "IVF_PQ requires m");
+        M = (int)cfg.get_int("m", 0);
+        nbits = (int)cfg.get_int("nbits", 8);
+        KB2_REQUIRE(M >= 1 && dim % M == 0, KB2_INVALID_ARGS, "dim must be a multiple of m");
+        KB2_REQUIRE(nbits >= 1 && nbits <= 24, KB2_OUT_OF_RANGE_IN_JSON, "nbits out of range");
+        refine = cfg.get_bool("refine", false);
+        if (refine) {
+            std::string rt = cfg.get_str("refine_type", "flat");
+            for (auto& ch : rt) ch = (char)tolower((unsigned char)ch);
+            if (rt == "flat" || rt == "fp32" || rt == "float32" || rt == "data_view") refine_kind = 0;
+            else if (rt == "fp16" || rt == "float16") refine_kind = 1;
+            else if (rt == "bf16" || rt == "bfloat16") refine_kind = 2;
+            else throw Error(KB2_NOT_IMPLEMENTED, "refine_type " + rt + " is not implemented (flat / fp16 / bf16 are)");
+        }
+    }
+
+    void
+    save(BlobWriter& w) override {
+        KB2_REQUIRE(trained, KB2_INDEX_NOT_TRAINED, "index not trained");
+        KB2_REQUIRE(shard_world == 1, KB2_NOT_IMPLEMENTED, "serialising a shard");
+        seal();
+        w.put<int64_t>(nlist);
+        w.put<int32_t>(M);
+        w.put<int32_t>(nbits);
+        w.put<int32_t>(refine ? 1 + refine_kind : 0);   // 0 none, 1 fp32, 2 fp16, 3 bf16 refine store
+        DevBuf<float> dec;
+        const float* v32 = (is_pq && refine) ? vecs_f32(dec) : nullptr;
+        if (v32) KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
+        std::vector<float> c((size_t)nlist * dim);
+        KB2_CUDA_CHECK(cudaMemcpy(c.data(), centroids.p, c.size() * 4, cudaMemcpyDeviceToHost));
+        w.put_bytes(c.data(), c.size() * 4);
+        if (is_pq) {
+            std::vector<float> pc((size_t)M * 256 * dsub);
+            KB2_CUDA_CHECK(cudaMemcpy(pc.data(), pqc.p, pc.size() * 4, cudaMemcpyDeviceToHost));
+            w.put_bytes(pc.data(), pc.size() * 4);
+        }
+        const size_t cs = is_pq ? (size_t)M : (size_t)dim * 4;
+        for (int64_t l = 0; l < nlist; l++) {
+            const int64_t len = h_list_len[l];
+            w.put<int64_t>(len);
+            if (!len) continue;
+            std::vector<int64_t> ids(len);
+            std::vector<uint8_t> cd((size_t)len * cs);
+            export_list(l, ids.data(), cd.data());
+            w.put_bytes(ids.data(), len * 8);
+            w.put_bytes(cd.data(), cd.size());
+            if (is_pq && refine) {
+                std::vector<float> rv((size_t)len * dim);
+                KB2_CUDA_CHECK(cudaMemcpy(rv.data(), v32 + h_list_off[l] * dim, rv.size() * 4, cudaMemcpyDeviceToHost));
+                w.put_bytes(rv.data(), rv.size() * 4);
+            }
+        }
+    }
+    void
+    load(BlobReader& r) override {
+        const int64_t nl = r.get<int64_t>();
+        M = r.get<int32_t>();
+        nbits = r.get<int32_t>();
+        const int rf = r.get<int32_t>();
+        KB2_REQUIRE(rf >= 0 && rf <= 3, KB2_INVALID_BINARY_SET, "bad refine field in blob");
+        refine = rf != 0;
+        refine_kind = rf ? rf - 1 : 0;
+        KB2_REQUIRE(nl >= 1 && (uint64_t)nl <= r.n / ((size_t)dim * 4), KB2_INVALID_BINARY_SET, "bad nlist in blob");
+        if (is_pq) KB2_REQUIRE(M > 0 && dim % M == 0 && nbits == 8, KB2_INVALID_BINARY_SET, "bad m / nbits in blob");
+        std::vector<float> c((size_t)nl * dim);
+        memcpy(c.data(), r.get_bytes(c.size() * 4), c.size() * 4);
+        std::vector<float> pc;
+        if (is_pq) {
+            pc.resize((size_t)M * 256 * (dim / M));
+            memcpy(pc.data(), r.get_bytes(pc.size() * 4), pc.size() * 4);
+        }
+        import_begin(nl, c.data(), is_pq ? pc.data() : nullptr);
+        const size_t cs = is_pq ? (size_t)M : (size_t)dim * 4;
+        const bool with_raw = is_pq && refine;
+        std::vector<float> raw_rows;  // import order
+        for (int64_t l = 0; l < nl; l++) {
+            const int64_t len = r.get<int64_t>();
+            KB2_REQUIRE(len >= 0 && (uint64_t)len <= r.n / 8, KB2_INVALID_BINARY_SET, "bad list length in blob");
+            if (!len) continue;
+            std::vector<int64_t> ids(len);
+            memcpy(ids.data(), r.get_bytes(len * 8), len * 8);
+            const uint8_t* cd = r.get_bytes((size_t)len * cs);
+            import_list(l, len, ids.data(), cd);
+            if (with_raw) {
+                const uint8_t* rv = r.get_bytes((size_t)len * dim * 4);
+                const size_t o = raw_rows.size();
+                raw_rows.resize(o + (size_t)len * dim);
+                memcpy(raw_rows.data() + o, rv, (size_t)len * dim * 4);
+            }
+        }
+        import_finish(with_raw ? raw_rows.data() : nullptr, with_raw ? (int64_t)(raw_rows.size() / dim) : 0, true);
+    }
+
+    void
+    to_faiss(FaissIndexData& o) override {
+        KB2_REQUIRE(trained, KB2_INDEX_NOT_TRAINED, "index not trained");
+        seal();
+        o.nlist = nlist;
+        o.nprobe = 1;
+        o.centroids.resize((size_t)nlist * o.d);
+        KB2_CUDA_CHECK(cudaMemcpy(o.centroids.data(), centroids.p, o.centroids.size() * 4, cudaMemcpyDeviceToHost));
+        o.M = M;
+        o.code_size = is_pq ? (uint64_t)M : (uint64_t)o.d * 4;
+        if (is_pq) {
+            KB2_REQUIRE(nbits == 8, KB2_NOT_IMPLEMENTED, "faiss stream: nbits != 8");
+            o.pq_centroids.resize((size_t)256 * o.d);
+            KB2_CUDA_CHECK(cudaMemcpy(o.pq_centroids.data(), pqc.p, o.pq_centroids.size() * 4, cudaMemcpyDeviceToHost));
+        }
+        o.list_ids.assign(nlist, {});
+        o.list_codes.assign(nlist, {});
+        for (int64_t l = 0; l < nlist; l++) {
+            const int64_t len = h_list_len[l];
+            if (!len) continue;
+            o.list_ids[l].resize(len);
+            o.list_codes[l].resize((size_t)len * o.code_size);
+            export_list(l, o.list_ids[l].data(), o.list_codes[l].data());
+        }
+        o.has_refine = is_pq && refine;
+        if (o.has_refine) {
+            KB2_REQUIRE(!custom_labels, KB2_NOT_IMPLEMENTED, "faiss stream: refine store with custom ids");
+            KB2_REQUIRE(refine_kind == 0, KB2_NOT_IMPLEMENTED, "faiss stream: only a flat fp32 refine store is written");
+            // refine store in id order: row r lives at position pos_of_row[r]
+            DevBuf<float> byrow;
+            byrow.ensure((size_t)std::max<int64_t>(o.ntotal, 1) * o.d);
+            gather_rows_kernel<<<grid1d(o.ntotal * 32, 256), 256, 0, stream>>>(vecs.p, pos_of_row.p, o.ntotal, o.d, o.d, byrow.p);
+            o.refine_xb.resize((size_t)o.ntotal * o.d);
+            KB2_CUDA_CHECK(cudaMemcpyAsync(o.refine_xb.data(), byrow.p, o.refine_xb.size() * 4, cudaMemcpyDeviceToHost, stream));
+            KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
+            o.k_factor = 1.f;
+        }
+    }
+    void
+    from_faiss(const FaissIndexData& o) override {
+        KB2_REQUIRE(!o.cosine, KB2_NOT_IMPLEMENTED, "faiss stream: cosine IVF indexes are not supported");
+        nlist = o.nlist;
+        M = o.M;
+        nbits = 8;
+        refine = o.has_refine;
+        import_begin(o.nlist, o.centroids.data(), is_pq ? o.pq_centroids.data() : nullptr);
+        for (int64_t l = 0; l < o.nlist; l++)
+            if (!o.list_ids[l].empty()) import_list(l, (int64_t)o.list_ids[l].size(), o.list_ids[l].data(), o.list_codes[l].data());
+        import_finish(o.has_refine ? o.refine_xb.data() : nullptr, o.has_refine ? o.ntotal : 0);
+    }
+
+    void
+    append_meta(std::string& s) const override {
+        s += ", \"nlist\": " + std::to_string(nlist);
+        if (is_pq) s += ", \"m\": " + std::to_string(M) + ", \"nbits\": " + std::to_string(nbits) + ", \"refine\": " + (refine ? "true" : "false");
+    }
+    bool takes_emb_list() const override { return !is_pq; }
 };
 
 }  // namespace kb2

@@ -25,7 +25,7 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
     IvfIndex* iv = dynamic_cast<IvfIndex*>(&ix);
     HnswIndex* hn = dynamic_cast<HnswIndex*>(&ix);
     KB2_REQUIRE(fi || iv || hn, KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
-    KB2_REQUIRE(!dynamic_cast<CagraIndex*>(&ix), KB2_NOT_IMPLEMENTED, "RangeSearch is not implemented on GPU_CAGRA");
+    ix.refuse(IndexBase::kRangeSearch);
     KB2_REQUIRE(ix.count() > 0, KB2_EMPTY_INDEX, "index is empty");
     if (nq == 0) {
         *out_lims = (int64_t*)calloc(1, sizeof(int64_t));
@@ -226,6 +226,20 @@ merge_topk_device(int metric, int world, int64_t nq, int k, const int64_t* in_id
 // stream inside a BinarySet — K/impl/index_write.cpp:716-745; wire compatibility is SURVEY §8f
 // rank 2 and not claimed here.)
 // ------------------------------------------------------------------------------------------
+// a fresh index of the named type (before IndexBase::init), or null when the type is unknown
+inline std::unique_ptr<IndexBase>
+make_index(const std::string& type) {
+    if (type == "FLAT") return std::make_unique<FlatIndex>();
+    if (type == "IVF_FLAT" || type == "IVF_PQ") {
+        auto iv = std::make_unique<IvfIndex>();
+        iv->is_pq = (type == "IVF_PQ");
+        return iv;
+    }
+    if (type == "HNSW") return std::make_unique<HnswIndex>();
+    if (type == "GPU_CAGRA" || type == "GPU_CUVS_CAGRA") return std::make_unique<CagraIndex>();
+    return nullptr;
+}
+
 inline void
 serialize_index(IndexBase& ix, std::vector<uint8_t>& blob) {
     BlobWriter w{blob};
@@ -234,60 +248,7 @@ serialize_index(IndexBase& ix, std::vector<uint8_t>& blob) {
     w.put_str(ix.type);
     w.put<int32_t>(ix.cosine ? KB2_METRIC_COSINE : ix.metric);
     w.put<int32_t>(ix.dim);
-    if (auto* fi = dynamic_cast<FlatIndex*>(&ix)) {
-        const int64_t n = fi->count();
-        w.put<int64_t>(n);
-        w.put<int32_t>(fi->custom_labels ? 1 : 0);
-        std::vector<float> h((size_t)n * ix.dim);
-        if (n) KB2_CUDA_CHECK(cudaMemcpy(h.data(), fi->base.p, h.size() * 4, cudaMemcpyDeviceToHost));
-        w.put_bytes(h.data(), h.size() * 4);
-        if (fi->custom_labels) {
-            std::vector<int64_t> l(n);
-            if (n) KB2_CUDA_CHECK(cudaMemcpy(l.data(), fi->labels.p, n * 8, cudaMemcpyDeviceToHost));
-            w.put_bytes(l.data(), n * 8);
-        }
-    } else if (auto* iv = dynamic_cast<IvfIndex*>(&ix)) {
-        KB2_REQUIRE(iv->trained, KB2_INDEX_NOT_TRAINED, "index not trained");
-        KB2_REQUIRE(iv->shard_world == 1, KB2_NOT_IMPLEMENTED, "serialising a shard");
-        iv->seal();
-        w.put<int64_t>(iv->nlist);
-        w.put<int32_t>(iv->M);
-        w.put<int32_t>(iv->nbits);
-        w.put<int32_t>(iv->refine ? 1 + iv->refine_kind : 0);   // 0 none, 1 fp32, 2 fp16, 3 bf16 refine store
-        DevBuf<float> dec;
-        const float* v32 = (iv->is_pq && iv->refine) ? iv->vecs_f32(dec) : nullptr;
-        if (v32) KB2_CUDA_CHECK(cudaStreamSynchronize(iv->stream));
-        std::vector<float> c((size_t)iv->nlist * ix.dim);
-        KB2_CUDA_CHECK(cudaMemcpy(c.data(), iv->centroids.p, c.size() * 4, cudaMemcpyDeviceToHost));
-        w.put_bytes(c.data(), c.size() * 4);
-        if (iv->is_pq) {
-            std::vector<float> pc((size_t)iv->M * 256 * iv->dsub);
-            KB2_CUDA_CHECK(cudaMemcpy(pc.data(), iv->pqc.p, pc.size() * 4, cudaMemcpyDeviceToHost));
-            w.put_bytes(pc.data(), pc.size() * 4);
-        }
-        const size_t cs = iv->is_pq ? (size_t)iv->M : (size_t)ix.dim * 4;
-        for (int64_t l = 0; l < iv->nlist; l++) {
-            const int64_t len = iv->h_list_len[l];
-            w.put<int64_t>(len);
-            if (!len) continue;
-            std::vector<int64_t> ids(len);
-            std::vector<uint8_t> cd((size_t)len * cs);
-            iv->export_list(l, ids.data(), cd.data());
-            w.put_bytes(ids.data(), len * 8);
-            w.put_bytes(cd.data(), cd.size());
-            if (iv->is_pq && iv->refine) {
-                std::vector<float> rv((size_t)len * ix.dim);
-                KB2_CUDA_CHECK(cudaMemcpy(rv.data(), v32 + iv->h_list_off[l] * ix.dim, rv.size() * 4, cudaMemcpyDeviceToHost));
-                w.put_bytes(rv.data(), rv.size() * 4);
-            }
-        }
-    } else if (auto* cg = dynamic_cast<CagraIndex*>(&ix)) {
-        cg->serialize(w);
-    } else if (auto* hn = dynamic_cast<HnswIndex*>(&ix)) {
-        hn->serialize(w);
-    } else {
-        throw Error(KB2_NOT_IMPLEMENTED, "serialize: unknown index class");
-    }
+    ix.save(w);
     // optional trailing section of an emb-list index: "ELST", the MAX_SIM metric, n_docs, offsets[n_docs + 1]
     if (ix.emb_list) {
         w.put<uint32_t>(kEmbListTag);
@@ -303,90 +264,15 @@ deserialize_index(const uint8_t* blob, size_t size, int device) {
     KB2_REQUIRE(r.get<uint32_t>() == 0x4932424b, KB2_INVALID_BINARY_SET, "bad magic");
     KB2_REQUIRE(r.get<uint32_t>() == 1, KB2_INVALID_BINARY_SET, "unsupported version");
     const std::string type = r.get_str();
-    const int metric_raw = r.get<int32_t>();
-    const bool cosine = metric_raw == KB2_METRIC_COSINE;
-    const int metric = cosine ? KB2_METRIC_IP : metric_raw;
+    const int metric = r.get<int32_t>();
     const int dim = r.get<int32_t>();
     KB2_REQUIRE(dim > 0 && dim <= (1 << 20), KB2_INVALID_BINARY_SET, "bad dim in blob");
-    KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP, KB2_INVALID_BINARY_SET, "bad metric in blob");
-    std::unique_ptr<IndexBase> ix;
-    if (type == "FLAT") {
-        auto* fi = new FlatIndex();
-        ix.reset(fi);
-        fi->type = type; fi->metric = metric; fi->dim = dim; fi->device = device;
-        fi->init_common();
-        const int64_t n = r.get<int64_t>();
-        KB2_REQUIRE(n >= 0 && (uint64_t)n <= size / ((size_t)dim * 4), KB2_INVALID_BINARY_SET, "bad row count in blob");
-        const int custom = r.get<int32_t>();
-        const float* data = (const float*)r.get_bytes((size_t)n * dim * 4);
-        const int64_t* labels = custom ? (const int64_t*)r.get_bytes((size_t)n * 8) : nullptr;
-        // blob memory may be unaligned: stage through vectors
-        std::vector<float> hd((size_t)n * dim);
-        memcpy(hd.data(), data, hd.size() * 4);
-        std::vector<int64_t> hl;
-        if (custom) { hl.resize(n); memcpy(hl.data(), labels, n * 8); }
-        fi->add(hd.data(), n, custom ? hl.data() : nullptr);
-    } else if (type == "IVF_FLAT" || type == "IVF_PQ") {
-        auto* iv = new IvfIndex();
-        ix.reset(iv);
-        iv->type = type; iv->metric = metric; iv->dim = dim; iv->device = device;
-        iv->is_pq = (type == "IVF_PQ");
-        iv->init_common();
-        const int64_t nlist = r.get<int64_t>();
-        iv->M = r.get<int32_t>();
-        iv->nbits = r.get<int32_t>();
-        {
-            const int rf = r.get<int32_t>();
-            KB2_REQUIRE(rf >= 0 && rf <= 3, KB2_INVALID_BINARY_SET, "bad refine field in blob");
-            iv->refine = rf != 0;
-            iv->refine_kind = rf ? rf - 1 : 0;
-        }
-        KB2_REQUIRE(nlist >= 1 && (uint64_t)nlist <= size / ((size_t)dim * 4), KB2_INVALID_BINARY_SET, "bad nlist in blob");
-        if (iv->is_pq)
-            KB2_REQUIRE(iv->M > 0 && dim % iv->M == 0 && iv->nbits == 8, KB2_INVALID_BINARY_SET, "bad m / nbits in blob");
-        std::vector<float> c((size_t)nlist * dim);
-        memcpy(c.data(), r.get_bytes(c.size() * 4), c.size() * 4);
-        std::vector<float> pc;
-        if (iv->is_pq) {
-            pc.resize((size_t)iv->M * 256 * (dim / iv->M));
-            memcpy(pc.data(), r.get_bytes(pc.size() * 4), pc.size() * 4);
-        }
-        iv->import_begin(nlist, c.data(), iv->is_pq ? pc.data() : nullptr);
-        const size_t cs = iv->is_pq ? (size_t)iv->M : (size_t)dim * 4;
-        std::vector<float> raw_rows;  // import order
-        for (int64_t l = 0; l < nlist; l++) {
-            const int64_t len = r.get<int64_t>();
-            KB2_REQUIRE(len >= 0 && (uint64_t)len <= size / 8, KB2_INVALID_BINARY_SET, "bad list length in blob");
-            if (!len) continue;
-            std::vector<int64_t> ids(len);
-            memcpy(ids.data(), r.get_bytes(len * 8), len * 8);
-            const uint8_t* cd = r.get_bytes((size_t)len * cs);
-            iv->import_list(l, len, ids.data(), cd);
-            if (iv->is_pq && iv->refine) {
-                const uint8_t* rv = r.get_bytes((size_t)len * dim * 4);
-                const size_t o = raw_rows.size();
-                raw_rows.resize(o + (size_t)len * dim);
-                memcpy(raw_rows.data() + o, rv, (size_t)len * dim * 4);
-            }
-        }
-        const bool with_raw = iv->is_pq && iv->refine;
-        iv->import_finish(with_raw ? raw_rows.data() : nullptr, with_raw ? (int64_t)(raw_rows.size() / dim) : 0, true);
-    } else if (type == "GPU_CAGRA" || type == "GPU_CUVS_CAGRA") {
-        auto* cg = new CagraIndex();
-        ix.reset(cg);
-        cg->type = type; cg->metric = metric; cg->dim = dim; cg->device = device;
-        cg->init_common();
-        cg->deserialize(r);
-    } else if (type == "HNSW") {
-        auto* hn = new HnswIndex();
-        ix.reset(hn);
-        hn->type = type; hn->metric = metric; hn->dim = dim; hn->device = device;
-        hn->init_common();
-        hn->deserialize(r);
-    } else {
-        throw Error(KB2_INVALID_BINARY_SET, "unknown index type in blob");
-    }
-    ix->cosine = cosine;   // stored vectors are already normalised; queries will be
+    KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP || metric == KB2_METRIC_COSINE, KB2_INVALID_BINARY_SET,
+                "bad metric in blob");
+    std::unique_ptr<IndexBase> ix = make_index(type);
+    KB2_REQUIRE(ix, KB2_INVALID_BINARY_SET, "unknown index type in blob");
+    ix->init(type, metric, dim, device);   // COSINE: the stored vectors are already normalised; queries will be
+    ix->load(r);
     if (r.o < r.n) {
         KB2_REQUIRE(r.get<uint32_t>() == kEmbListTag, KB2_INVALID_BINARY_SET, "unknown section after the index in blob");
         const int el_metric = r.get<int32_t>();
