@@ -82,8 +82,10 @@ int kb2_device_count(void);
  * "GPU_CAGRA" | "GPU_CUVS_CAGRA" (DESIGN §4.12): a fixed-degree graph built on the device at kb2_index_add (train is a
  *             no-op) and searched by a batched itopk kernel.  Metrics L2, IP, COSINE.  Build keys
  *             intermediate_graph_degree (1..1007, default 128) and graph_degree (1..256, <= the former, default 64),
- *             else KB2_OUT_OF_RANGE_IN_JSON.  The intermediate graph is always the exact k-NN graph: build_algo,
- *             nn_descent_niter, cache_dataset_on_device and adapt_for_cpu are accepted and have no effect.  Search keys
+ *             else KB2_OUT_OF_RANGE_IN_JSON.  The intermediate graph is the exact k-NN graph, or with build_algo
+ *             "NN_DESCENT" (any case) the NN-descent graph, nn_descent_niter (1..1000, default 20, else
+ *             KB2_OUT_OF_RANGE_IN_JSON) its iteration cap; any other build_algo builds the exact graph.
+ *             cache_dataset_on_device and adapt_for_cpu are accepted and have no effect.  Search keys
  *             itopk_size (default max(k, 64), rounded up to a multiple of 32, <= 1024), search_width (default
  *             max(ceil(k / 32), 1)), max_iterations (0: until no pool entry is unexpanded), num_random_samplings
  *             (default 1); max(itopk_size, 32 * search_width) >= k and search_width * graph_degree <= 4096, else
@@ -317,6 +319,17 @@ int kb2_index_last_stage_info(kb2_index_t h, float* out4);
  * path to the fp32 one (the reference computes these distances with src/simd fvec_L2sqr_ny). */
 int kb2_debug_gemm_keys(const float* q, int64_t nq, const float* x, int64_t nb, int dim, int metric, int use_tc,
                         float* out_keys, int device);
+
+/* validation hook: step 1 of the GPU_CAGRA build alone (DESIGN §4.12) over the n rows x (device, n x dim fp32), with
+ * the build keys of json (intermediate_graph_degree, build_algo, nn_descent_niter; errors as kb2_index_create).  metric:
+ * KB2_METRIC_L2 or KB2_METRIC_IP.  m = min(intermediate_graph_degree, n - 1); out_ids (device, n x m int32) receives
+ * G0, best first, and out_keys (device, n x m) their keys (squared L2, or minus the inner product).  *out_iters: the
+ * NN-descent iterations run (0 for the exact graph); out_updates (host, up to updates_cap entries): updates(t) of each;
+ * *out_ms: device ms of the step.  out_iters, out_updates and out_ms may be NULL.  Used by tests to hold the device
+ * graph to the numpy model and to measure its recall. */
+int kb2_debug_cagra_knn_graph(const float* x, int64_t n, int dim, int metric, const char* json, int32_t* out_ids,
+                              float* out_keys, int* out_iters, int64_t* out_updates, int updates_cap, float* out_ms,
+                              int device);
 
 /* validation hook: exact MaxSim scores of (query list, document) pairs, pair_lims [n_lists + 1] (host) giving each
  * list's run of pair_docs (distinct documents, ascending), computed by the emb-list index re-rank kernel

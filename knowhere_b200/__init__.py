@@ -91,6 +91,7 @@ def _declare(L):
     L.kb2_index_search_emb_list.argtypes = [vp, vp, vp, i64, i32, c.c_char_p, vp, i64, vp, vp, vp]
     L.kb2_index_emb_list_stage_ms.argtypes = [vp, vp]
     L.kb2_debug_maxsim_pairs.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, i32, vp, vp, i32]
+    L.kb2_debug_cagra_knn_graph.argtypes = [vp, i64, i32, i32, c.c_char_p, vp, vp, vp, vp, i32, vp, i32]
     if hasattr(L, "kb2_faiss_describe"):
         L.kb2_faiss_describe.argtypes = [vp, c.c_size_t, i32, vp, c.c_size_t]
         L.kb2_faiss_rewrite.argtypes = [vp, c.c_size_t, i32, c.POINTER(vp), c.POINTER(c.c_size_t)]
@@ -540,6 +541,24 @@ def debug_maxsim_pairs(queries, query_lims, base, base_lims, pair_lims, pair_doc
                                     base.shape[1], _METRICS[metric], _ptr(pl), _ptr(pair_docs), 1 if use_rerank else 0,
                                     _ptr(out), ctypes.byref(ms), device))
     return out[:int(pl[-1])], ms.value
+
+
+def debug_cagra_knn_graph(x, metric="L2", config=None, device=0):
+    """validation hook (kb2_debug_cagra_knn_graph): step 1 of the GPU_CAGRA build alone, exact or NN-descent as the build
+    keys in config say.  x: CUDA tensor [n, d] fp32.  Returns (G0 int32 CUDA tensor [n, m], keys fp32 CUDA tensor [n, m],
+    NN-descent iterations run, updates(t) numpy int64, device ms), m = min(intermediate_graph_degree, n - 1)."""
+    import torch
+    L = lib()
+    n, d = x.shape
+    m = min(int((config or {}).get("intermediate_graph_degree", 128)), n - 1)
+    ids = torch.empty((n, m), dtype=torch.int32, device=x.device)
+    keys = torch.empty((n, m), dtype=torch.float32, device=x.device)
+    iters = ctypes.c_int()
+    upd = np.zeros(1000, np.int64)
+    ms = ctypes.c_float()
+    _check(L.kb2_debug_cagra_knn_graph(_ptr(x), n, d, _METRICS[metric], _cfg(config), _ptr(ids), _ptr(keys),
+                                       ctypes.byref(iters), _ptr(upd), len(upd), ctypes.byref(ms), device))
+    return ids, keys, iters.value, upd[:iters.value].copy(), ms.value
 
 
 def brute_force_range_search(base, queries, radius, range_filter=None, metric="L2", bitset=None, device=0):

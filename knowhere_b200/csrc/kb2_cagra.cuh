@@ -5,7 +5,8 @@
 //
 // Build, m = min(intermediate_graph_degree, n - 1), g = min(graph_degree, m):
 //   1. G0[i]: the m rows nearest to row i, best first, ties by ascending id (dense_knn over row chunks, k = m + 1, then
-//      row i removed where it appears, else the last entry dropped).  Always exact: no NN-descent / IVF-PQ graph.
+//      row i removed where it appears, else the last entry dropped); or, with build_algo NN_DESCENT, the NN-descent
+//      graph defined at cagra_nnd_join_kernel.
 //   2. detour(i, b) = #{a < b : G0[i][b] in G0[G0[i][a]][0:b]}                          (cagra_prune_kernel)
 //   3. P[i]: the g entries of G0[i] with the smallest (detour, b), in that order         (cagra_prune_kernel)
 //   4. R[v]: the sources i of the edges i -> v = P[i][p], ordered by (p, i)              (one cub radix sort)
@@ -23,6 +24,7 @@
 //   * the result: the first k entries of T the bitset does not filter out (filtered rows route but are not returned).
 #pragma once
 #include <cub/cub.cuh>
+#include <numeric>
 
 #include "kb2_hnsw.cuh"
 
@@ -47,9 +49,11 @@ cagra_seed(uint64_t j) {
 }
 
 // ============================================================================================ build
-// G0 row i <- the m + 1 nearest ids of row i without i (or without the last one when i is not among them)
+// G0 row i <- the m + 1 nearest ids of row i without i (or without the last one when i is not among them); with g0_key,
+// their keys too (dist: the dense_knn distances, negated for IP)
 __global__ void __launch_bounds__(256)
-cagra_drop_self_kernel(const int64_t* __restrict__ knn, int64_t rows, int64_t row0, int m, int32_t* __restrict__ g0) {
+cagra_drop_self_kernel(const int64_t* __restrict__ knn, const float* __restrict__ dist, int ip, int64_t rows, int64_t row0,
+                       int m, int32_t* __restrict__ g0, float* __restrict__ g0_key) {
     const int64_t r = (int64_t)blockIdx.x * (blockDim.x / kWarp) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (r >= rows) return;
@@ -63,7 +67,11 @@ cagra_drop_self_kernel(const int64_t* __restrict__ knn, int64_t rows, int64_t ro
         const unsigned bal = __ballot_sync(0xffffffffu, hit);
         if (bal) { pos = b + __ffs(bal) - 1; break; }
     }
-    for (int c = lane; c < m; c += kWarp) out[c] = (int32_t)in[c < pos ? c : c + 1];
+    for (int c = lane; c < m; c += kWarp) {
+        const int s = c < pos ? c : c + 1;
+        out[c] = (int32_t)in[s];
+        if (g0_key) g0_key[self * m + c] = ip ? -dist[r * (m + 1) + s] : dist[r * (m + 1) + s];
+    }
 }
 
 // Steps 2-3, one CTA per row i: detour counts through an id -> rank table of G0[i] in shared memory (each warp reads
@@ -169,6 +177,496 @@ cagra_merge_kernel(const int32_t* __restrict__ pruned, const int32_t* __restrict
     append(rsrc + rstart[i], rstart[i + 1] - rstart[i]);
     append(pruned + i * g + half, g - half);
     for (int c = lane; c < g; c += kWarp) graph[i * g + c] = out[c];
+}
+
+// ============================================================================================ NN-descent (step 1)
+// With build_algo NN_DESCENT, G0 is the NN-descent graph (DESIGN §4.12; tests/cagra_nnd_model.py restates it).
+// m = min(igd, n - 1), S = min(32, m).  Row i keeps L[i]: m entries (key, id, new), best first by (key, id), distinct ids,
+// never i.
+//   init:  L[i][j] = (i + 1 + (o_i + j * stride) mod (n - 1)) mod n, o_i = cagra_seed(i) mod (n - 1), stride the first
+//          integer >= max(1, floor(0.618 (n - 1))) coprime to n - 1; every entry new.
+//   iteration t < niter:
+//     forward  new_f(i) / old_f(i): the first <= S entries of L[i] flagged new / old; the sampled new entries become old;
+//     reverse  new_r(i) / old_r(i): the <= S sources j with i in new_f(j) / old_f(j) of smallest (nnd_hash(j, i, t), j);
+//     join     C_new = new_f u new_r, C_old = old_f u old_r; every pair {u, v}, u != v, u in C_new, v in C_new u C_old,
+//              proposes (key(u, v), v) to u and (key(u, v), u) to v;
+//     update   L[u] <- the best m of L[u] u proposals(u) by (key, id), one entry per id; entries that enter are new;
+//     stop     when updates(t) = #new entries <= 1e-4 n m.
+//   G0[i]: the ids of L[i].
+// Every key comes from nnd_gram (3xTF32 mma.sync with the lower id in the A role), so a pair has the same key bits in
+// every kernel that computes it; the update is then the top m of a totally ordered set, and a proposal is only dropped
+// unlocked when it is worse than the live m-th key of its target (which only improves): the graph does not depend on
+// the order in which the joins run.
+__device__ __forceinline__ bool cagra_less(float ka, uint32_t ia, float kb, uint32_t ib);
+__device__ __forceinline__ int cagra_rank(const float* key, const uint32_t* id, int len, float k, uint32_t i);
+
+constexpr int kNndS = 32;
+constexpr int kNndMaxC = 4 * kNndS;          // candidates of one join: |C_new|, |C_old| <= 2S
+constexpr int kNndThreads = 256;
+constexpr int kNndWarps = kNndThreads / kWarp;
+constexpr int kNndKc = 32;                   // dims staged per Gram step
+constexpr int kNndXld = kNndKc + 4;          // staged row stride (fragment loads hit 32 distinct banks)
+constexpr int kNndKld = kNndMaxC + 4;        // key tile row stride
+constexpr uint32_t kNndNew = 0x80000000u;    // "new" flag of a list entry's id (cagra_less ignores it)
+constexpr uint32_t kNndIdMask = 0x7fffffffu;
+constexpr double kNndDelta = 1e-4;           // termination threshold (updates <= delta n m), cuVS's default
+
+// priority of source j among the reverse samples of target i at iteration t (smaller first; ties by j)
+__host__ __device__ __forceinline__ uint32_t
+nnd_hash(uint32_t src, uint32_t tgt, int t) {
+    return (uint32_t)(cagra_seed(cagra_seed((uint64_t)t) ^ (((uint64_t)src << 32) | tgt)) >> 32);
+}
+
+__device__ __forceinline__ void
+nnd_split(float x, uint32_t& hi, uint32_t& lo) {
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(__fsub_rn(x, __uint_as_float(hi))));
+}
+__device__ __forceinline__ void
+nnd_mma(float* c, const uint32_t* a, const uint32_t* b) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+// key of a pair from the lower id's norm, the higher id's norm and their dot product; + 0 turns -0 into +0
+template <int METRIC>
+__device__ __forceinline__ float
+nnd_key(float n_lo, float n_hi, float dot) {
+    return __fadd_rn(METRIC == KB2_METRIC_L2 ? __fmaf_rn(-2.f, dot, __fadd_rn(n_lo, n_hi)) : -dot, 0.f);
+}
+// float -> uint32 with the same order
+__device__ __forceinline__ uint32_t
+nnd_ord(float k) {
+    const uint32_t u = __float_as_uint(k);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float
+nnd_unord(uint32_t u) {
+    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+
+// CTA-wide: the keys of the pairs r < c < C of the candidates s_id[0, C) (C <= kNndMaxC, ascending distinct ids) into
+// s_key[r][c] and s_key[c][r].  focus >= 0: only the tiles holding row or column `focus` are needed.  Rows are gathered
+// kNndKc dims at a time with cp.async (zero-filled past d and past C) and contracted in 16 x 8 tiles on the tensor cores,
+// hi.hi + hi.lo + lo.hi per k-step of 8, fp32 accumulation.  Tile (r, c) always has the lower id in the A role and runs
+// the same k-steps in the same order, so a pair's key has the same bits in every call.  Starts and ends at a barrier.
+template <int METRIC>
+__device__ __forceinline__ void
+nnd_gram(const float* __restrict__ x, int d, const uint32_t* s_id, const float* s_norm, int C, int focus, float* s_x,
+         float* s_key) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
+    const int cp = (C + 15) & ~15;
+    const int nct = cp >> 3, ntiles = (cp >> 4) * nct;
+    constexpr int kTiles = (kNndMaxC / 16) * (kNndMaxC / 8) / kNndWarps;   // tiles per warp at most
+    auto live = [&](int q) {
+        const int rt = q / nct, ct = q % nct;
+        if (q >= ntiles || 8 * ct + 7 <= 16 * rt) return false;   // every (r, c) of the tile has r >= c
+        return focus < 0 || (focus >> 4) == rt || (focus >> 3) == ct;
+    };
+    float acc[kTiles][4];
+#pragma unroll
+    for (int j = 0; j < kTiles; j++) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+    for (int k0 = 0; k0 < d; k0 += kNndKc) {
+        for (int e = tid; e < cp * kNndKc; e += kNndThreads) {
+            const int r = e / kNndKc, kk = e % kNndKc;
+            const bool ok = r < C && k0 + kk < d;
+            const float* src = ok ? x + (int64_t)s_id[r] * d + k0 + kk : x;
+            const uint32_t dst = (uint32_t)__cvta_generic_to_shared(s_x + r * kNndXld + kk);
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(ok ? 4 : 0) : "memory");
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        asm volatile("cp.async.wait_all;" ::: "memory");
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < kTiles; j++) {
+            const int q = warp + kNndWarps * j;
+            if (!live(q)) continue;
+            const float* A = s_x + ((q / nct) * 16 + g) * kNndXld + t4;
+            const float* B = s_x + ((q % nct) * 8 + g) * kNndXld + t4;
+#pragma unroll
+            for (int ks = 0; ks < kNndKc; ks += 8) {
+                uint32_t ah[4], al[4], bh[2], bl[2];
+                nnd_split(A[ks], ah[0], al[0]);
+                nnd_split(A[8 * kNndXld + ks], ah[1], al[1]);
+                nnd_split(A[ks + 4], ah[2], al[2]);
+                nnd_split(A[8 * kNndXld + ks + 4], ah[3], al[3]);
+                nnd_split(B[ks], bh[0], bl[0]);
+                nnd_split(B[ks + 4], bh[1], bl[1]);
+                nnd_mma(acc[j], ah, bh);
+                nnd_mma(acc[j], ah, bl);
+                nnd_mma(acc[j], al, bh);
+            }
+        }
+        __syncthreads();
+    }
+    // accumulator e of a tile: row g + 8 (e >> 1), column 2 t4 + (e & 1)
+#pragma unroll
+    for (int j = 0; j < kTiles; j++) {
+        const int q = warp + kNndWarps * j;
+        if (!live(q)) continue;
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const int r = (q / nct) * 16 + g + 8 * (e >> 1), c = (q % nct) * 8 + 2 * t4 + (e & 1);
+            if (r < c && c < C) {
+                const float k = nnd_key<METRIC>(s_norm[r], s_norm[c], acc[j][e]);
+                s_key[r * kNndKld + c] = k;
+                s_key[c * kNndKld + r] = k;
+            }
+        }
+    }
+    __syncthreads();
+}
+
+// CTA-wide: s_out[rank] = s_in[e] in ascending order (ties by position), s_perm[rank] = e if given.  Ends at a barrier.
+__device__ __forceinline__ void
+nnd_rank_sort(const uint32_t* s_in, int C, uint32_t* s_out, int16_t* s_perm) {
+    for (int e = threadIdx.x; e < C; e += kNndThreads) {
+        const uint32_t v = s_in[e];
+        int r = 0;
+        for (int f = 0; f < C; f++) {
+            const uint32_t w = s_in[f];
+            r += (w < v) || (w == v && f < e);
+        }
+        s_out[r] = v;
+        if (s_perm) s_perm[r] = (int16_t)e;
+    }
+    __syncthreads();
+}
+
+// shared memory of the init and join kernels: key tile | staged rows | candidate norms, ids (+ per-warp lists and batches)
+__host__ __device__ constexpr size_t
+nnd_smem_common() {
+    return (size_t)kNndMaxC * kNndKld * 4 + (size_t)kNndMaxC * kNndXld * 4 + (size_t)kNndMaxC * 4 * 4 + 256;
+}
+
+// L[i] <- the initial list of row i, best first: one CTA per row; the m ids are keyed in chunks of kNndMaxC - 1 together
+// with i (the Gram tiles holding i only), then sorted by (key, id).  Dynamic smem: nnd_smem_common() + 8 KB.
+template <int METRIC>
+__global__ void __launch_bounds__(kNndThreads)
+cagra_nnd_init_kernel(const float* __restrict__ x, const float* __restrict__ norms, int64_t n, int d, int m, int64_t stride,
+                      float* __restrict__ lkey, uint32_t* __restrict__ lid) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float* s_key = (float*)smem_raw;
+    float* s_x = s_key + kNndMaxC * kNndKld;
+    float* s_norm = s_x + kNndMaxC * kNndXld;
+    uint32_t* s_raw = (uint32_t*)(s_norm + kNndMaxC);
+    uint32_t* s_id = s_raw + kNndMaxC;
+    int16_t* s_perm = (int16_t*)(s_id + kNndMaxC);
+    int* s_focus = (int*)(s_perm + kNndMaxC);
+    float* s_lk = (float*)(smem_raw + nnd_smem_common());   // 1024 keys, then 1024 ids
+    uint32_t* s_li = (uint32_t*)(s_lk + 1024);
+    const int tid = threadIdx.x;
+    const int64_t i = blockIdx.x;
+    const uint64_t nm1 = (uint64_t)(n - 1);
+    const uint64_t o = cagra_seed((uint64_t)i) % nm1;
+    for (int j = tid; j < m; j += kNndThreads) s_li[j] = (uint32_t)(((uint64_t)i + 1 + (o + (uint64_t)j * (uint64_t)stride) % nm1) % (uint64_t)n);
+    __syncthreads();
+    for (int j0 = 0; j0 < m; j0 += kNndMaxC - 1) {
+        const int cnt = min(kNndMaxC - 1, m - j0);
+        for (int e = tid; e <= cnt; e += kNndThreads) s_raw[e] = e == 0 ? (uint32_t)i : s_li[j0 + e - 1];
+        __syncthreads();
+        nnd_rank_sort(s_raw, cnt + 1, s_id, s_perm);
+        for (int e = tid; e <= cnt; e += kNndThreads) {
+            s_norm[e] = METRIC == KB2_METRIC_L2 ? norms[s_id[e]] : 0.f;
+            if (s_perm[e] == 0) *s_focus = e;
+        }
+        __syncthreads();
+        const int f = *s_focus;
+        nnd_gram<METRIC>(x, d, s_id, s_norm, cnt + 1, f, s_x, s_key);
+        for (int e = tid; e <= cnt; e += kNndThreads)
+            if (e != f) s_lk[j0 + s_perm[e] - 1] = s_key[e * kNndKld + f];
+        __syncthreads();
+    }
+    // best first by (key, id): one block radix sort of (ordered key, id), its storage over the key tile
+    using Sort = cub::BlockRadixSort<uint64_t, kNndThreads, 4>;
+    static_assert(sizeof(typename Sort::TempStorage) <= (size_t)kNndMaxC * kNndKld * 4, "sort storage");
+    uint64_t k[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+        const int j = tid * 4 + u;
+        k[u] = j < m ? ((uint64_t)nnd_ord(s_lk[j]) << 32) | s_li[j] : ~0ull;
+    }
+    Sort(*reinterpret_cast<typename Sort::TempStorage*>(s_key)).Sort(k);
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+        const int j = tid * 4 + u;
+        if (j < m) {
+            lkey[i * m + j] = nnd_unord((uint32_t)(k[u] >> 32));
+            lid[i * m + j] = (uint32_t)k[u] | kNndNew;
+        }
+    }
+}
+
+// Forward samples of row i (one warp per row): fwd[i][0, S) the first <= S new entries (then flagged old), fwd[i][32,
+// 32 + S) the first <= S old ones, ~0 past the counts.  Each sample j -> v also writes its reverse-sort entry: key
+// v << 33 | old << 32 | nnd_hash(i, v, t), value i (~0 keys for the unused slots sort last).
+__global__ void __launch_bounds__(256)
+cagra_nnd_sample_kernel(uint32_t* __restrict__ lid, int64_t n, int m, int S, int t, uint32_t* __restrict__ fwd,
+                        uint64_t* __restrict__ rkey, uint32_t* __restrict__ rsrc) {
+    const int64_t i = (int64_t)blockIdx.x * (blockDim.x / kWarp) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;
+    uint32_t* L = lid + i * m;
+    uint32_t* F = fwd + i * 2 * kNndS;
+    uint64_t* K = rkey + i * 2 * kNndS;
+    const unsigned lt = (1u << lane) - 1;
+    int cn = 0, co = 0;
+    for (int b = 0; b < m && (cn < S || co < S); b += kWarp) {
+        const int q = b + lane;
+        const uint32_t v = q < m ? L[q] : 0u;
+        const bool isn = q < m && (v & kNndNew), iso = q < m && !(v & kNndNew);
+        const unsigned bn = __ballot_sync(0xffffffffu, isn), bo = __ballot_sync(0xffffffffu, iso);
+        const int pn = cn + __popc(bn & lt), po = co + __popc(bo & lt);
+        const uint32_t tgt = v & kNndIdMask;
+        if (isn && pn < S) {
+            F[pn] = tgt;
+            L[q] = tgt;
+            K[pn] = ((uint64_t)tgt << 33) | nnd_hash((uint32_t)i, tgt, t);
+        }
+        if (iso && po < S) {
+            F[kNndS + po] = tgt;
+            K[kNndS + po] = ((uint64_t)tgt << 33) | (1ull << 32) | nnd_hash((uint32_t)i, tgt, t);
+        }
+        cn = min(S, cn + __popc(bn));
+        co = min(S, co + __popc(bo));
+    }
+    for (int s = lane; s < 2 * kNndS; s += kWarp) {
+        if ((s < kNndS && s >= cn) || (s >= kNndS && s - kNndS >= co)) {
+            F[s] = ~0u;
+            K[s] = ~0ull;
+        }
+        rsrc[i * 2 * kNndS + s] = (uint32_t)i;
+    }
+}
+
+// rs[2 v + o] = the first sorted reverse entry of target v with old flag >= o (v = 0..n; rs[2 n] ends the real ones)
+__global__ void
+cagra_nnd_offsets_kernel(const uint64_t* __restrict__ key, int64_t ne, int64_t n, int64_t* __restrict__ rs) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t > 2 * n) return;
+    const uint64_t probe = ((uint64_t)(t >> 1) << 33) | ((uint64_t)(t & 1) << 32);
+    int64_t lo = 0, hi = ne;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (key[mid] < probe) lo = mid + 1; else hi = mid;
+    }
+    rs[t] = lo;
+}
+
+// bounded spin (~3 s of SM clocks): a protocol bug must end the launch with an error, never hang the GPU
+__device__ __forceinline__ void
+nnd_lock(int* l) {
+    if (atomicCAS(l, 0, 1) != 0) {
+        const long long t0 = clock64();
+        while (atomicCAS(l, 0, 1) != 0) {
+            __nanosleep(64);
+            if (clock64() - t0 > 6000000000ll) __trap();
+        }
+    }
+    __threadfence();
+}
+
+struct NndJoinParams {
+    const float* x;
+    const float* norms;
+    int64_t n;
+    int d, m, S;
+    const uint32_t* fwd;     // n x 2 kNndS forward samples
+    const uint32_t* rsrc;    // sorted reverse sources
+    const int64_t* rs;       // 2 n + 1 offsets into rsrc
+    float* lkey;             // n x m lists
+    uint32_t* lid;
+    int* lock;               // n row locks
+};
+
+// per-warp shared memory of the join: the target's list (m keys, m ids), a batch (kNndMaxC keys, ids, ranks)
+__host__ __device__ constexpr size_t
+nnd_join_warp_smem(int m) {
+    return ((size_t)m * 8 + (size_t)kNndMaxC * 12 + 15) & ~(size_t)15;
+}
+
+// One join per CTA (row i): the candidates (C_new before C_old, sorted by id, deduplicated keeping the new copy), their
+// key tile (nnd_gram), then one warp per candidate u: the proposals to u that pass the live m-th key of L[u], sorted by
+// (key, id), merged into L[u] under the row lock (one lane takes it; a warp holds one lock at a time and waits on none
+// while it holds it).
+template <int METRIC>
+__global__ void __launch_bounds__(kNndThreads, 2)
+cagra_nnd_join_kernel(NndJoinParams p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float* s_key = (float*)smem_raw;
+    float* s_x = s_key + kNndMaxC * kNndKld;
+    float* s_norm = s_x + kNndMaxC * kNndXld;
+    uint32_t* s_raw = (uint32_t*)(s_norm + kNndMaxC);
+    uint32_t* s_sorted = s_raw + kNndMaxC;
+    uint32_t* s_id = s_sorted + kNndMaxC;
+    int* s_ctl = (int*)(s_id + kNndMaxC);
+    uint8_t* s_new = (uint8_t*)(s_ctl + 4);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const unsigned lt = (1u << lane) - 1;
+    const int m = p.m;
+    unsigned char* wbase = smem_raw + nnd_smem_common() + (size_t)warp * nnd_join_warp_smem(m);
+    float* wl_key = (float*)wbase;
+    uint32_t* wl_id = (uint32_t*)(wl_key + m);
+    float* wb_key = (float*)(wl_id + m);
+    uint32_t* wb_id = (uint32_t*)(wb_key + kNndMaxC);
+    int* wr = (int*)(wb_id + kNndMaxC);
+    const int64_t i = blockIdx.x;
+
+    // candidates: slots [0, 32) new_f, [32, 64) new_r, [64, 96) old_f, [96, 128) old_r as id << 1 | old (~0: none)
+    if (tid < kNndMaxC) {
+        const int part = tid >> 5, s = tid & 31;
+        uint32_t v = ~0u;
+        if (s < p.S) {
+            if (part == 0 || part == 2) {
+                const uint32_t f = p.fwd[i * 2 * kNndS + (part >> 1) * kNndS + s];
+                if (f != ~0u) v = (f << 1) | (uint32_t)(part >> 1);
+            } else {
+                const int64_t a = p.rs[2 * i + (part >> 1)], b = p.rs[2 * i + (part >> 1) + 1];
+                if (a + s < b) v = (p.rsrc[a + s] << 1) | (uint32_t)(part >> 1);
+            }
+        }
+        s_raw[tid] = v;
+    }
+    __syncthreads();
+    nnd_rank_sort(s_raw, kNndMaxC, s_sorted, nullptr);
+    if (warp == 0) {
+        int C = 0;
+        for (int b = 0; b < kNndMaxC; b += kWarp) {
+            const uint32_t v = s_sorted[b + lane];
+            const bool ok = v != ~0u && (b + lane == 0 || (s_sorted[b + lane - 1] >> 1) != (v >> 1));
+            const unsigned bal = __ballot_sync(0xffffffffu, ok);
+            if (ok) {
+                const int pos = C + __popc(bal & lt);
+                s_id[pos] = v >> 1;
+                s_new[pos] = (uint8_t)!(v & 1u);
+            }
+            C += __popc(bal);
+        }
+        if (lane == 0) s_ctl[0] = C;
+    }
+    __syncthreads();
+    const int C = s_ctl[0];
+    if (C < 2) return;
+    for (int e = tid; e < C; e += kNndThreads) s_norm[e] = METRIC == KB2_METRIC_L2 ? p.norms[s_id[e]] : 0.f;
+    __syncthreads();
+    nnd_gram<METRIC>(p.x, p.d, s_id, s_norm, C, -1, s_x, s_key);
+
+    for (int r = warp; r < C; r += kNndWarps) {
+        const uint32_t u = s_id[r];
+        const bool rnew = s_new[r] != 0;
+        float* Lk = p.lkey + (int64_t)u * m;
+        uint32_t* Li = p.lid + (int64_t)u * m;
+        const float thr = __ldcg(Lk + m - 1);   // the live m-th key: it only improves, so worse proposals cannot enter
+        int B = 0;
+        for (int c0 = 0; c0 < C; c0 += kWarp) {
+            const int c = c0 + lane;
+            float k = 0.f;
+            bool ok = c < C && c != r && (rnew || s_new[c]);
+            if (ok) {
+                k = s_key[r * kNndKld + c];
+                ok = k <= thr;
+            }
+            const unsigned bal = __ballot_sync(0xffffffffu, ok);
+            if (ok) {
+                const int pos = B + __popc(bal & lt);
+                wb_key[pos] = k;
+                wb_id[pos] = s_id[c];
+            }
+            B += __popc(bal);
+        }
+        if (B == 0) continue;
+        // bitonic sort of the batch by (key, id), padded to a power of two >= 32
+        int len = kWarp;
+        while (len < B) len <<= 1;
+        for (int q = B + lane; q < len; q += kWarp) { wb_key[q] = INFINITY; wb_id[q] = kNndIdMask; }
+        __syncwarp();
+        for (int size = 2; size <= len; size <<= 1) {
+            for (int stride = size >> 1; stride > 0; stride >>= 1) {
+                for (int t = lane; t < (len >> 1); t += kWarp) {
+                    const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+                    const bool up = (lo & size) == 0;
+                    const float ka = wb_key[lo], kb = wb_key[hi];
+                    const uint32_t ia = wb_id[lo], ib = wb_id[hi];
+                    if (cagra_less(kb, ib, ka, ia) == up) {
+                        wb_key[lo] = kb; wb_id[lo] = ib;
+                        wb_key[hi] = ka; wb_id[hi] = ia;
+                    }
+                }
+                __syncwarp();
+            }
+        }
+        if (lane == 0) nnd_lock(p.lock + u);
+        __syncwarp();
+        for (int q = lane; q < m; q += kWarp) {
+            wl_key[q] = __ldcg(Lk + q);
+            wl_id[q] = __ldcg(Li + q);
+        }
+        __syncwarp();
+        // rank of each proposal in L[u]; drop those already present (same id means same key bits) or ranked past m
+        int nb = 0;
+        for (int b0 = 0; b0 < B; b0 += kWarp) {
+            const int b = b0 + lane;
+            float k = 0.f;
+            uint32_t v = 0;
+            int rk = m;
+            bool keep = false;
+            if (b < B) {
+                k = wb_key[b];
+                v = wb_id[b];
+                rk = cagra_rank(wl_key, wl_id, m, k, v);
+                keep = rk < m && !(wl_key[rk] == k && (wl_id[rk] & kNndIdMask) == v);
+            }
+            __syncwarp();
+            const unsigned bal = __ballot_sync(0xffffffffu, keep);
+            if (keep) {
+                const int pos = nb + __popc(bal & lt);
+                wb_key[pos] = k;
+                wb_id[pos] = v;
+                wr[pos] = rk;
+            }
+            nb += __popc(bal);
+            __syncwarp();
+        }
+        if (nb > 0) {
+            // merge: list entry q moves to q + #{proposals ranked <= q}; proposal b lands at wr[b] + b; past m drops out
+            for (int q = wr[0] + lane; q < m; q += kWarp) {
+                int lo = 0, hi = nb;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (wr[mid] <= q) lo = mid + 1; else hi = mid;
+                }
+                if (q + lo < m) {
+                    __stcg(Lk + q + lo, wl_key[q]);
+                    __stcg(Li + q + lo, wl_id[q]);
+                }
+            }
+            for (int b = lane; b < nb; b += kWarp) {
+                if (wr[b] + b < m) {
+                    __stcg(Lk + wr[b] + b, wb_key[b]);
+                    __stcg(Li + wr[b] + b, wb_id[b] | kNndNew);
+                }
+            }
+        }
+        __threadfence();
+        __syncwarp();
+        if (lane == 0) atomicExch(p.lock + u, 0);
+    }
+}
+
+// updates(t): the entries flagged new
+__global__ void
+cagra_nnd_count_kernel(const uint32_t* __restrict__ lid, int64_t total, unsigned long long* __restrict__ out) {
+    unsigned c = 0;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x)
+        c += lid[e] >> 31;
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
+}
+
+__global__ void
+cagra_nnd_ids_kernel(const uint32_t* __restrict__ lid, int64_t total, int32_t* __restrict__ g0) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < total) g0[e] = (int32_t)(lid[e] & kNndIdMask);
 }
 
 // ============================================================================================ search
@@ -370,6 +868,9 @@ cagra_search_kernel(CagraSearchParams c) {
 // ============================================================================================ host
 struct CagraIndex : HnswIndex {
     int igd = 128, gd = 64;   // build keys (gpu_cuvs_cagra_config.h); the graph's degree is min(gd, igd, n - 1)
+    bool nn_descent = false;  // build_algo NN_DESCENT: step 1 is the NN-descent graph, else the exact k-NN graph
+    int nnd_niter = 20;       // nn_descent_niter: NN-descent's iteration cap
+    std::vector<int64_t> nnd_updates;   // updates(t) of each NN-descent iteration of the last build
     float build_ms[3] = {0.f, 0.f, 0.f};   // k-NN graph, pruning, merge (CUDA events)
 
     int degree() const { return h_cum.size() >= 2 ? h_cum[1] : 0; }
@@ -415,22 +916,12 @@ struct CagraIndex : HnswIndex {
     build_graph(int m, int g) {
         cudaStream_t st = stream;
         DevBuf<int32_t> g0, pruned, src, src_sorted, graph;
-        DevBuf<int64_t> knn_ids, rstart;
-        DevBuf<float> knn_dist;
+        DevBuf<int64_t> rstart;
         DevBuf<uint64_t> key, key_sorted;
         DevBuf<uint8_t> tmp;
-        // 1. exact k-NN graph: a bounded batch of rows at a time (dense_knn's scratch grows with the batch)
-        const int64_t chunk = std::min<int64_t>(n, 4096);
+        // 1. the intermediate graph
         g0.alloc_exact((size_t)n * m);
-        knn_ids.alloc_exact((size_t)chunk * (m + 1));
-        knn_dist.alloc_exact((size_t)chunk * (m + 1));
-        for (int64_t r0 = 0; r0 < n; r0 += chunk) {
-            const int64_t rows = std::min(chunk, n - r0);
-            dense_knn(*this, d_vecs.p + r0 * dim, rows, d_vecs.p, d_norms.p, n, dim, metric, m + 1, m + 17, nullptr, 0, nullptr,
-                      knn_ids.p, knn_dist.p, true);
-            cagra_drop_self_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(knn_ids.p, rows, r0, m, g0.p);
-            KB2_CUDA_CHECK(cudaGetLastError());
-        }
+        knn_graph(m, g0.p, nullptr);
         KB2_CUDA_CHECK(cudaEventRecord(ev1, st));
         // 2-3. detour counts and the pruned rows
         pruned.alloc_exact((size_t)n * g);
@@ -465,6 +956,102 @@ struct CagraIndex : HnswIndex {
         KB2_CUDA_CHECK(cudaEventElapsedTime(&build_ms[1], ev1, ev2));
         KB2_CUDA_CHECK(cudaEventElapsedTime(&build_ms[2], ev2, ev3));
         last.launches = 0;
+    }
+
+    // Step 1 over the n rows of d_vecs: G0 (n x m int32, best first) and, if g0_key is given, its keys.  The exact k-NN
+    // graph, or with build_algo NN_DESCENT the NN-descent graph (nnd_updates: updates(t) of each iteration run).
+    void
+    knn_graph(int m, int32_t* g0, float* g0_key) {
+        nnd_updates.clear();
+        if (nn_descent) {
+            nnd_graph(m, g0, g0_key);
+            return;
+        }
+        cudaStream_t st = stream;
+        // a bounded batch of rows at a time (dense_knn's scratch grows with the batch)
+        const int64_t chunk = std::min<int64_t>(n, 4096);
+        DevBuf<int64_t> knn_ids;
+        DevBuf<float> knn_dist;
+        knn_ids.alloc_exact((size_t)chunk * (m + 1));
+        knn_dist.alloc_exact((size_t)chunk * (m + 1));
+        for (int64_t r0 = 0; r0 < n; r0 += chunk) {
+            const int64_t rows = std::min(chunk, n - r0);
+            dense_knn(*this, d_vecs.p + r0 * dim, rows, d_vecs.p, d_norms.p, n, dim, metric, m + 1, m + 17, nullptr, 0, nullptr,
+                      knn_ids.p, knn_dist.p, true);
+            cagra_drop_self_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(knn_ids.p, knn_dist.p, metric == KB2_METRIC_IP,
+                                                                                rows, r0, m, g0, g0_key);
+            KB2_CUDA_CHECK(cudaGetLastError());
+        }
+    }
+
+    // NN-descent (definition at cagra_nnd_join_kernel).  Memory: the lists (8 B per entry), the forward samples and the
+    // reverse-sample sort (2 x 64 entries of 12 B per row, double-buffered): O(n m).
+    void
+    nnd_graph(int m, int32_t* g0, float* g0_key) {
+        cudaStream_t st = stream;
+        const int S = std::min(kNndS, m);
+        const int64_t nm = n * m, ne = n * 2 * kNndS;
+        KB2_REQUIRE(ne < (1ll << 31), KB2_INVALID_ARGS,
+                    "GPU_CAGRA NN_DESCENT: at most " + std::to_string((1ll << 31) / (2 * kNndS) - 1) + " rows");
+        DevBuf<float> lkey;
+        DevBuf<uint32_t> lid, fwd, rsrc[2];
+        DevBuf<uint64_t> rkey[2];
+        DevBuf<int64_t> rs;
+        DevBuf<int> lock;
+        DevBuf<uint8_t> tmp;
+        DevBuf<unsigned long long> cnt;
+        lkey.alloc_exact((size_t)nm);
+        lid.alloc_exact((size_t)nm);
+        fwd.alloc_exact((size_t)ne);
+        for (int b = 0; b < 2; b++) {
+            rkey[b].alloc_exact((size_t)ne);
+            rsrc[b].alloc_exact((size_t)ne);
+        }
+        rs.alloc_exact((size_t)(2 * n + 1));
+        lock.alloc_exact((size_t)n);
+        cnt.alloc_exact(1);
+        KB2_CUDA_CHECK(cudaMemsetAsync(lock.p, 0, (size_t)n * 4, st));
+        int64_t stride = std::max<int64_t>(1, (n - 1) * 618 / 1000);
+        while (std::gcd(stride, n - 1) != 1) stride++;
+        const size_t smem_init = nnd_smem_common() + 8192;
+        const size_t smem_join = nnd_smem_common() + (size_t)kNndWarps * nnd_join_warp_smem(m);
+        with_metric(metric, [&](auto mt) {
+            launch<cagra_nnd_init_kernel<decltype(mt)::value>>((unsigned)n, kNndThreads, smem_init, st, d_vecs.p, d_norms.p, n,
+                                                               dim, m, stride, lkey.p, lid.p);
+        });
+        KB2_CUDA_CHECK(cudaGetLastError());
+        int vbits = 1;
+        while ((1ll << vbits) <= n) vbits++;   // 2^vbits > n: the ~0 keys of unused slots sort after every target
+        cub::DoubleBuffer<uint64_t> dk(rkey[0].p, rkey[1].p);
+        cub::DoubleBuffer<uint32_t> dv(rsrc[0].p, rsrc[1].p);
+        size_t tb = 0;
+        KB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dv, (int)ne, 0, 33 + vbits, st));
+        tmp.alloc_exact(tb);
+        unsigned long long* hc = (unsigned long long*)h_counter.ensure(64);
+        const unsigned rows_per_cta = 256 / kWarp;
+        for (int t = 0; t < nnd_niter; t++) {
+            dk.selector = 0;
+            dv.selector = 0;
+            cagra_nnd_sample_kernel<<<(unsigned)((n + rows_per_cta - 1) / rows_per_cta), 256, 0, st>>>(lid.p, n, m, S, t, fwd.p,
+                                                                                                       rkey[0].p, rsrc[0].p);
+            KB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(tmp.p, tb, dk, dv, (int)ne, 0, 33 + vbits, st));
+            cagra_nnd_offsets_kernel<<<grid1d(2 * n + 1, 256), 256, 0, st>>>(dk.Current(), ne, n, rs.p);
+            NndJoinParams jp{d_vecs.p, d_norms.p, n, dim, m, S, fwd.p, dv.Current(), rs.p, lkey.p, lid.p, lock.p};
+            with_metric(metric, [&](auto mt) {
+                launch<cagra_nnd_join_kernel<decltype(mt)::value>>((unsigned)n, kNndThreads, smem_join, st, jp);
+            });
+            KB2_CUDA_CHECK(cudaGetLastError());
+            KB2_CUDA_CHECK(cudaMemsetAsync(cnt.p, 0, 8, st));
+            cagra_nnd_count_kernel<<<(unsigned)std::min<int64_t>((nm + 255) / 256, 4096), 256, 0, st>>>(lid.p, nm, cnt.p);
+            KB2_CUDA_CHECK(cudaMemcpyAsync(hc, cnt.p, 8, cudaMemcpyDeviceToHost, st));
+            KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+            nnd_updates.push_back((int64_t)hc[0]);
+            if ((double)hc[0] <= kNndDelta * (double)n * (double)m) break;
+        }
+        cagra_nnd_ids_kernel<<<grid1d(nm, 256), 256, 0, st>>>(lid.p, nm, g0);
+        KB2_CUDA_CHECK(cudaGetLastError());
+        if (g0_key) KB2_CUDA_CHECK(cudaMemcpyAsync(g0_key, lkey.p, (size_t)nm * 4, cudaMemcpyDeviceToDevice, st));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
     }
 
     // shared memory of one cagra_search_kernel CTA (layout at the kernel)
@@ -583,8 +1170,10 @@ struct CagraIndex : HnswIndex {
         if (timing) KB2_CUDA_CHECK(cudaEventElapsedTime(&last_kernel_ms, ev0, ev1));
     }
 
-    // gpu_cuvs_cagra_config.h; build_algo, nn_descent_niter, cache_dataset_on_device and adapt_for_cpu are accepted and have
-    // no effect (the intermediate graph is always the exact k-NN graph)
+    // gpu_cuvs_cagra_config.h.  build_algo "NN_DESCENT" (any case) builds the intermediate graph by NN-descent with
+    // nn_descent_niter (1..1000, default 20) as its iteration cap; any other build_algo, or none, builds the exact k-NN
+    // graph.  build_algo is a build-time key and is not stored.  cache_dataset_on_device and adapt_for_cpu are accepted
+    // and have no effect.
     void
     configure(const JsonObj& cfg) override {
         igd = (int)cfg.get_int("intermediate_graph_degree", 128);
@@ -592,6 +1181,12 @@ struct CagraIndex : HnswIndex {
         KB2_REQUIRE(igd >= 1 && igd <= kCagraMaxIgd, KB2_OUT_OF_RANGE_IN_JSON, "intermediate_graph_degree out of range (1..1007)");
         KB2_REQUIRE(gd >= 1 && gd <= kCagraMaxGd && gd <= igd, KB2_OUT_OF_RANGE_IN_JSON,
                     "graph_degree out of range (1..256, and at most intermediate_graph_degree)");
+        std::string algo = cfg.get_str("build_algo", "");
+        for (char& c : algo) c = (char)toupper((unsigned char)c);
+        nn_descent = algo == "NN_DESCENT";
+        nnd_niter = (int)cfg.get_int("nn_descent_niter", 20);
+        KB2_REQUIRE(!nn_descent || (nnd_niter >= 1 && nnd_niter <= 1000), KB2_OUT_OF_RANGE_IN_JSON,
+                    "nn_descent_niter out of range (1..1000)");
     }
 
     void

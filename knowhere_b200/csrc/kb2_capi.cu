@@ -996,6 +996,41 @@ kb2_debug_gemm_keys(const float* q, int64_t nq, const float* x, int64_t nb, int 
     });
 }
 
+// ---------------------------------------------------------------- validation hook for GPU_CAGRA's intermediate graph
+int
+kb2_debug_cagra_knn_graph(const float* x, int64_t n, int dim, int metric, const char* json, int32_t* out_ids, float* out_keys,
+                          int* out_iters, int64_t* out_updates, int updates_cap, float* out_ms, int device) {
+    return guarded([&] {
+        require_device(device);
+        KB2_REQUIRE(x && out_ids && out_keys, KB2_INVALID_ARGS, "null buffer");
+        KB2_REQUIRE(is_device_ptr(x) && is_device_ptr(out_ids) && is_device_ptr(out_keys), KB2_INVALID_ARGS,
+                    "debug_cagra_knn_graph takes device rows, ids and keys");
+        KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP, KB2_INVALID_METRIC_TYPE, "metric must be L2 or IP");
+        KB2_REQUIRE(n >= 2 && n < (1ll << 31) && dim > 0, KB2_INVALID_ARGS, "bad sizes");
+        JsonObj cfg = JsonObj::parse(json);
+        KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
+        CagraIndex ix;
+        ix.init("GPU_CAGRA", metric, dim, device);
+        ix.configure(cfg);
+        ix.n = n;
+        ix.d_vecs.borrow(x, (size_t)n * dim);
+        ix.d_norms.alloc_exact((size_t)n);
+        KB2_CUDA_CHECK(cudaDeviceSynchronize());   // the caller's rows are ready before the index's stream reads them
+        row_norms_kernel<<<grid1d(n * 32, 256), 256, 0, ix.stream>>>(x, n, dim, ix.d_norms.p);
+        const int m = (int)std::min<int64_t>(ix.igd, n - 1);
+        KB2_CUDA_CHECK(cudaEventRecord(ix.ev0, ix.stream));
+        ix.knn_graph(m, out_ids, out_keys);
+        KB2_CUDA_CHECK(cudaEventRecord(ix.ev1, ix.stream));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(ix.stream));
+        KB2_CUDA_CHECK(cudaGetLastError());
+        if (out_iters) *out_iters = (int)ix.nnd_updates.size();
+        for (int t = 0; out_updates && t < (int)ix.nnd_updates.size() && t < updates_cap; t++) out_updates[t] = ix.nnd_updates[t];
+        float ms = 0.f;
+        KB2_CUDA_CHECK(cudaEventElapsedTime(&ms, ix.ev0, ix.ev1));
+        if (out_ms) *out_ms = ms;
+    });
+}
+
 // ---------------------------------------------------------------- introspection
 int
 kb2_index_last_search_counters(kb2_index_t h, int64_t* out8) {
