@@ -48,6 +48,7 @@ enum {
     KB2_INDEX_NOT_TRAINED = 8,
     KB2_INDEX_ALREADY_TRAINED = 9,
     KB2_MALLOC_ERROR = 13,
+    KB2_INVALID_VALUE_IN_JSON = 16,
     KB2_INVALID_BINARY_SET = 19,
     KB2_CUDA_RUNTIME_ERROR = 22,
     KB2_INTERNAL_ERROR = 27,
@@ -56,10 +57,11 @@ enum {
 
 /* metric ids (reference: include/knowhere/comp/index_param.h metric names "L2","IP","COSINE"; the MAX_SIM_* emb-list
  * metrics, index_param.h:280-285, only for kb2_bruteforce_search_emb_list and kb2_index_set_emb_list; "MAX_SIM" is
- * MAX_SIM_COSINE) */
+ * MAX_SIM_COSINE; "BM25" only for sparse rows, with IP) */
 enum {
     KB2_METRIC_L2 = 0, KB2_METRIC_IP = 1, KB2_METRIC_COSINE = 2,
-    KB2_METRIC_MAX_SIM_L2 = 3, KB2_METRIC_MAX_SIM_IP = 4, KB2_METRIC_MAX_SIM_COSINE = 5
+    KB2_METRIC_MAX_SIM_L2 = 3, KB2_METRIC_MAX_SIM_IP = 4, KB2_METRIC_MAX_SIM_COSINE = 5,
+    KB2_METRIC_BM25 = 6
 };
 
 typedef struct kb2_index* kb2_index_t;
@@ -96,7 +98,18 @@ int kb2_device_count(void);
  *             second add, custom ids and sharding return KB2_NOT_IMPLEMENTED, as does RangeSearch;
  *             kb2_index_set_emb_list returns KB2_INVALID_METRIC_TYPE.  kb2_hnsw_export returns the graph as one
  *             HNSW level (levels 1, cum {0, degree}, entry point 0), kb2_hnsw_last_stats {rows evaluated, parents
- *             expanded}, and kb2_index_serialize_faiss an "IHNf" stream the reference's CPU HNSW node loads. */
+ *             expanded}, and kb2_index_serialize_faiss an "IHNf" stream the reference's CPU HNSW node loads.
+ * "SPARSE_INVERTED_INDEX" | "SPARSE_WAND" (DESIGN §4.13): sparse float rows (kb2_index_add_sparse), metric IP or BM25
+ *             (else KB2_INVALID_METRIC_TYPE); dim is ignored and kb2_index_dim returns 0.  Build keys as
+ *             sparse_index_node.cc:121-126 and sparse_index_config.h:173-205: BM25 needs bm25_k1 (0..3), bm25_b (0..1)
+ *             and bm25_avgdl (>= 0) (missing: KB2_INVALID_ARGS, out of range: KB2_OUT_OF_RANGE_IN_JSON);
+ *             inverted_index_algo must be one of the reference's six names (any case) and quant_type fp16 / fp32 (IP)
+ *             or u16 / u32 (BM25), else KB2_INVALID_ARGS.  drop_ratio_build, inverted_index_codec, block_max_block_size
+ *             and sindi_window_size are accepted without effect: values stay fp32 and every search is exhaustive and
+ *             exact, the same for both types and every algorithm.  The dense train / add / search / range search
+ *             return KB2_INVALID_ARGS naming the sparse entry point; sharding, emb-lists, GetVectorByIds and the faiss
+ *             stream KB2_NOT_IMPLEMENTED.  HasRawData is 0, IsTrained 1; the meta JSON adds sparse_dim and nnz.
+ *             kb2_index_size_bytes counts the device postings and term table and the host copy of the rows. */
 int kb2_index_create(const char* index_type, int metric, int dim, const char* json_cfg, int device,
                      kb2_index_t* out);
 void kb2_index_destroy(kb2_index_t h);
@@ -224,6 +237,44 @@ int kb2_bruteforce_range_search(const float* base, int64_t nb, int dim, int metr
                                 const uint8_t* bitset, int64_t bitset_nbits, int64_t** out_lims,
                                 int64_t** out_ids, float** out_dist, int device, void* cuda_stream);
 
+/* ---- sparse float vectors: SPARSE_INVERTED_INDEX / SPARSE_WAND (src/index/sparse/sparse_index_node.cc) and
+ * BruteForce::SearchSparse (src/common/comp/brute_force.cc:1227-1340).  DESIGN §4.13.
+ * A row set is CSR: indptr int64[n + 1] (indptr[0] = 0, non-decreasing), indices uint32[indptr[n]] strictly ascending
+ * within a row, values float32[indptr[n]] finite and >= 0; each array host or device.  Anything else is
+ * KB2_INVALID_ARGS before any kernel indexes by the data.  Scores, evaluated in fp32 in this order:
+ *   IP:   s(q, r) = sum over the kept query entries (t, w) that row r holds (value v), in query order, of w * v
+ *   BM25: the same sum of ((w * (k1 + 1)) * v) / ((v + k1 * (1 - b)) + ((k1 * b) / max(avgdl, 1)) * L_r), L_r = the sum
+ *         of row r's values (scorer.h:81-104; avgdl of the search keys)
+ * Candidates are the rows with s > 0 the bitset keeps; results are ordered by s descending, ties by ascending row; row ids
+ * are positions in add order.  Missing entries: id -1, distance -FLT_MAX (the reference pads with NaN). */
+/* IndexNode::Add on a sparse index (sparse_index_node.cc Train + Add): appends n rows; may be called more than once and
+ * gives the same index as one call with the concatenated rows.  No custom ids. */
+int kb2_index_add_sparse(kb2_index_t h, const int64_t* indptr, const uint32_t* indices, const float* values, int64_t n);
+/* IndexNode::Search on a sparse index (sparse_index_node.cc:767-792, inverted_index.h:151-190): the exact top-k, k 1..16384.
+ * Search keys: drop_ratio_search in [0, 1) (else KB2_OUT_OF_RANGE_IN_JSON) keeps a query entry when its value is >= the
+ * value at position (size_t)(float(ratio) * float(nnz_q)) of the query's values in ascending order (0 when that position
+ * is 0); entries whose index no stored row has are dropped too.  BM25: bm25_avgdl is required (KB2_INVALID_ARGS); bm25_k1
+ * and bm25_b, if given, must equal the build values (KB2_INVALID_VALUE_IN_JSON).  search_algo, dim_max_score_ratio,
+ * refine_factor and bulk_query_nnz_threshold are accepted without effect.  out_ids / out_dist [nq][k], both host or
+ * both device.  kb2_index_last_search_counters: [3] postings scored, [2] their bytes (8 each). */
+int kb2_index_search_sparse(kb2_index_t h, const int64_t* q_indptr, const uint32_t* q_indices, const float* q_values,
+                            int64_t nq, int k, const char* json, const uint8_t* bitset, int64_t bitset_nbits,
+                            int64_t* out_ids, float* out_dist);
+/* IndexNode::RangeSearch on a sparse index: the hits radius < s <= range_filter (has_range_filter = 0: radius < s) among the
+ * candidates, each query's best first, ties by row; same keys as kb2_index_search_sparse and the outputs of
+ * kb2_index_range_search. */
+int kb2_index_range_search_sparse(kb2_index_t h, const int64_t* q_indptr, const uint32_t* q_indices, const float* q_values,
+                                  int64_t nq, float radius, float range_filter, int has_range_filter, const char* json,
+                                  const uint8_t* bitset, int64_t bitset_nbits, int64_t** out_lims, int64_t** out_ids,
+                                  float** out_dist);
+/* BruteForce::SearchSparse (brute_force.cc:1227-1340): nb base rows against nq queries, metric KB2_METRIC_IP or
+ * KB2_METRIC_BM25 (json: bm25_k1, bm25_b and bm25_avgdl, as for the index), k 1..16384.  Every query entry is kept (no
+ * drop_ratio_search), so the result equals a sparse index's over the same rows at drop_ratio_search 0, bit for bit. */
+int kb2_bruteforce_search_sparse(const int64_t* base_indptr, const uint32_t* base_indices, const float* base_values,
+                                 int64_t nb, const int64_t* q_indptr, const uint32_t* q_indices, const float* q_values,
+                                 int64_t nq, int metric, int k, const char* json, const uint8_t* bitset,
+                                 int64_t bitset_nbits, int64_t* out_ids, float* out_dist, int device);
+
 /* ---- emb-list (multi-vector) exact search: knowhere::BruteForce::Search with a MAX_SIM_* metric and EMB_LIST_OFFSET on
  * both datasets (src/common/comp/brute_force.cc:258-300,424-584,626-665; include/knowhere/emb_list_utils.h).
  * Document i is base rows [base_lims[i], base_lims[i+1]), query list j is query rows [query_lims[j], query_lims[j+1]);
@@ -309,7 +360,8 @@ int kb2_index_last_kernel_ms(kb2_index_t h, float* out_ms);
 /* out4: [0] device ms of the whole list-scan stage of the last search, [1] device ms of its dominant kernel
  * (== kb2_index_last_kernel_ms), [2] engine that served it: 0 = query-major scan kernels, 1 = list-major
  * tensor-core engine (IVF_PQ m=16 d=128 with large batches; kb2_ivfpq_tc.cuh), 2 = large-k path, 3 = HNSW beam
- * search with one query per CTA (max(ef, k) too large for the four-queries-per-CTA kernels), 4 = GPU_CAGRA, [3] device ms of the collectives
+ * search with one query per CTA (max(ef, k) too large for the four-queries-per-CTA kernels), 4 = GPU_CAGRA, 5 = sparse tile
+ * scoring (a sparse search with k + 16 > 1024 reports 2), [3] device ms of the collectives
  * (+ merge kernel) of a sharded search with a communicator */
 int kb2_index_last_stage_info(kb2_index_t h, float* out4);
 

@@ -13,7 +13,7 @@ import numpy as np
 from ._build import LIB, build  # noqa: F401
 
 METRIC_L2, METRIC_IP = 0, 1
-_METRICS = {"L2": 0, "IP": 1, "COSINE": 2, 0: 0, 1: 1, 2: 2}
+_METRICS = {"L2": 0, "IP": 1, "COSINE": 2, "BM25": 6, 0: 0, 1: 1, 2: 2, 6: 6}
 
 _lib = None
 
@@ -91,6 +91,11 @@ def _declare(L):
     L.kb2_index_search_emb_list.argtypes = [vp, vp, vp, i64, i32, c.c_char_p, vp, i64, vp, vp, vp]
     L.kb2_index_emb_list_stage_ms.argtypes = [vp, vp]
     L.kb2_debug_maxsim_pairs.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, i32, vp, vp, i32]
+    L.kb2_index_add_sparse.argtypes = [vp, vp, vp, vp, i64]
+    L.kb2_index_search_sparse.argtypes = [vp, vp, vp, vp, i64, i32, c.c_char_p, vp, i64, vp, vp]
+    L.kb2_index_range_search_sparse.argtypes = [vp, vp, vp, vp, i64, f32, f32, i32, c.c_char_p, vp, i64,
+                                                c.POINTER(vp), c.POINTER(vp), c.POINTER(vp)]
+    L.kb2_bruteforce_search_sparse.argtypes = [vp, vp, vp, i64, vp, vp, vp, i64, i32, i32, c.c_char_p, vp, i64, vp, vp, i32]
     L.kb2_debug_cagra_knn_graph.argtypes = [vp, i64, i32, i32, c.c_char_p, vp, vp, vp, vp, i32, vp, i32]
     if hasattr(L, "kb2_faiss_describe"):
         L.kb2_faiss_describe.argtypes = [vp, c.c_size_t, i32, vp, c.c_size_t]
@@ -383,6 +388,30 @@ class Index:
         _check(self.L.kb2_index_emb_list_stage_ms(self.h, _ptr(v)))
         return dict(stage1=float(v[0]), candidates=float(v[1]), rerank=float(v[2]), select=float(v[3]))
 
+    # -- sparse float vectors: SPARSE_INVERTED_INDEX / SPARSE_WAND (DESIGN §4.13).  Row sets are CSR: an (indptr, indices,
+    #    values) tuple of numpy arrays or CUDA tensors, or any object with .indptr / .indices / .data.
+    def add_sparse(self, rows):
+        ip, ix, val, n = _csr(rows)
+        _check(self.L.kb2_index_add_sparse(self.h, _ptr(ip), _ptr(ix), _ptr(val), n))
+
+    def search_sparse(self, q, k, config=None, bitset=None):
+        """Exact top-k of the query rows: (ids, dist) [nq, k], CUDA tensors when the query arrays are; dist is the score."""
+        ip, ix, val, nq = _csr(q)
+        ids, dist = _out(ip, nq, k)
+        _check(self.L.kb2_index_search_sparse(self.h, _ptr(ip), _ptr(ix), _ptr(val), nq, k, _cfg(config), _ptr(bitset),
+                                              _nbits(bitset), _ptr(ids), _ptr(dist)))
+        return ids, dist
+
+    def range_search_sparse(self, q, radius, range_filter=None, config=None, bitset=None):
+        """(lims, ids, dist): the rows with radius < score <= range_filter, each query's best first."""
+        ip, ix, val, nq = _csr(q)
+        pl, pi, pd = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        _check(self.L.kb2_index_range_search_sparse(self.h, _ptr(ip), _ptr(ix), _ptr(val), nq, radius,
+                                                    0.0 if range_filter is None else range_filter,
+                                                    0 if range_filter is None else 1, _cfg(config), _ptr(bitset),
+                                                    _nbits(bitset), ctypes.byref(pl), ctypes.byref(pi), ctypes.byref(pd)))
+        return _take_range(self.L, nq, pl, pi, pd)
+
     # -- introspection for bench.py
     def last_counters(self):
         c = np.zeros(8, np.int64)
@@ -396,7 +425,7 @@ class Index:
     def last_stage_info(self):
         v = np.zeros(4, np.float32)
         _check(self.L.kb2_index_last_stage_info(self.h, _ptr(v)))
-        return dict(stage_ms=float(v[0]), kernel_ms=float(v[1]), engine=("scan", "tc", "large_k", "hnsw_wide", "cagra")[int(round(v[2]))], comm_ms=float(v[3]))
+        return dict(stage_ms=float(v[0]), kernel_ms=float(v[1]), engine=("scan", "tc", "large_k", "hnsw_wide", "cagra", "sparse")[int(round(v[2]))], comm_ms=float(v[3]))
 
     def last_kernel_ms(self):
         v = ctypes.c_float()
@@ -466,6 +495,56 @@ def _take_range(L, nq, pl, pi, pd):
     L.kb2_free(pi)
     L.kb2_free(pd)
     return lims, ids, dist
+
+
+def _nbits(bitset):
+    return 0 if bitset is None else (bitset.numel() if _is_torch(bitset) else bitset.size) * 8
+
+
+def _csr(rows):
+    """(indptr int64, indices uint32, values float32, n) of a CSR row set, without scipy: an (indptr, indices, values)
+    tuple of numpy arrays or torch tensors, or any object with .indptr / .indices / .data.  Torch tensors stay where
+    they are (int32 indices pass as their uint32 bits); numpy arrays are converted."""
+    ip, ix, val = rows if isinstance(rows, tuple) else (rows.indptr, rows.indices, rows.data)
+    if _is_torch(ip):
+        import torch
+        ip = ip.to(torch.int64).contiguous()
+        if ix.dtype != torch.int32:
+            if ix.numel() and (int(ix.min()) < 0 or int(ix.max()) > 0xFFFFFFFF):
+                raise KnowhereError(1, "sparse indices must lie in [0, 2^32)")
+            ix = ix.to(torch.int64).to(torch.int32)   # the same 32 bits as uint32
+        ix = ix.contiguous()
+        val = val.to(torch.float32).contiguous()
+        return ip, ix, val, int(ip.numel()) - 1
+    ip = np.ascontiguousarray(ip, np.int64)
+    ix = np.asarray(ix)
+    if ix.dtype != np.uint32:
+        if ix.size and (ix.min() < 0 or ix.max() > 0xFFFFFFFF):
+            raise KnowhereError(1, "sparse indices must lie in [0, 2^32)")
+        ix = ix.astype(np.uint32)
+    return ip, np.ascontiguousarray(ix), np.ascontiguousarray(val, np.float32), ip.size - 1
+
+
+def _out(like, nq, k):
+    if _is_torch(like) and like.is_cuda:
+        import torch
+        return (torch.empty((nq, k), dtype=torch.int64, device=like.device),
+                torch.empty((nq, k), dtype=torch.float32, device=like.device))
+    return np.empty((nq, k), np.int64), np.empty((nq, k), np.float32)
+
+
+def brute_force_search_sparse(base, queries, k, metric="IP", config=None, bitset=None, device=0):
+    """knowhere::BruteForce::SearchSparse (reference src/common/comp/brute_force.cc:1227-1340): the exact top-k of the
+    query rows over the base rows, both CSR as Index.add_sparse takes them.  BM25 takes bm25_k1, bm25_b and bm25_avgdl
+    from config."""
+    L = lib()
+    bp, bi, bv, nb = _csr(base)
+    qp, qi, qv, nq = _csr(queries)
+    ids, dist = _out(qp, nq, k)
+    _check(L.kb2_bruteforce_search_sparse(_ptr(bp), _ptr(bi), _ptr(bv), nb, _ptr(qp), _ptr(qi), _ptr(qv), nq,
+                                          _METRICS[metric], k, _cfg(config), _ptr(bitset), _nbits(bitset), _ptr(ids),
+                                          _ptr(dist), device))
+    return ids, dist
 
 
 def brute_force_search(base, queries, k, metric="L2", bitset=None, device=0, stream=0):

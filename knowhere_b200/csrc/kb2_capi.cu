@@ -110,6 +110,19 @@ int
 on_index(kb2_index_t h, F&& f) {
     return on_index<IndexBase>(h, "", std::forward<F>(f));
 }
+// guarded call of f(sparse index), under its lock and on its device; a dense handle names its own entry points
+template <typename F>
+int
+on_sparse(kb2_index_t h, F&& f) {
+    return on_index(h, [&](IndexBase* ix) {
+        auto* sx = dynamic_cast<SparseIndex*>(ix);
+        KB2_REQUIRE(sx != nullptr, KB2_INVALID_ARGS,
+                    ix->type + " holds dense rows: use kb2_index_add / kb2_index_search / kb2_index_range_search");
+        sx->last = Counters{};
+        sx->wait_caller_work();
+        f(sx);
+    });
+}
 kb2_index_t
 to_handle(std::unique_ptr<IndexBase> ix) {
     auto* h = new Handle();
@@ -132,6 +145,7 @@ parse_metric(int metric, const JsonObj& cfg) {
         if (m == "L2") return KB2_METRIC_L2;
         if (m == "IP") return KB2_METRIC_IP;
         if (m == "COSINE") return KB2_METRIC_COSINE;
+        if (m == "BM25") return KB2_METRIC_BM25;
         throw Error(KB2_INVALID_METRIC_TYPE, "unsupported metric_type " + m);
     }
     return metric;
@@ -161,12 +175,19 @@ kb2_index_create(const char* index_type, int metric, int dim, const char* json_c
         JsonObj cfg = JsonObj::parse(json_cfg);
         KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
         metric = parse_metric(metric, cfg);
-        KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP || metric == KB2_METRIC_COSINE,
-                    KB2_INVALID_METRIC_TYPE, "metric must be L2, IP or COSINE");
-        if (dim <= 0) dim = (int)cfg.get_int("dim", 0);
-        KB2_REQUIRE(dim > 0, KB2_INVALID_ARGS, "dim must be positive");
-        require_device(device);
         const std::string t = index_type;
+        if (is_sparse_type(t)) {
+            // sparse_index_node.cc:114-119; sparse rows have no fixed dimension
+            KB2_REQUIRE(metric == KB2_METRIC_IP || metric == KB2_METRIC_BM25, KB2_INVALID_METRIC_TYPE,
+                        t + " only supports metric_type IP or BM25");
+            dim = 0;
+        } else {
+            KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP || metric == KB2_METRIC_COSINE,
+                        KB2_INVALID_METRIC_TYPE, "metric must be L2, IP or COSINE");
+            if (dim <= 0) dim = (int)cfg.get_int("dim", 0);
+            KB2_REQUIRE(dim > 0, KB2_INVALID_ARGS, "dim must be positive");
+        }
+        require_device(device);
         std::unique_ptr<IndexBase> ix = make_index(t);
         KB2_REQUIRE(ix, KB2_INVALID_ARGS, "unknown index type " + t);
         // COSINE = inner product of L2-normalised vectors: data is normalised when it enters the index and
@@ -560,8 +581,9 @@ kb2_index_get_meta(kb2_index_t h, char* json_out, size_t cap) {
     return guarded([&] {
         IndexBase* ix = ix_of(h);
         KB2_REQUIRE(json_out && cap > 0, KB2_INVALID_ARGS, "null argument");
+        const char* m = ix->cosine ? "COSINE" : ix->metric == KB2_METRIC_IP ? "IP" : ix->metric == KB2_METRIC_BM25 ? "BM25" : "L2";
         std::string s = "{\"type\": \"" + ix->type + "\", \"dim\": " + std::to_string(ix->dim) + ", \"rows\": " + std::to_string(ix->count()) +
-                        ", \"metric_type\": \"" + (ix->cosine ? "COSINE" : (ix->metric == KB2_METRIC_IP ? "IP" : "L2")) + "\"" +
+                        ", \"metric_type\": \"" + m + "\"" +
                         ", \"size_bytes\": " + std::to_string(ix->size_bytes()) + ", \"device\": " + std::to_string(ix->device) +
                         ", \"shard_rank\": " + std::to_string(ix->shard_rank) + ", \"shard_world\": " + std::to_string(ix->shard_world);
         ix->append_meta(s);
@@ -736,10 +758,83 @@ kb2_bruteforce_search_emb_list(const float* base, const int64_t* base_lims, int6
     });
 }
 
+// ---------------------------------------------------------------- sparse float vectors (kb2_sparse.cuh)
+int
+kb2_index_add_sparse(kb2_index_t h, const int64_t* indptr, const uint32_t* indices, const float* values, int64_t n) {
+    return on_sparse(h, [&](SparseIndex* sx) { sx->add_rows(indptr, indices, values, n); });
+}
+int
+kb2_index_search_sparse(kb2_index_t h, const int64_t* q_indptr, const uint32_t* q_indices, const float* q_values, int64_t nq, int k,
+                        const char* json, const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids, float* out_dist) {
+    return on_sparse(h, [&](SparseIndex* sx) {
+        JsonObj cfg = JsonObj::parse(json);
+        KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
+        sx->search_sparse(q_indptr, q_indices, q_values, nq, k, cfg, bitset, bitset_nbits, out_ids, out_dist, false);
+    });
+}
+int
+kb2_index_range_search_sparse(kb2_index_t h, const int64_t* q_indptr, const uint32_t* q_indices, const float* q_values, int64_t nq,
+                              float radius, float range_filter, int has_range_filter, const char* json, const uint8_t* bitset,
+                              int64_t bitset_nbits, int64_t** out_lims, int64_t** out_ids, float** out_dist) {
+    return on_sparse(h, [&](SparseIndex* sx) {
+        KB2_REQUIRE(out_lims && out_ids && out_dist, KB2_INVALID_ARGS, "null output");
+        JsonObj cfg = JsonObj::parse(json);
+        KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
+        sx->range_search_sparse(q_indptr, q_indices, q_values, nq, radius, range_filter, has_range_filter != 0, cfg, bitset,
+                                bitset_nbits, out_lims, out_ids, out_dist);
+    });
+}
+// The base rows become the rows of a per-device scratch sparse index (same build, same kernels), searched without
+// drop_ratio_search.  Its stream, events and search scratch are reused across calls; its rows and postings are not kept.
+namespace {
+struct SparseBfSlot {
+    std::mutex mu;
+    std::unique_ptr<SparseIndex> sx;
+};
+SparseBfSlot g_sparse_bf[64];
+}  // namespace
+
+int
+kb2_bruteforce_search_sparse(const int64_t* base_indptr, const uint32_t* base_indices, const float* base_values, int64_t nb,
+                             const int64_t* q_indptr, const uint32_t* q_indices, const float* q_values, int64_t nq, int metric, int k,
+                             const char* json, const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids, float* out_dist,
+                             int device) {
+    return guarded([&] {
+        KB2_REQUIRE(nb > 0 && nq >= 0, KB2_INVALID_ARGS, "bad sizes");
+        KB2_REQUIRE(k > 0 && k <= kMaxLargeK, KB2_INVALID_ARGS, "k out of range (1..16384)");
+        KB2_REQUIRE(metric == KB2_METRIC_IP || metric == KB2_METRIC_BM25, KB2_INVALID_METRIC_TYPE, "metric must be IP or BM25");
+        JsonObj cfg = JsonObj::parse(json);
+        KB2_REQUIRE(cfg.ok, KB2_INVALID_PARAM_IN_JSON, "malformed json");
+        require_device(device);
+        KB2_REQUIRE(device < 64, KB2_INVALID_ARGS, "bad device ordinal");
+        SparseBfSlot& slot = g_sparse_bf[device];
+        std::lock_guard<std::mutex> lk(slot.mu);
+        if (!slot.sx) {
+            slot.sx.reset(new SparseIndex());
+            slot.sx->init("SPARSE_INVERTED_INDEX", metric, 0, device);
+        }
+        SparseIndex& sx = *slot.sx;
+        sx.metric = metric;
+        sx.last = Counters{};
+        sx.clear_rows();
+        try {
+            sx.set_bm25(cfg);   // the search config's BM25 parameters; no build-only key is checked here
+            sx.wait_caller_work();
+            sx.add_rows(base_indptr, base_indices, base_values, nb);
+            sx.search_sparse(q_indptr, q_indices, q_values, nq, k, cfg, bitset, bitset_nbits, out_ids, out_dist, true);
+        } catch (...) {
+            sx.clear_rows();
+            throw;
+        }
+        sx.clear_rows();
+    });
+}
+
 // ---------------------------------------------------------------- emb-list search on an index (TokenANN)
 int
 kb2_index_set_emb_list(kb2_index_t h, const int64_t* lims, int64_t n_docs, int metric) {
     return on_index(h, [&](IndexBase* ix) {
+        ix->refuse(IndexBase::kEmbList);
         KB2_REQUIRE(lims != nullptr && n_docs >= 1, KB2_INVALID_ARGS, "emb-list offsets: null, or no document");
         set_emb_list(*ix, read_lims(lims, n_docs, "document"), metric);
     });

@@ -69,7 +69,8 @@ struct IndexBase {
     float last_kernel_ms = 0.f;      // dominant kernel of the last search (IVF_PQ tensor-core engine: the filter kernel)
     float last_stage_ms = 0.f;       // whole list-scan stage of the last search (all engines)
     int last_engine = 0;             // 0: query-major scan kernels, 1: list-major tensor-core engine, 2: large-k path,
-                                     // 3: HNSW beam with one query per CTA (hnsw_wide_kernel)
+                                     // 3: HNSW beam with one query per CTA (hnsw_wide_kernel), 4: GPU_CAGRA,
+                                     // 5: sparse tile scoring (kb2_sparse.cuh)
     float last_comm_ms = 0.f;        // collectives (+ merge) of the last sharded search
     Comm* comm = nullptr;            // not owned (kb2_index_set_comm)
     virtual void set_comm(Comm* c) { comm = c; }
@@ -245,7 +246,7 @@ struct IndexBase {
     // the type's fields of GetIndexMeta, appended to the common JSON prefix
     virtual void append_meta(std::string&) const {}
     // operations a type may leave out: refuse() throws the type's status and message where the operation starts
-    enum Op { kShard, kHnswImport, kRangeSearch };
+    enum Op { kShard, kHnswImport, kRangeSearch, kEmbList };
     virtual void refuse(Op) const {}
     virtual bool takes_emb_list() const { return false; }   // kb2_index_set_emb_list
 };

@@ -13,6 +13,7 @@
 #include "kb2_emb_list_index.cuh"
 #include "kb2_hnsw.cuh"
 #include "kb2_index.cuh"
+#include "kb2_sparse.cuh"
 
 namespace kb2 {
 
@@ -24,8 +25,8 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
     FlatIndex* fi = dynamic_cast<FlatIndex*>(&ix);
     IvfIndex* iv = dynamic_cast<IvfIndex*>(&ix);
     HnswIndex* hn = dynamic_cast<HnswIndex*>(&ix);
-    KB2_REQUIRE(fi || iv || hn, KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
     ix.refuse(IndexBase::kRangeSearch);
+    KB2_REQUIRE(fi || iv || hn, KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
     KB2_REQUIRE(ix.count() > 0, KB2_EMPTY_INDEX, "index is empty");
     if (nq == 0) {
         *out_lims = (int64_t*)calloc(1, sizeof(int64_t));
@@ -237,6 +238,7 @@ make_index(const std::string& type) {
     }
     if (type == "HNSW") return std::make_unique<HnswIndex>();
     if (type == "GPU_CAGRA" || type == "GPU_CUVS_CAGRA") return std::make_unique<CagraIndex>();
+    if (is_sparse_type(type)) return std::make_unique<SparseIndex>();
     return nullptr;
 }
 
@@ -266,9 +268,14 @@ deserialize_index(const uint8_t* blob, size_t size, int device) {
     const std::string type = r.get_str();
     const int metric = r.get<int32_t>();
     const int dim = r.get<int32_t>();
-    KB2_REQUIRE(dim > 0 && dim <= (1 << 20), KB2_INVALID_BINARY_SET, "bad dim in blob");
-    KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP || metric == KB2_METRIC_COSINE, KB2_INVALID_BINARY_SET,
-                "bad metric in blob");
+    if (is_sparse_type(type)) {
+        KB2_REQUIRE(dim == 0, KB2_INVALID_BINARY_SET, "bad dim in blob");
+        KB2_REQUIRE(metric == KB2_METRIC_IP || metric == KB2_METRIC_BM25, KB2_INVALID_BINARY_SET, "bad metric in blob");
+    } else {
+        KB2_REQUIRE(dim > 0 && dim <= (1 << 20), KB2_INVALID_BINARY_SET, "bad dim in blob");
+        KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP || metric == KB2_METRIC_COSINE, KB2_INVALID_BINARY_SET,
+                    "bad metric in blob");
+    }
     std::unique_ptr<IndexBase> ix = make_index(type);
     KB2_REQUIRE(ix, KB2_INVALID_BINARY_SET, "unknown index type in blob");
     ix->init(type, metric, dim, device);   // COSINE: the stored vectors are already normalised; queries will be
