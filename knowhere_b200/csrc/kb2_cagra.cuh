@@ -1200,7 +1200,7 @@ struct CagraIndex : HnswIndex {
         igd = r.get<int32_t>();
         gd = r.get<int32_t>();
         HnswIndex::load(r);
-        KB2_REQUIRE(max_level == 0 && h_cum.size() == 2 && !custom_labels, KB2_INVALID_BINARY_SET, "GPU_CAGRA: bad graph in blob");
+        KB2_REQUIRE(max_level == 0 && h_cum.size() == 2 && !labels.custom, KB2_INVALID_BINARY_SET, "GPU_CAGRA: bad graph in blob");
         for (int64_t i = 0; i < n; i++)
             KB2_REQUIRE(h_offsets[i] == i * h_cum[1], KB2_INVALID_BINARY_SET, "GPU_CAGRA: bad graph in blob");
     }

@@ -635,8 +635,6 @@ bf_prepare(BfSlot& slot, int device, int metric, int dim, void* cuda_stream, con
     fi.norms.ensure(nb);
     row_norms_kernel<<<grid1d(nb * 32, 256), 256, 0, fi.stream>>>(fi.base.p, nb, dim, fi.norms.p);
     fi.norms_used = (size_t)nb;
-    fi.custom_labels = false;
-    fi.n_global_added = nb;
     KB2_CUDA_CHECK(cudaGetLastError());
     return fi;
 }

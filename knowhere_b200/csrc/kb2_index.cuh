@@ -52,6 +52,43 @@ dev_append(DevBuf<T>& buf, size_t& used, const T* src, size_t count, cudaStream_
     used += count;
 }
 
+// Row -> external id of a dense index.  While every id is its row no array exists and device() is null, which every kernel
+// reads as "the id is the row"; the first custom id, or ids that are not the rows (a shard's slice), turn it into an array.
+struct RowLabels {
+    DevBuf<int64_t> d;
+    size_t used = 0;
+    bool custom = false;
+    const int64_t* device() const { return custom ? d.p : nullptr; }
+    // ids of the m rows stored after the `have` ones: ids[0, m) (host or device), else first_id + i.  `force` keeps an
+    // array even without ids.
+    void
+    append(int64_t have, const int64_t* ids, int64_t m, int64_t first_id, bool force, cudaStream_t st) {
+        if (!custom && (ids || force)) {
+            std::vector<int64_t> h(have);
+            for (int64_t i = 0; i < have; i++) h[i] = i;
+            used = 0;
+            if (have) dev_append(d, used, h.data(), (size_t)have, st);
+            KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+            custom = true;
+        }
+        if (!custom || m <= 0) return;
+        std::vector<int64_t> h;
+        if (!ids) {
+            h.resize(m);
+            for (int64_t i = 0; i < m; i++) h[i] = first_id + i;
+        }
+        dev_append(d, used, ids ? ids : h.data(), (size_t)m, st);
+        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+    }
+    // the first n ids on the host, or nothing while they are the rows
+    std::vector<int64_t>
+    host(int64_t n) const {
+        std::vector<int64_t> h(custom ? n : 0);
+        if (!h.empty()) KB2_CUDA_CHECK(cudaMemcpy(h.data(), d.p, h.size() * 8, cudaMemcpyDeviceToHost));
+        return h;
+    }
+};
+
 struct EmbListState;   // kb2_emb_list_index.cuh
 
 // ============================================================================================
@@ -63,6 +100,14 @@ struct IndexBase {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     int shard_rank = 0, shard_world = 1;
+    // FLAT and HNSW shards keep a row slice of each add(): rows offered over all calls, first global row of the first slice
+    int64_t n_global = 0, shard_lo = 0;
+    // rows [lo, hi) of an n-row add() that this shard keeps (all of them without sharding)
+    std::pair<int64_t, int64_t>
+    shard_slice(int64_t n) const {
+        return {n * shard_rank / shard_world, n * (shard_rank + 1) / shard_world};
+    }
+    RowLabels labels;
     std::mutex mu;
     Counters last;
     bool timing = false;
@@ -227,7 +272,8 @@ struct IndexBase {
     virtual void search(const float* q, int64_t nq, int k, const JsonObj& cfg, const uint8_t* bitset, int64_t nbits,
                         int64_t* out_ids, float* out_dist) = 0;
     virtual int64_t count() const = 0;
-    virtual int64_t bitset_rows() const { return count(); }   // rows a BitsetView must cover (whole index, also on a shard)
+    // rows a BitsetView must cover (whole index, also on a shard)
+    virtual int64_t bitset_rows() const { return shard_world > 1 ? n_global : count(); }
     virtual int64_t size_bytes() const = 0;
     virtual bool is_trained() const = 0;
     virtual bool has_raw() const = 0;
@@ -248,7 +294,22 @@ struct IndexBase {
     // operations a type may leave out: refuse() throws the type's status and message where the operation starts
     enum Op { kShard, kHnswImport, kRangeSearch, kEmbList };
     virtual void refuse(Op) const {}
+    // RangeSearch (kb2_range.cuh): every hit of the rp.sp.nq queries described by rp (queries, bitset, radius, filter), on
+    // the host, its pos the index's row.  A type whose hits carry the rank of their probed list sets nprobe, and
+    // max_empty_result_buckets applies.
+    virtual std::vector<RangeHit>
+    range_hits(const RangeParams&, const JsonObj&, int&) {
+        throw Error(KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
+    }
     virtual bool takes_emb_list() const { return false; }   // kb2_index_set_emb_list
+    // emb-lists (kb2_emb_list_index.cuh): the fp32 rows the MaxSim re-rank reads, and each row's position among them (null:
+    // row order)
+    virtual std::pair<const float*, const int32_t*>
+    emb_list_rows() {
+        throw Error(KB2_NOT_IMPLEMENTED, "emb-lists are not implemented on " + type);
+    }
+    // emb-lists: the config of the stage-1 search, which returns vec_topk rows per token for k documents per query list
+    virtual void emb_list_base_config(JsonObj&, int k, int vec_topk) const {}
 };
 
 // ============================================================================================
@@ -588,70 +649,85 @@ dense_knn(IndexBase& ix, const float* Q, int64_t nq, const float* X, const float
 }
 
 // ============================================================================================
+// RangeSearch scans (range_scan_kernel); kb2_range.cuh orders the hits and builds lims
+// ============================================================================================
+inline std::vector<RangeHit>
+hits_to_host(IndexBase& ix, const RangeHit* hits, size_t n) {
+    std::vector<RangeHit> h(n);
+    if (n) KB2_CUDA_CHECK(cudaMemcpy(h.data(), hits, n * sizeof(RangeHit), cudaMemcpyDeviceToHost));
+    ix.last.d2h += (int64_t)(n * sizeof(RangeHit));
+    return h;
+}
+
+// the hits of range_scan_kernel over rp (rp.sp.nq x rp.sp.nsplit CTAs of smem bytes), row positions as the scan emits them.
+// A scan whose hits overflow the buffer runs once more into a buffer of the count it reported.
+inline std::vector<RangeHit>
+range_scan(IndexBase& ix, RangeParams rp, size_t smem) {
+    cudaStream_t st = ix.stream;
+    DevBuf<RangeHit> hits;
+    DevBuf<unsigned long long> cnt;
+    cnt.ensure(1);
+    unsigned long long cap = (unsigned long long)std::max<int64_t>(1 << 20, (int64_t)rp.sp.nq * 256), found = 0;
+    for (int attempt = 0; attempt < 2; attempt++) {
+        hits.ensure(cap);
+        KB2_CUDA_CHECK(cudaMemsetAsync(cnt.p, 0, 8, st));
+        rp.hits = hits.p;
+        rp.count = cnt.p;
+        rp.cap = cap;
+        launch<range_scan_kernel>((unsigned)((int64_t)rp.sp.nq * rp.sp.nsplit), kScanThreads, smem, st, rp);
+        ix.last.launches++;
+        KB2_CUDA_CHECK(cudaGetLastError());
+        KB2_CUDA_CHECK(cudaMemcpyAsync(&found, cnt.p, 8, cudaMemcpyDeviceToHost, st));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+        if (found <= cap) break;
+        cap = found;
+    }
+    return hits_to_host(ix, hits.p, found);
+}
+
+// range_scan of the n rows X, stored in row order (FLAT, HNSW's brute-force case)
+inline std::vector<RangeHit>
+range_scan_rows(IndexBase& ix, RangeParams rp, const float* X, int64_t n) {
+    const int64_t nq = rp.sp.nq;
+    rp.kind = 0;
+    rp.sp.vecs = X;
+    rp.sp.rows = nullptr;
+    rp.single_len = n;
+    rp.sp.nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nq - 1) / nq), std::max<int64_t>(1, n / 1024));
+    return range_scan(ix, rp, (size_t)ix.dim * 4 + 128);
+}
+
+// ============================================================================================
 // FLAT
 // ============================================================================================
 struct FlatIndex : IndexBase {
     DevBuf<float> base, norms;
-    DevBuf<int64_t> labels;   // only when custom ids were given or the shard is offset
-    size_t n_used = 0, norms_used = 0, labels_used = 0;
-    bool custom_labels = false;
-    int64_t n_global_added = 0;  // rows offered to add() over all calls (for sharding)
+    size_t n_used = 0, norms_used = 0;
     int n_add_calls = 0;
-    int64_t shard_lo = 0;        // first global row of this shard's slice (single add() call)
-    int64_t bitset_rows() const override { return shard_world > 1 ? n_global_added : count(); }
 
     void train(const float*, int64_t) override {}
     bool is_trained() const override { return true; }
     bool has_raw() const override { return true; }
     int64_t count() const override { return (int64_t)(n_used / std::max(dim, 1)); }
-    int64_t size_bytes() const override { return (int64_t)(n_used * 4 + norms_used * 4 + labels_used * 8); }
+    int64_t size_bytes() const override { return (int64_t)(n_used * 4 + norms_used * 4 + labels.used * 8); }
 
     void
     add(const float* x, int64_t n, const int64_t* ids) override {
         if (n <= 0) return;
-        // sharding: this rank keeps the contiguous slice [lo, hi) of each add() call
-        int64_t lo = 0, hi = n;
-        if (shard_world > 1) {
-            lo = n * shard_rank / shard_world;
-            hi = n * (shard_rank + 1) / shard_world;
-        }
+        const auto [lo, hi] = shard_slice(n);
         const int64_t m = hi - lo;
-        const int64_t first_label = n_global_added + lo;
         if (n_add_calls++ == 0) shard_lo = lo;
-        const bool need_labels = custom_labels || ids != nullptr || shard_world > 1;
-        if (need_labels && !custom_labels) {
-            // materialise identity labels for what is already stored
-            const int64_t have = count();
-            std::vector<int64_t> h(have);
-            for (int64_t i = 0; i < have; i++) h[i] = i;
-            labels_used = 0;
-            if (have) dev_append(labels, labels_used, h.data(), (size_t)have, stream);
-            KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
-            custom_labels = true;
-        }
         if (m > 0) {
             dev_append(base, n_used, x + lo * dim, (size_t)m * dim, stream);
             DevBuf<float> tmp;
             tmp.ensure(m);
             row_norms_kernel<<<grid1d(m * 32, 256), 256, 0, stream>>>(base.p + n_used - (size_t)m * dim, m, dim, tmp.p);
             dev_append(norms, norms_used, tmp.p, (size_t)m, stream);
-            if (custom_labels) {
-                std::vector<int64_t> h(m);
-                if (ids) {
-                    if (is_device_ptr(ids)) {
-                        KB2_CUDA_CHECK(cudaMemcpyAsync(h.data(), ids + lo, m * 8, cudaMemcpyDeviceToHost, stream));
-                        KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
-                    } else {
-                        memcpy(h.data(), ids + lo, m * 8);
-                    }
-                } else {
-                    for (int64_t i = 0; i < m; i++) h[i] = first_label + i;
-                }
-                dev_append(labels, labels_used, h.data(), (size_t)m, stream);
-            }
             KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
         }
-        n_global_added += n;
+        // a shard's ids are global rows: an id array from its first add() on
+        labels.append(count() - m, ids ? ids + lo : nullptr, m, n_global + lo, shard_world > 1, stream);
+        n_global += n;
     }
 
     void
@@ -671,7 +747,7 @@ struct FlatIndex : IndexBase {
         KB2_REQUIRE(!(dbits && shard_world > 1 && n_add_calls > 1), KB2_NOT_IMPLEMENTED,
                     "FLAT shard: bitset after several add() calls");
         last.flagged = dense_knn(*this, dq, nq, base.p, norms.p, n, dim, metric, k, k + 16, dbits, shard_world > 1 ? shard_lo : 0,
-                                 custom_labels ? labels.p : nullptr, d_ids, d_dist, true, timing ? ev1 : nullptr);
+                                 labels.device(), d_ids, d_dist, true, timing ? ev1 : nullptr);
         last.codes = nq * n;
         last.code_bytes = n * (int64_t)dim * 4;  // list-major contraction reads the base once per batch
         last.pairs = nq;
@@ -685,7 +761,7 @@ struct FlatIndex : IndexBase {
 
     void
     get_vectors(const int64_t* ids, int64_t n, float* out) override {
-        KB2_REQUIRE(!custom_labels, KB2_NOT_IMPLEMENTED, "GetVectorByIds with custom ids");
+        KB2_REQUIRE(!labels.custom, KB2_NOT_IMPLEMENTED, "GetVectorByIds with custom ids");
         std::vector<int64_t> h(n);
         if (is_device_ptr(ids)) {
             KB2_CUDA_CHECK(cudaMemcpy(h.data(), ids, n * 8, cudaMemcpyDeviceToHost));
@@ -703,15 +779,12 @@ struct FlatIndex : IndexBase {
     save(BlobWriter& w) override {
         const int64_t n = count();
         w.put<int64_t>(n);
-        w.put<int32_t>(custom_labels ? 1 : 0);
+        w.put<int32_t>(labels.custom ? 1 : 0);
         std::vector<float> h((size_t)n * dim);
         if (n) KB2_CUDA_CHECK(cudaMemcpy(h.data(), base.p, h.size() * 4, cudaMemcpyDeviceToHost));
         w.put_bytes(h.data(), h.size() * 4);
-        if (custom_labels) {
-            std::vector<int64_t> l(n);
-            if (n) KB2_CUDA_CHECK(cudaMemcpy(l.data(), labels.p, n * 8, cudaMemcpyDeviceToHost));
-            w.put_bytes(l.data(), n * 8);
-        }
+        const std::vector<int64_t> l = labels.host(n);
+        w.put_bytes(l.data(), l.size() * 8);
     }
     void
     load(BlobReader& r) override {
@@ -729,13 +802,17 @@ struct FlatIndex : IndexBase {
     }
     void
     to_faiss(FaissIndexData& o) override {
-        KB2_REQUIRE(!custom_labels, KB2_NOT_IMPLEMENTED, "faiss stream: FLAT with custom ids");
+        KB2_REQUIRE(!labels.custom, KB2_NOT_IMPLEMENTED, "faiss stream: FLAT with custom ids");
         o.xb.resize((size_t)o.ntotal * o.d);
         if (o.ntotal) KB2_CUDA_CHECK(cudaMemcpy(o.xb.data(), base.p, o.xb.size() * 4, cudaMemcpyDeviceToHost));
     }
     void
     from_faiss(const FaissIndexData& o) override {
         if (o.ntotal) add(o.cosine ? normalized(o.xb.data(), o.ntotal) : o.xb.data(), o.ntotal, nullptr);
+    }
+    std::vector<RangeHit>
+    range_hits(const RangeParams& rp, const JsonObj&, int&) override {
+        return range_scan_rows(*this, rp, base.p, count());
     }
 };
 
@@ -755,9 +832,7 @@ struct IvfIndex : IndexBase {
     DevBuf<int32_t> f_assign;
     DevBuf<uint8_t> f_codes;
     DevBuf<float> f_vecs;
-    DevBuf<int64_t> f_labels;
-    size_t f_assign_used = 0, f_codes_used = 0, f_vecs_used = 0, f_labels_used = 0;
-    bool custom_labels = false;
+    size_t f_assign_used = 0, f_codes_used = 0, f_vecs_used = 0;
     int64_t n_total = 0;
     // sealed (list-order) layout
     bool sealed = false;
@@ -771,7 +846,6 @@ struct IvfIndex : IndexBase {
     DevBuf<uint8_t> codes;     // [G][npad][16] or [npad][M]
     DevBuf<uint16_t> vecs16;          // refine store when refine_kind != 0 (vecs is released after seal)
     DevBuf<float> t1, vecs, vnorm2;   // vnorm2[pos] = |x|^2 (IVF_FLAT: row term of the list-major tensor-core engine)
-    DevBuf<int64_t> labels;    // row -> label (sealed copy of f_labels)
     DevBuf<int32_t> s_qkey, s_qkey2, s_qidx, s_qperm;
     DevBuf<uint8_t> s_sort_tmp;
 
@@ -787,6 +861,7 @@ struct IvfIndex : IndexBase {
         return tmp.p;
     }
     int64_t count() const override { return n_total; }
+    int64_t bitset_rows() const override { return n_total; }   // a shard holds every row (it owns whole lists)
     int64_t
     size_bytes() const override {
         return (int64_t)(centroids.bytes() + pqc.bytes() + codes.bytes() + t1.bytes() + vecs.bytes() + vecs16.bytes() + rows.bytes() +
@@ -874,32 +949,10 @@ struct IvfIndex : IndexBase {
             dev_append(f_codes, f_codes_used, cb.p, (size_t)n * M, stream);
         }
         if (keeps_vecs()) dev_append(f_vecs, f_vecs_used, dx, (size_t)n * dim, stream);
-        append_labels(ids, n);
+        labels.append(n_total, ids, n, n_total, false, stream);
         KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
         KB2_CUDA_CHECK(cudaGetLastError());
         n_total += n;
-    }
-
-    void
-    append_labels(const int64_t* ids, int64_t n) {
-        if (ids && !custom_labels) {
-            std::vector<int64_t> h(n_total);
-            for (int64_t i = 0; i < n_total; i++) h[i] = i;
-            f_labels_used = 0;
-            if (n_total) dev_append(f_labels, f_labels_used, h.data(), (size_t)n_total, stream);
-            KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
-            custom_labels = true;
-        }
-        if (custom_labels) {
-            if (ids) {
-                dev_append(f_labels, f_labels_used, ids, (size_t)n, stream);
-            } else {
-                std::vector<int64_t> h(n);
-                for (int64_t i = 0; i < n; i++) h[i] = n_total + i;
-                dev_append(f_labels, f_labels_used, h.data(), (size_t)n, stream);
-            }
-            KB2_CUDA_CHECK(cudaStreamSynchronize(stream));
-        }
     }
 
     // ---------------------------------------------------------------- list-order layout
@@ -1009,13 +1062,9 @@ struct IvfIndex : IndexBase {
                 vecs.release();
             }
         }
-        if (custom_labels) {
-            labels.alloc_exact(std::max<int64_t>(n, 1));
-            KB2_CUDA_CHECK(cudaMemcpyAsync(labels.p, f_labels.p, n * 8, cudaMemcpyDeviceToDevice, st));
-        }
         KB2_CUDA_CHECK(cudaStreamSynchronize(st));
         KB2_CUDA_CHECK(cudaGetLastError());
-        // the insertion-order payload is no longer needed (assign/labels stay: small)
+        // the insertion-order payload is no longer needed (assign stays: small)
         f_codes.release();
         f_vecs.release();
         sealed = true;
@@ -1043,6 +1092,37 @@ struct IvfIndex : IndexBase {
         }
         KB2_CUDA_CHECK(cudaStreamSynchronize(st));
         sealed = false;
+    }
+
+    // the scan parameters every IVF scan starts from: the queries, the bitset, the probes in s_probe_* and the list store.
+    // rp.sp for the query-major scan kernels, rp whole for range_scan_kernel (RangeSearch, the large-k path).
+    RangeParams
+    list_params(const float* dq, int64_t nq, int nprobe, const uint8_t* dbits) const {
+        RangeParams rp{};
+        IvfScanParams& sp = rp.sp;
+        sp.queries = dq;
+        sp.nq = (int)nq;
+        sp.d = dim;
+        sp.metric = metric;
+        sp.bitset = dbits;
+        sp.probe_ids = s_probe_ids.p;
+        sp.probe_dis = s_probe_dis.p;
+        sp.nprobe = nprobe;
+        sp.list_off = list_off.p;
+        sp.list_len = list_len.p;
+        sp.rows = rows.p;
+        sp.vecs = vecs.p;
+        sp.pq_centroids = pqc.p;
+        sp.M = M;
+        sp.dsub = dsub;
+        sp.codes = (const uint4*)codes.p;
+        sp.npad = npad;
+        sp.t1 = t1.p;
+        rp.kind = is_pq ? (G > 0 ? 1 : 2) : 0;
+        rp.G = G;
+        rp.codes_b = codes.p;
+        rp.single_len = -1;
+        return rp;
     }
 
     // ---------------------------------------------------------------- query-major scan launch (all IVF kinds)
@@ -1552,30 +1632,8 @@ struct IvfIndex : IndexBase {
         const int64_t g = large_k_group(nq, L * 8 + large_k_row_bytes(K));
         s_lk_rows.ensure((size_t)g * L);
         s_lk_cand.ensure((size_t)g * K);
-        RangeParams rp{};
+        RangeParams rp = list_params(dq, nq, nprobe, dbits);
         IvfScanParams& sp = rp.sp;
-        sp.queries = dq;
-        sp.nq = (int)nq;
-        sp.d = dim;
-        sp.metric = metric;
-        sp.bitset = dbits;
-        sp.probe_ids = s_probe_ids.p;
-        sp.probe_dis = s_probe_dis.p;
-        sp.nprobe = nprobe;
-        sp.list_off = list_off.p;
-        sp.list_len = list_len.p;
-        sp.rows = rows.p;
-        sp.vecs = vecs.p;
-        sp.pq_centroids = pqc.p;
-        sp.M = M;
-        sp.dsub = dsub;
-        sp.codes = (const uint4*)codes.p;
-        sp.npad = npad;
-        sp.t1 = t1.p;
-        rp.kind = is_pq ? (G > 0 ? 1 : 2) : 0;
-        rp.G = G;
-        rp.codes_b = codes.p;
-        rp.single_len = -1;
         rp.dense = s_lk_rows.p;
         rp.dense_ld = L;
         rp.scanned = d_counter.p;
@@ -1587,7 +1645,7 @@ struct IvfIndex : IndexBase {
         fp.k_sel = K;
         fp.k_out = k;
         fp.rows = rows.p;
-        fp.labels = custom_labels ? labels.p : nullptr;
+        fp.labels = labels.device();
         fp.rerank = use_refine ? 1 : 0;
         fp.raw = vecs.p;
         fp.raw16 = (is_pq && refine_kind) ? vecs16.p : nullptr;
@@ -1705,29 +1763,11 @@ struct IvfIndex : IndexBase {
         const int np_max = (nprobe + nsplit - 1) / nsplit;
         s_partial2.ensure((size_t)nq * nsplit * Ksel);
         KB2_CUDA_CHECK(cudaMemsetAsync(d_counter.p, 0, 64, st));
-        IvfScanParams sp{};
-        sp.queries = dq;
-        sp.nq = (int)nq;
-        sp.d = dim;
-        sp.metric = metric;
-        sp.probe_ids = s_probe_ids.p;
-        sp.probe_dis = s_probe_dis.p;
-        sp.nprobe = nprobe;
-        sp.list_off = list_off.p;
-        sp.list_len = list_len.p;
+        IvfScanParams sp = list_params(dq, nq, nprobe, dbits).sp;
         sp.nsplit = nsplit;
         sp.K = Ksel;
         sp.kout = Ksel;
         sp.partial = s_partial2.p;
-        sp.bitset = dbits;
-        sp.rows = rows.p;
-        sp.vecs = vecs.p;
-        sp.pq_centroids = pqc.p;
-        sp.M = M;
-        sp.dsub = dsub;
-        sp.codes = (const uint4*)codes.p;
-        sp.npad = npad;
-        sp.t1 = t1.p;
         sp.counters = d_counter.p;
         sp.qperm = qperm;
         const unsigned grid = (unsigned)(nq * nsplit);
@@ -1768,7 +1808,7 @@ struct IvfIndex : IndexBase {
             fp.k_sel = flat_tc ? k_base + 16 : k_base;   // tensor-core IVF_FLAT: 3xTF32 keys, exact re-rank of the k+16 best
             fp.k_out = k;
             fp.rows = rows.p;
-            fp.labels = custom_labels ? labels.p : nullptr;
+            fp.labels = labels.device();
             fp.rerank = (use_refine || flat_tc) ? 1 : 0;
             fp.raw = vecs.p;
             fp.raw16 = (is_pq && refine_kind) ? vecs16.p : nullptr;
@@ -1810,7 +1850,7 @@ struct IvfIndex : IndexBase {
     void
     get_vectors(const int64_t* ids, int64_t n, float* out) override {
         KB2_REQUIRE(keeps_vecs(), KB2_NOT_IMPLEMENTED, "index holds no raw data");
-        KB2_REQUIRE(!custom_labels && shard_world == 1, KB2_NOT_IMPLEMENTED, "GetVectorByIds with custom ids / shards");
+        KB2_REQUIRE(!labels.custom && shard_world == 1, KB2_NOT_IMPLEMENTED, "GetVectorByIds with custom ids / shards");
         seal();
         std::vector<int64_t> h(n);
         if (is_device_ptr(ids)) {
@@ -1892,12 +1932,11 @@ struct IvfIndex : IndexBase {
                 imp_codes.swap(c2);
                 for (int64_t i = 0; i < n; i++) imp_labels[i] = i;
             }
-            custom_labels = !perm;
+            labels = RowLabels{};
+            if (!perm) labels.append(0, imp_labels.data(), n, 0, true, stream);
         }
         f_assign_used = 0;
         dev_append(f_assign, f_assign_used, imp_assign.data(), (size_t)n, stream);
-        f_labels_used = 0;
-        if (custom_labels) dev_append(f_labels, f_labels_used, imp_labels.data(), (size_t)n, stream);
         if (is_pq) {
             f_codes_used = 0;
             dev_append(f_codes, f_codes_used, imp_codes.data(), imp_codes.size(), stream);
@@ -1940,12 +1979,8 @@ struct IvfIndex : IndexBase {
         if (len == 0) return;
         std::vector<int32_t> hrows(len);
         KB2_CUDA_CHECK(cudaMemcpy(hrows.data(), rows.p + off, len * 4, cudaMemcpyDeviceToHost));
-        std::vector<int64_t> hl;
-        if (custom_labels) {
-            hl.resize(n_total);
-            KB2_CUDA_CHECK(cudaMemcpy(hl.data(), labels.p, n_total * 8, cudaMemcpyDeviceToHost));
-        }
-        for (int64_t i = 0; i < len; i++) ids[i] = custom_labels ? hl[hrows[i]] : hrows[i];
+        const std::vector<int64_t> hl = labels.host(n_total);
+        for (int64_t i = 0; i < len; i++) ids[i] = hl.empty() ? hrows[i] : hl[hrows[i]];
         if (!is_pq) {
             KB2_CUDA_CHECK(cudaMemcpy(cds, vecs.p + off * dim, (size_t)len * dim * 4, cudaMemcpyDeviceToHost));
         } else if (G > 0) {
@@ -2086,7 +2121,7 @@ struct IvfIndex : IndexBase {
         }
         o.has_refine = is_pq && refine;
         if (o.has_refine) {
-            KB2_REQUIRE(!custom_labels, KB2_NOT_IMPLEMENTED, "faiss stream: refine store with custom ids");
+            KB2_REQUIRE(!labels.custom, KB2_NOT_IMPLEMENTED, "faiss stream: refine store with custom ids");
             KB2_REQUIRE(refine_kind == 0, KB2_NOT_IMPLEMENTED, "faiss stream: only a flat fp32 refine store is written");
             // refine store in id order: row r lives at position pos_of_row[r]
             DevBuf<float> byrow;
@@ -2116,7 +2151,38 @@ struct IvfIndex : IndexBase {
         s += ", \"nlist\": " + std::to_string(nlist);
         if (is_pq) s += ", \"m\": " + std::to_string(M) + ", \"nbits\": " + std::to_string(nbits) + ", \"refine\": " + (refine ? "true" : "false");
     }
+    // RangeSearch: the hits of the nprobe nearest lists, their positions mapped to rows
+    std::vector<RangeHit>
+    range_hits(const RangeParams& q, const JsonObj& cfg, int& nprobe) override {
+        KB2_REQUIRE(trained, KB2_INDEX_NOT_TRAINED, "index not trained");
+        seal();
+        const int64_t nq = q.sp.nq;
+        nprobe = (int)std::min<int64_t>(std::max<int64_t>(cfg.get_int("nprobe", 8), 1), nlist);
+        s_probe_ids.ensure((size_t)nq * nprobe);
+        s_probe_dis.ensure((size_t)nq * nprobe);
+        coarse_probes(q.sp.queries, 0, nq, nprobe);
+        RangeParams rp = list_params(q.sp.queries, nq, nprobe, q.sp.bitset);
+        rp.radius = q.radius;
+        rp.range_filter = q.range_filter;
+        rp.has_filter = q.has_filter;
+        rp.sp.nsplit = (nq < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq) : 1;
+        const int np_max = (nprobe + rp.sp.nsplit - 1) / rp.sp.nsplit;
+        size_t smem = (size_t)dim * 4 + 64 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12;
+        if (is_pq) smem += (size_t)M * 1024;
+        KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "range search: m too large");
+        std::vector<RangeHit> h = range_scan(*this, rp, smem);
+        std::vector<int32_t> hrows(npad);
+        KB2_CUDA_CHECK(cudaMemcpy(hrows.data(), rows.p, npad * 4, cudaMemcpyDeviceToHost));
+        for (RangeHit& e : h) e.pos = (uint32_t)hrows[e.pos];
+        return h;
+    }
+
     bool takes_emb_list() const override { return !is_pq; }
+    std::pair<const float*, const int32_t*>
+    emb_list_rows() override {
+        seal();
+        return {vecs.p, pos_of_row.p};
+    }
 };
 
 }  // namespace kb2

@@ -21,12 +21,7 @@ inline void
 range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius, float range_filter, bool has_filter,
                    const JsonObj& cfg, const uint8_t* bitset, int64_t nbits, int64_t** out_lims, int64_t** out_ids,
                    float** out_dist) {
-    cudaStream_t st = ix.stream;
-    FlatIndex* fi = dynamic_cast<FlatIndex*>(&ix);
-    IvfIndex* iv = dynamic_cast<IvfIndex*>(&ix);
-    HnswIndex* hn = dynamic_cast<HnswIndex*>(&ix);
     ix.refuse(IndexBase::kRangeSearch);
-    KB2_REQUIRE(fi || iv || hn, KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
     KB2_REQUIRE(ix.count() > 0, KB2_EMPTY_INDEX, "index is empty");
     if (nq == 0) {
         *out_lims = (int64_t*)calloc(1, sizeof(int64_t));
@@ -34,116 +29,24 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
         *out_dist = (float*)malloc(4);
         return;
     }
-    const float* dq = ix.to_device(queries, (size_t)nq * ix.dim, ix.s_q);
-    const uint8_t* dbits = ix.bitset_to_device(bitset, nbits);
     RangeParams rp{};
-    IvfScanParams& sp = rp.sp;
-    sp.queries = dq;
-    sp.nq = (int)nq;
-    sp.d = ix.dim;
-    sp.metric = ix.metric;
-    sp.bitset = dbits;
+    rp.sp.queries = ix.to_device(queries, (size_t)nq * ix.dim, ix.s_q);
+    rp.sp.nq = (int)nq;
+    rp.sp.d = ix.dim;
+    rp.sp.metric = ix.metric;
+    rp.sp.bitset = ix.bitset_to_device(bitset, nbits);
     rp.radius = radius;
     rp.range_filter = range_filter;
     rp.has_filter = has_filter ? 1 : 0;
     rp.single_len = -1;
-    int nprobe = 1;
-    int max_empty = 0;
-    size_t smem = (size_t)ix.dim * 4 + 64;
-    DevBuf<RangeHit> hits;
-    unsigned long long found = 0;
-    bool graph_hits = false;   // hits came from the HNSW traversal (range_filter still to be applied)
-    if (hn) {
-        bool bf = false;
-        found = hn->range_hits(dq, nq, radius, cfg, dbits, hits, bf);
-        graph_hits = !bf;
-    }
-    if (fi || (hn && !graph_hits)) {
-        // exact scan of the stored vectors (FLAT; HNSW when the reference falls back to brute force)
-        rp.kind = 0;
-        sp.vecs = fi ? fi->base.p : hn->d_vecs.p;
-        sp.rows = nullptr;
-        rp.single_len = ix.count();
-        sp.nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nq - 1) / nq),
-                                           std::max<int64_t>(1, ix.count() / 1024));
-        smem += 64;
-    } else if (iv) {
-        KB2_REQUIRE(iv->trained, KB2_INDEX_NOT_TRAINED, "index not trained");
-        iv->seal();
-        nprobe = (int)std::min<int64_t>(std::max<int64_t>(cfg.get_int("nprobe", 8), 1), iv->nlist);
-        max_empty = (int)cfg.get_int("max_empty_result_buckets", 2);
-        ix.s_probe_ids.ensure((size_t)nq * nprobe);
-        ix.s_probe_dis.ensure((size_t)nq * nprobe);
-        iv->coarse_probes(dq, 0, nq, nprobe);
-        sp.probe_ids = ix.s_probe_ids.p;
-        sp.probe_dis = ix.s_probe_dis.p;
-        sp.nprobe = nprobe;
-        sp.list_off = iv->list_off.p;
-        sp.list_len = iv->list_len.p;
-        sp.rows = iv->rows.p;
-        sp.vecs = iv->vecs.p;
-        sp.pq_centroids = iv->pqc.p;
-        sp.M = iv->M;
-        sp.dsub = iv->dsub;
-        sp.codes = (const uint4*)iv->codes.p;
-        sp.npad = iv->npad;
-        sp.t1 = iv->t1.p;
-        rp.kind = iv->is_pq ? (iv->G > 0 ? 1 : 2) : 0;
-        rp.G = iv->G;
-        rp.codes_b = iv->codes.p;
-        sp.nsplit = (nq < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq) : 1;
-        const int np_max = (nprobe + sp.nsplit - 1) / sp.nsplit;
-        smem += (size_t)(np_max + 1) * 4 + (size_t)np_max * 12;
-        if (iv->is_pq) smem += (size_t)iv->M * 1024;
-        KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "range search: m too large");
-    }
-    DevBuf<unsigned long long> cnt;
-    cnt.ensure(1);
-    unsigned long long cap = (unsigned long long)std::max<int64_t>(1 << 20, nq * 256);
-    for (int attempt = 0; attempt < 2 && !graph_hits; attempt++) {
-        hits.ensure(cap);
-        KB2_CUDA_CHECK(cudaMemsetAsync(cnt.p, 0, 8, st));
-        rp.hits = hits.p;
-        rp.count = cnt.p;
-        rp.cap = cap;
-        launch<range_scan_kernel>((unsigned)(nq * sp.nsplit), kScanThreads, smem, st, rp);
-        ix.last.launches++;
-        KB2_CUDA_CHECK(cudaGetLastError());
-        KB2_CUDA_CHECK(cudaMemcpyAsync(&found, cnt.p, 8, cudaMemcpyDeviceToHost, st));
-        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
-        if (found <= cap) break;
-        cap = found;
-    }
-    std::vector<RangeHit> h(found);
-    if (found) KB2_CUDA_CHECK(cudaMemcpy(h.data(), hits.p, found * sizeof(RangeHit), cudaMemcpyDeviceToHost));
-    ix.last.d2h += (int64_t)(found * sizeof(RangeHit));
-    // labels
-    std::vector<int32_t> hrows;
-    std::vector<int64_t> hlabels;
-    const bool custom = fi ? fi->custom_labels : (iv ? iv->custom_labels : hn->custom_labels);
-    if (iv) {
-        hrows.resize(iv->npad);
-        KB2_CUDA_CHECK(cudaMemcpy(hrows.data(), iv->rows.p, iv->npad * 4, cudaMemcpyDeviceToHost));
-    }
-    if (custom) {
-        const int64_t n = ix.count();
-        hlabels.resize(n);
-        if (hn) hlabels = hn->h_labels;
-        else KB2_CUDA_CHECK(cudaMemcpy(hlabels.data(), fi ? fi->labels.p : iv->labels.p, n * 8, cudaMemcpyDeviceToHost));
-    }
+    int nprobe = 0;
+    const std::vector<RangeHit> h = ix.range_hits(rp, cfg, nprobe);
+    const std::vector<int64_t> hlabels = ix.labels.host(ix.count());
     struct Out { int64_t q; int probe; float dist; int64_t label; };
     std::vector<Out> o;
-    o.reserve(found);
-    for (size_t i = 0; i < found; i++) {
-        if (graph_hits) {
-            // pass-0 hits of a query whose BFS queue overflowed are incomplete: the rerun (later entries) has them all
-            if (i < hn->range_pass0_hits && hn->range_overflowed[h[i].q]) continue;
-            if (!in_range_host(h[i].dist, radius, range_filter, has_filter, ix.metric)) continue;
-        }
-        int64_t row = iv ? (int64_t)hrows[h[i].pos] : (int64_t)h[i].pos;
-        o.push_back(Out{h[i].q, h[i].probe, h[i].dist, custom ? hlabels[row] : row});
-    }
-    found = o.size();
+    o.reserve(h.size());
+    for (const RangeHit& e : h) o.push_back(Out{e.q, e.probe, e.dist, hlabels.empty() ? (int64_t)e.pos : hlabels[e.pos]});
+    const size_t found = o.size();
     const bool is_ip = ix.metric == KB2_METRIC_IP;
     std::sort(o.begin(), o.end(), [&](const Out& a, const Out& b) {
         if (a.q != b.q) return a.q < b.q;
@@ -152,7 +55,8 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
     });
     // max_empty_result_buckets: drop hits of probes after `max_empty` consecutive empty probes
     std::vector<char> keep(found, 1);
-    if (iv && max_empty > 0) {
+    const int max_empty = nprobe > 0 ? (int)cfg.get_int("max_empty_result_buckets", 2) : 0;
+    if (max_empty > 0) {
         size_t i = 0;
         std::vector<int> per_probe(nprobe);
         while (i < found) {
