@@ -402,6 +402,7 @@ launch_finalize(IndexBase& ix, FinalizeParams fp, int64_t nq) {
         fp.split_small = 256;
     }
     const size_t smem = (size_t)fp.n_sort * 8 + (size_t)fp.k_sel * 16 + (size_t)fp.d * 4 + 16;
+    KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_INVALID_ARGS, "dimension too large for the exact re-rank");
     unsigned grid = (unsigned)nq;
     if (fp.split_small > 0 && nq > 8 * num_sms()) {   // tail pass: a few CTAs per SM walk the rows, most of which they skip
         grid = 8u * num_sms();
@@ -685,16 +686,27 @@ range_scan(IndexBase& ix, RangeParams rp, size_t smem) {
     return hits_to_host(ix, hits.p, found);
 }
 
-// range_scan of the n rows X, stored in row order (FLAT, HNSW's brute-force case)
+// range_scan of the n rows X, stored in row order (FLAT, HNSW's brute-force case).  A shard's local row r is bitset
+// position shard_lo + r.
 inline std::vector<RangeHit>
 range_scan_rows(IndexBase& ix, RangeParams rp, const float* X, int64_t n) {
     const int64_t nq = rp.sp.nq;
+    const size_t smem = (size_t)ix.dim * 4 + 128;
+    KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "range search: dimension too large for the exact scan");
     rp.kind = 0;
     rp.sp.vecs = X;
     rp.sp.rows = nullptr;
     rp.single_len = n;
+    rp.bit_base = ix.shard_world > 1 ? ix.shard_lo : 0;
     rp.sp.nsplit = (int)std::min<int64_t>(std::max<int64_t>(1, (2 * num_sms() + nq - 1) / nq), std::max<int64_t>(1, n / 1024));
-    return range_scan(ix, rp, (size_t)ix.dim * 4 + 128);
+    return range_scan(ix, rp, smem);
+}
+
+// max_empty_result_buckets (ivf_config.h:51-58): an IVF range search stops after this many consecutive probes that add
+// no hit inside the radius; 0 or less scans every probe
+inline int
+range_max_empty(const JsonObj& cfg) {
+    return (int)cfg.get_int("max_empty_result_buckets", 2);
 }
 
 // ============================================================================================
@@ -812,6 +824,8 @@ struct FlatIndex : IndexBase {
     }
     std::vector<RangeHit>
     range_hits(const RangeParams& rp, const JsonObj&, int&) override {
+        KB2_REQUIRE(!(rp.sp.bitset && shard_world > 1 && n_add_calls > 1), KB2_NOT_IMPLEMENTED,
+                    "FLAT shard: bitset after several add() calls");
         return range_scan_rows(*this, rp, base.p, count());
     }
 };
@@ -2164,7 +2178,9 @@ struct IvfIndex : IndexBase {
         RangeParams rp = list_params(q.sp.queries, nq, nprobe, q.sp.bitset);
         rp.radius = q.radius;
         rp.range_filter = q.range_filter;
-        rp.has_filter = q.has_filter;
+        // with max_empty_result_buckets on, a probe is empty when it adds no hit inside the radius, whatever range_filter
+        // says (faiss range_search_preassigned): the scan emits the radius hits and range_search_index filters after the cut
+        rp.has_filter = range_max_empty(cfg) > 0 ? 0 : q.has_filter;
         rp.sp.nsplit = (nq < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq) : 1;
         const int np_max = (nprobe + rp.sp.nsplit - 1) / rp.sp.nsplit;
         size_t smem = (size_t)dim * 4 + 64 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12;

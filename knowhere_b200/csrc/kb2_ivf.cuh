@@ -574,7 +574,7 @@ struct RangeParams {
     int64_t dense_ld;
     const uint32_t* qlist;
     int64_t q0;
-    int64_t bit_base;    // bitset position of row 0 (FLAT shard); only the dense mode reads it
+    int64_t bit_base;    // bitset position of row 0 when rows are stored in row order (a FLAT or HNSW shard's shard_lo)
     unsigned long long* scanned;   // dense mode, optional: rows scanned
 };
 
@@ -703,7 +703,7 @@ range_scan_kernel(RangeParams rp) {
         } else if (lane < nrows) {
             const uint32_t pos = pos0 + lane;
             bool ok = true;
-            if (p.bitset) ok = !bit_is_set(p.bitset, p.rows ? (int64_t)p.rows[pos] : (int64_t)pos);
+            if (p.bitset) ok = !bit_is_set(p.bitset, p.rows ? (int64_t)p.rows[pos] : rp.bit_base + (int64_t)pos);
             const float dist = (p.metric == KB2_METRIC_L2) ? mykey : -mykey;
             if (ok && in_range(dist, rp.radius, rp.range_filter, rp.has_filter, p.metric)) {
                 const unsigned long long slot = atomicAdd(rp.count, 1ull);

@@ -53,9 +53,10 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
         if (a.dist != b.dist) return is_ip ? a.dist > b.dist : a.dist < b.dist;
         return a.label < b.label;
     });
-    // max_empty_result_buckets: drop hits of probes after `max_empty` consecutive empty probes
+    // max_empty_result_buckets: drop hits of probes after `max_empty` consecutive empty probes.  A probe's hits are then
+    // every hit inside the radius (IvfIndex::range_hits), so range_filter applies here, after the cut.
     std::vector<char> keep(found, 1);
-    const int max_empty = nprobe > 0 ? (int)cfg.get_int("max_empty_result_buckets", 2) : 0;
+    const int max_empty = nprobe > 0 ? range_max_empty(cfg) : 0;
     if (max_empty > 0) {
         size_t i = 0;
         std::vector<int> per_probe(nprobe);
@@ -68,7 +69,8 @@ range_search_index(IndexBase& ix, const float* queries, int64_t nq, float radius
                 run = per_probe[pj] == 0 ? run + 1 : 0;
                 if (run == max_empty) { cut = pj + 1; break; }
             }
-            for (size_t t = i; t < j; t++) keep[t] = o[t].probe < cut;
+            for (size_t t = i; t < j; t++)
+                keep[t] = o[t].probe < cut && in_range_host(o[t].dist, radius, range_filter, has_filter, ix.metric);
             i = j;
         }
     }
