@@ -383,17 +383,6 @@ int kb2_debug_cagra_knn_graph(const float* x, int64_t n, int dim, int metric, co
                               float* out_keys, int* out_iters, int64_t* out_updates, int updates_cap, float* out_ms,
                               int device);
 
-/* validation hook: exact MaxSim scores of (query list, document) pairs, pair_lims [n_lists + 1] (host) giving each
- * list's run of pair_docs (distinct documents, ascending), computed by the emb-list index re-rank kernel
- * (use_rerank = 1, maxsim_rerank_kernel) or by the BruteForce re-rank (use_rerank = 0, maxsim_exact_kernel).  metric:
- * KB2_METRIC_L2 or KB2_METRIC_IP; out_scores[pairs] is the score (the negated key for IP).  queries, base, pair_docs
- * and out_scores are device pointers, the offsets host pointers; a document outside [0, n_docs) is KB2_INVALID_ARGS.
- * out_ms (nullable): device ms of the kernel.  Used by
- * tests to hold the two kernels to the same bits. */
-int kb2_debug_maxsim_pairs(const float* queries, const int64_t* query_lims, int64_t n_lists, const float* base,
-                           const int64_t* base_lims, int64_t n_docs, int dim, int metric, const int64_t* pair_lims,
-                           const int32_t* pair_docs, int use_rerank, float* out_scores, float* out_ms, int device);
-
 #ifdef __cplusplus
 }
 #endif

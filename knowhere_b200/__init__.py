@@ -90,7 +90,6 @@ def _declare(L):
     L.kb2_index_emb_list_offsets.argtypes = [vp, vp, vp]
     L.kb2_index_search_emb_list.argtypes = [vp, vp, vp, i64, i32, c.c_char_p, vp, i64, vp, vp, vp]
     L.kb2_index_emb_list_stage_ms.argtypes = [vp, vp]
-    L.kb2_debug_maxsim_pairs.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, i32, vp, vp, i32]
     L.kb2_index_add_sparse.argtypes = [vp, vp, vp, vp, i64]
     L.kb2_index_search_sparse.argtypes = [vp, vp, vp, vp, i64, i32, c.c_char_p, vp, i64, vp, vp]
     L.kb2_index_range_search_sparse.argtypes = [vp, vp, vp, vp, i64, f32, f32, i32, c.c_char_p, vp, i64,
@@ -604,22 +603,6 @@ def brute_force_search_emb_list(base, base_lims, queries, query_lims, k, metric=
                                             n_lists, k, _ptr(bitset), nbits, _ptr(ids), _ptr(dist), _ptr(st), device,
                                             ctypes.c_void_p(stream)))
     return (ids, dist, st) if stats else (ids, dist)
-
-
-def debug_maxsim_pairs(queries, query_lims, base, base_lims, pair_lims, pair_docs, metric="L2", use_rerank=True,
-                       device=0):
-    """validation hook (kb2_debug_maxsim_pairs): exact MaxSim scores of the (list, document) pairs pair_docs[pair_lims[l]
-    : pair_lims[l+1]] by the index re-rank kernel or the BruteForce one.  queries / base / pair_docs (int32): CUDA
-    tensors; offsets: numpy int64.  Returns (scores CUDA tensor [pairs], kernel ms)."""
-    import torch
-    L = lib()
-    ql, xl, pl = (np.ascontiguousarray(a, np.int64) for a in (query_lims, base_lims, pair_lims))
-    out = torch.empty(max(int(pl[-1]), 1), dtype=torch.float32, device=queries.device)
-    ms = ctypes.c_float()
-    _check(L.kb2_debug_maxsim_pairs(_ptr(queries), _ptr(ql), len(ql) - 1, _ptr(base), _ptr(xl), len(xl) - 1,
-                                    base.shape[1], _METRICS[metric], _ptr(pl), _ptr(pair_docs), 1 if use_rerank else 0,
-                                    _ptr(out), ctypes.byref(ms), device))
-    return out[:int(pl[-1])], ms.value
 
 
 def debug_cagra_knn_graph(x, metric="L2", config=None, device=0):

@@ -882,123 +882,6 @@ kb2_index_emb_list_stage_ms(kb2_index_t h, float* out4) {
     });
 }
 
-namespace {
-__global__ void
-pairs_to_scores_kernel(const uint64_t* e, int64_t n, int metric, float* out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float key = unpack_key(e[i]);
-    out[i] = metric == KB2_METRIC_L2 ? key : -key;
-}
-__global__ void
-pairs_pad_kernel(const int64_t* pl, const int32_t* docs, int64_t n_lists, int64_t K, uint64_t* cand) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_lists * K) return;
-    const int64_t l = i / K, j = i % K;
-    cand[i] = pl[l] + j < pl[l + 1] ? (uint64_t)(uint32_t)docs[pl[l] + j] : kEmpty;
-}
-// documents -> candidate entries; flags[0] = 1 when a document is outside [0, n_docs)
-__global__ void
-pairs_widen_kernel(const int32_t* docs, int64_t n, int64_t n_docs, uint64_t* cand, int* flags) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int32_t d = docs[i];
-    if (d < 0 || d >= n_docs) flags[0] = 1;
-    cand[i] = (uint64_t)(uint32_t)(d < 0 || d >= n_docs ? 0 : d);
-}
-__global__ void
-pairs_unpad_kernel(const int64_t* pl, const uint64_t* in, int64_t n_lists, int64_t K, uint64_t* out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_lists * K) return;
-    const int64_t l = i / K, j = i % K;
-    if (pl[l] + j < pl[l + 1]) out[pl[l] + j] = in[i];
-}
-}  // namespace
-
-int
-kb2_debug_maxsim_pairs(const float* queries, const int64_t* query_lims, int64_t n_lists, const float* base,
-                       const int64_t* base_lims, int64_t n_docs, int dim, int metric, const int64_t* pair_lims,
-                       const int32_t* pair_docs, int use_rerank, float* out_scores, float* out_ms, int device) {
-    return guarded([&] {
-        require_device(device);
-        KB2_REQUIRE(queries && base && pair_docs && out_scores && query_lims && base_lims && pair_lims, KB2_INVALID_ARGS, "null buffer");
-        KB2_REQUIRE(is_device_ptr(queries) && is_device_ptr(base) && is_device_ptr(pair_docs) && is_device_ptr(out_scores),
-                    KB2_INVALID_ARGS, "debug_maxsim_pairs takes device rows, documents and scores");
-        KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP, KB2_INVALID_METRIC_TYPE, "metric must be L2 or IP");
-        KB2_REQUIRE(n_lists >= 1 && n_docs >= 1 && dim > 0, KB2_INVALID_ARGS, "bad sizes");
-        const std::vector<int64_t> ql = read_lims(query_lims, n_lists, "query");
-        const std::vector<int64_t> xl = read_lims(base_lims, n_docs, "base");
-        const std::vector<int64_t> pl = read_lims(pair_lims, n_lists, "pair");
-        const int64_t np = pl.back();
-        int64_t K = 1;
-        for (int64_t l = 0; l < n_lists; l++) K = std::max(K, pl[l + 1] - pl[l]);
-        DevBuf<int64_t> dql, dxl, dpl;
-        DevBuf<uint64_t> cand, out, tmp;
-        DevBuf<msim::RerankItem> items;
-        DevBuf<int32_t> cnt, off;
-        DevBuf<unsigned long long> stats;
-        dql.ensure(ql.size());
-        dxl.ensure(xl.size());
-        dpl.ensure(pl.size());
-        KB2_CUDA_CHECK(cudaMemcpy(dql.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice));
-        KB2_CUDA_CHECK(cudaMemcpy(dxl.p, xl.data(), xl.size() * 8, cudaMemcpyHostToDevice));
-        KB2_CUDA_CHECK(cudaMemcpy(dpl.p, pl.data(), pl.size() * 8, cudaMemcpyHostToDevice));
-        out.ensure(std::max<int64_t>(np, 1));
-        // the documents must be valid before either kernel reads their offsets
-        tmp.ensure(std::max<int64_t>(np, 1));
-        DevBuf<int> flags;
-        flags.ensure(1);
-        KB2_CUDA_CHECK(cudaMemset(flags.p, 0, 4));
-        if (np) pairs_widen_kernel<<<grid1d(np, 256), 256>>>(pair_docs, np, n_docs, tmp.p, flags.p);
-        int bad = 0;
-        KB2_CUDA_CHECK(cudaMemcpy(&bad, flags.p, 4, cudaMemcpyDeviceToHost));
-        KB2_REQUIRE(!bad, KB2_INVALID_ARGS, "pair documents must lie in [0, n_docs)");
-        cudaEvent_t e0, e1;
-        KB2_CUDA_CHECK(cudaEventCreate(&e0));
-        KB2_CUDA_CHECK(cudaEventCreate(&e1));
-        const bool vec4 = (dim & 3) == 0 && (reinterpret_cast<uintptr_t>(queries) & 15) == 0 && (reinterpret_cast<uintptr_t>(base) & 15) == 0;
-        if (use_rerank) {
-            // the candidate CSR is the pair CSR (tmp: documents in the low 32 bits)
-            cnt.ensure(n_lists + 1);
-            off.ensure(n_lists + 1);
-            stats.ensure(2);
-            KB2_CUDA_CHECK(cudaMemset(stats.p, 0, 16));
-            msim::rerank_plan_kernel<<<grid1d(n_lists, 128), 128>>>(dpl.p, tmp.p, dxl.p, dql.p, 0, n_lists, cnt.p, nullptr, nullptr, stats.p);
-            std::vector<int32_t> hcnt(n_lists), hoff(n_lists + 1, 0);
-            KB2_CUDA_CHECK(cudaMemcpy(hcnt.data(), cnt.p, n_lists * 4, cudaMemcpyDeviceToHost));
-            for (int64_t l = 0; l < n_lists; l++) hoff[l + 1] = hoff[l] + hcnt[l];
-            KB2_CUDA_CHECK(cudaMemcpy(off.p, hoff.data(), (n_lists + 1) * 4, cudaMemcpyHostToDevice));
-            items.ensure(std::max<int32_t>(hoff[n_lists], 1));
-            msim::rerank_plan_kernel<<<grid1d(n_lists, 128), 128>>>(dpl.p, tmp.p, dxl.p, dql.p, 0, n_lists, nullptr, off.p, items.p, nullptr);
-            const msim::RerankParams rp{queries, dql.p, base, nullptr, dxl.p, dim, 0, items.p, tmp.p, out.p};
-            KB2_CUDA_CHECK(cudaEventRecord(e0));
-            if (hoff[n_lists] > 0)
-                with_metric(metric, [&](auto m) { msim::launch_rerank<decltype(m)::value>(vec4, (unsigned)hoff[n_lists], 0, rp); });
-            KB2_CUDA_CHECK(cudaEventRecord(e1));
-        } else {
-            cand.ensure((size_t)n_lists * K);
-            pairs_pad_kernel<<<grid1d(n_lists * K, 256), 256>>>(dpl.p, pair_docs, n_lists, K, cand.p);
-            tmp.ensure((size_t)n_lists * K);
-            msim::ExactParams ep{queries, dql.p, base, dxl.p, dim, nullptr, 0, nullptr, cand.p, tmp.p, nullptr, 0, K, n_lists * K};
-            KB2_CUDA_CHECK(cudaEventRecord(e0));
-            with_metric(metric, [&](auto m) {
-                if (vec4) msim::maxsim_exact_kernel<decltype(m)::value, true><<<(unsigned)((ep.npairs + 7) / 8), 256>>>(ep);
-                else msim::maxsim_exact_kernel<decltype(m)::value, false><<<(unsigned)((ep.npairs + 7) / 8), 256>>>(ep);
-            });
-            KB2_CUDA_CHECK(cudaEventRecord(e1));
-            pairs_unpad_kernel<<<grid1d(n_lists * K, 256), 256>>>(dpl.p, tmp.p, n_lists, K, out.p);
-        }
-        KB2_CUDA_CHECK(cudaGetLastError());
-        if (np) pairs_to_scores_kernel<<<grid1d(np, 256), 256>>>(out.p, np, metric, out_scores);
-        KB2_CUDA_CHECK(cudaDeviceSynchronize());
-        float ms = 0.f;
-        KB2_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-        cudaEventDestroy(e0);
-        cudaEventDestroy(e1);
-        if (out_ms) *out_ms = ms;
-    });
-}
-
 // ---------------------------------------------------------------- multi-GPU: NCCL communicator behind the ABI
 int
 kb2_comm_unique_id(uint8_t* out128) {

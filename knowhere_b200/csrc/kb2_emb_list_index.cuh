@@ -10,8 +10,8 @@
 //      HNSW checks ef >= k against the list-level k and searches with max(ef, vec_topk);
 //   2. candidates: cand_keys_kernel maps each stage-1 id to (list << 32) | document, one radix sort and one unique pass
 //      compact them, and cand_off_kernel finds each list's run: a CSR of distinct documents per list, ascending;
-//   3. re-rank: rerank_plan_kernel packs each list's candidates into work items and msim::maxsim_rerank_kernel computes
-//      their exact MaxSim keys, bit-identical to the BruteForce re-rank (kb2_maxsim.cuh);
+//   3. re-rank: msim::rerank (kb2_maxsim.cuh), the BruteForce re-rank, packs each list's candidates into work items and
+//      computes their exact MaxSim keys with msim::maxsim_rerank_kernel;
 //   4. select: a segmented radix sort orders each list's (key, document) entries and el_emit_kernel writes the k best,
 //      padded with id -1 and -FLT_MAX (larger is better) or FLT_MAX (MAX_SIM_L2), as emb_list_strategy.cc:111-114.
 // Ties in the score are ordered by ascending document id (the reference's order follows unordered_set iteration).
@@ -35,9 +35,9 @@ struct EmbListState {
     // per-search scratch (grow-only)
     DevBuf<float> q, s1_dist;
     DevBuf<int64_t> qlims, s1_ids, cand_off;
-    DevBuf<int32_t> row_list, item_cnt, item_off;
+    DevBuf<int32_t> row_list;
     DevBuf<uint64_t> keys, keys_sorted, cand, cand_key, cand_sorted;
-    DevBuf<msim::RerankItem> items;
+    msim::RerankScratch rr;
     DevBuf<uint8_t> doc_bits, row_bits, tmp;
     DevBuf<unsigned long long> counters;   // [0] candidate pairs, [1] token x row distances, [2] unique count
     cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -212,7 +212,6 @@ search_emb_list(IndexBase& ix, const float* queries, const std::vector<int64_t>&
     const auto [X, pos] = ix.emb_list_rows();
     const bool vec4 = (d & 3) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
     KB2_CUDA_CHECK(cudaMemsetAsync(el.counters.p, 0, 2 * sizeof(unsigned long long), st));
-    unsigned long long* hc = (unsigned long long*)ix.h_counter.p + 12;   // [0] items, [1] candidates
 
     for (int64_t l0 = 0; l0 < n_lists;) {
         // whole lists, stage-1 entries within the scratch budget (at least one list)
@@ -248,37 +247,13 @@ search_emb_list(IndexBase& ix, const float* queries, const std::vector<int64_t>&
             b2 = el.tmp.n;
             KB2_CUDA_CHECK(cub::DeviceSelect::Unique(el.tmp.p, b2, el.keys_sorted.p, el.cand.p, el.counters.p + 2, (int)ne, st));
             cand_off_kernel<<<grid1d(L + 1, 256), 256, 0, st>>>(el.cand.p, el.counters.p + 2, L, el.cand_off.p);
-            // items of every list
-            el.item_cnt.ensure(L + 1);
-            el.item_off.ensure(L + 1);
-            KB2_CUDA_CHECK(cudaMemsetAsync(el.item_cnt.p + L, 0, 4, st));
-            msim::rerank_plan_kernel<<<grid1d(L, 128), 128, 0, st>>>(el.cand_off.p, el.cand.p, el.d_lims.p, el.qlims.p, l0, L,
-                                                                     el.item_cnt.p, nullptr, nullptr, el.counters.p);
-            size_t b3 = 0;
-            cub::DeviceScan::ExclusiveSum(nullptr, b3, el.item_cnt.p, el.item_off.p, (int)(L + 1), st);
-            el.tmp.ensure(b3);
-            b3 = el.tmp.n;
-            KB2_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(el.tmp.p, b3, el.item_cnt.p, el.item_off.p, (int)(L + 1), st));
-            KB2_CUDA_CHECK(cudaMemcpyAsync(hc, el.item_off.p + L, 4, cudaMemcpyDeviceToHost, st));
-            KB2_CUDA_CHECK(cudaMemcpyAsync(hc + 1, el.cand_off.p + L, 8, cudaMemcpyDeviceToHost, st));
-            KB2_CUDA_CHECK(cudaStreamSynchronize(st));
-            const int64_t nitems = (int64_t)*(const int32_t*)hc;
-            nu = (int64_t)hc[1];
-            el.items.ensure(std::max<int64_t>(nitems, 1));
-            msim::rerank_plan_kernel<<<grid1d(L, 128), 128, 0, st>>>(el.cand_off.p, el.cand.p, el.d_lims.p, el.qlims.p, l0, L,
-                                                                     nullptr, el.item_off.p, el.items.p, nullptr);
-            KB2_CUDA_CHECK(cudaGetLastError());
-            if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[2], st));
-            // 3. exact keys of every candidate
-            el.cand_key.ensure(std::max<int64_t>(nu, 1));
-            el.cand_sorted.ensure(std::max<int64_t>(nu, 1));
-            if (nitems > 0) {
-                const msim::RerankParams rp{dq, el.qlims.p, X, pos, el.d_lims.p, d, l0, el.items.p, el.cand.p, el.cand_key.p};
-                with_metric(ix.metric, [&](auto m) { msim::launch_rerank<decltype(m)::value>(vec4, (unsigned)nitems, st, rp); });
-                KB2_CUDA_CHECK(cudaGetLastError());
-            }
+            // 3. exact keys of every candidate (the plan ends the candidates stage and adds to counters[0..1])
+            const msim::RerankParams rp{dq, el.qlims.p, X, pos, el.d_lims.p, d, l0, nullptr, el.cand.p, nullptr};
+            nu = msim::rerank(ix, ix.metric, vec4, rp, el.cand_off.p, nullptr, L, el.cand_key, el.rr, el.counters.p,
+                              ix.timing ? el.ev[2] : nullptr);
             if (ix.timing) KB2_CUDA_CHECK(cudaEventRecord(el.ev[3], st));
             // 4. each list's candidates in (key, document) order
+            el.cand_sorted.ensure(std::max<int64_t>(nu, 1));
             if (nu > 0) {
                 size_t b4 = 0;
                 cub::DeviceSegmentedRadixSort::SortKeys(nullptr, b4, el.cand_key.p, el.cand_sorted.p, (int)nu, (int)L,
@@ -311,6 +286,7 @@ search_emb_list(IndexBase& ix, const float* queries, const std::vector<int64_t>&
         }
         l0 = l1;
     }
+    unsigned long long* hc = (unsigned long long*)ix.h_counter.p + 12;
     KB2_CUDA_CHECK(cudaMemcpyAsync(hc, el.counters.p, 16, cudaMemcpyDeviceToHost, st));
     ix.results_out(n_lists, k, out_ids, out_dist, d_ids, d_dist);
     stats[0] = n_lists;

@@ -270,10 +270,11 @@ large_emit_kernel(FinalizeParams p, LargeFin lf, int64_t rows) {
     }
 }
 
+template <typename T>
 __global__ void
-segment_offsets_kernel(int32_t* off, int64_t nseg, int len) {
+segment_offsets_kernel(T* off, int64_t nseg, int64_t len) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t <= nseg) off[t] = (int32_t)(t * len);
+    if (t <= nseg) off[t] = (T)(t * len);
 }
 
 }  // namespace kb2

@@ -12,11 +12,13 @@
 //      M and base tokens on N; its epilogue takes each query token's extremum over every document of the base tile and sums
 //      them over the tokens of each query list.  It writes one approximate key per (query list, document) to S, never the
 //      token-by-token distances.
-//   2. select_rows_kernel keeps the K = k + 16 best of each S row; maxsim_exact_kernel recomputes their keys in fp32 on the
-//      CUDA cores in a fixed order; a segmented radix sort orders them by (key, document); maxsim_emit_kernel writes the k
-//      best and certifies the list against the filter's error bound (maxsim_bound).
-//   3. Lists that could not be certified are redone with exact keys for every document (maxsim_exact_kernel over all
-//      documents), selected and emitted again.  dim % 4 != 0 (no TMA) takes that exact all-documents path for every list.
+//   2. select_rows_kernel keeps the K = k + 16 best of each S row; rerank() recomputes their keys in fp32 on the CUDA
+//      cores in a fixed order (maxsim_rerank_kernel); a segmented radix sort orders them by (key, document);
+//      maxsim_emit_kernel writes the k best and certifies the list against the filter's error bound (maxsim_bound).
+//   3. Lists that could not be certified are redone with exact keys for every document (rerank() with every unfiltered
+//      document as a candidate), selected and emitted again.  dim % 4 != 0 (no TMA) takes that exact all-documents path
+//      for every list.
+// The index-level emb-list search (kb2_emb_list_index.cuh) re-ranks its gathered candidates through the same rerank().
 #pragma once
 #include "kb2_index.cuh"
 
@@ -236,109 +238,11 @@ maxsim_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     }
 }
 
-// Exact key of (query list, document) pairs in fp32 on the CUDA cores, in the order of get_sum_max_sim: for each query
-// token in order, the extremum over the document's vectors in order (each distance an fmaf chain over the dimensions in
-// order), summed over the tokens in order.  One warp per pair; lane l owns tokens l, l + 32, ...
-//   candidates mode (cand != nullptr): pair (b, j) is the document of entry j of candidate row b (kEmpty stays kEmpty);
-//     out_cand[b][j] = (exact key, document).
-//   all-documents mode: pair (b, j) is document j; out_all[b][j] = exact key, +inf for an empty or filtered document.
-// Row b is query list qlist[b], or l0 + b.  grid = ceil(rows * per_row / 8), block 256.
-struct ExactParams {
-    const float* Q;
-    const int64_t* qlims;
-    const float* X;
-    const int64_t* xlims;
-    int d;
-    const uint8_t* bitset;
-    int64_t l0;
-    const uint32_t* qlist;
-    const uint64_t* cand;
-    uint64_t* out_cand;
-    float* out_all;
-    int64_t lda;
-    int64_t per_row;   // K (candidates) or n_docs (all documents)
-    int64_t npairs;
-};
-
-template <int METRIC, bool VEC4>
-__global__ void __launch_bounds__(256)
-maxsim_exact_kernel(const ExactParams p) {
-    const int lane = threadIdx.x & 31;
-    const int64_t pair = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (pair >= p.npairs) return;
-    const int64_t b = pair / p.per_row, j = pair % p.per_row;
-    const int64_t lst = p.qlist ? (int64_t)p.qlist[b] : p.l0 + b;
-    int64_t doc = j;
-    if (p.cand) {
-        const uint64_t e = p.cand[b * p.per_row + j];
-        if (e == kEmpty) {
-            if (lane == 0) p.out_cand[b * p.per_row + j] = kEmpty;
-            return;
-        }
-        doc = unpack_pos(e);
-    }
-    const int64_t qa = p.qlims[lst], qe = p.qlims[lst + 1];
-    const int64_t xa = p.xlims[doc], xe = p.xlims[doc + 1];
-    float total = INFINITY;
-    if (qa < qe && xa < xe && !(p.bitset && bit_is_set(p.bitset, doc))) {
-        total = 0.f;
-        for (int64_t t0 = qa; t0 < qe; t0 += kWarp) {
-            const int64_t tq = t0 + lane;
-            float ext = INFINITY;
-            if (tq < qe) {
-                const float* q = p.Q + tq * p.d;
-                for (int64_t x = xa; x < xe; x++) {
-                    const float* xr = p.X + x * p.d;
-                    float acc = 0.f;
-                    if (VEC4) {
-                        const float4* q4 = reinterpret_cast<const float4*>(q);
-                        const float4* x4 = reinterpret_cast<const float4*>(xr);
-                        for (int i = 0; i < (p.d >> 2); i++) {
-                            const float4 qv = __ldg(q4 + i), xv = __ldg(x4 + i);
-                            if (METRIC == KB2_METRIC_L2) {
-                                float df;
-                                df = qv.x - xv.x; acc = fmaf(df, df, acc);
-                                df = qv.y - xv.y; acc = fmaf(df, df, acc);
-                                df = qv.z - xv.z; acc = fmaf(df, df, acc);
-                                df = qv.w - xv.w; acc = fmaf(df, df, acc);
-                            } else {
-                                acc = fmaf(qv.x, xv.x, acc);
-                                acc = fmaf(qv.y, xv.y, acc);
-                                acc = fmaf(qv.z, xv.z, acc);
-                                acc = fmaf(qv.w, xv.w, acc);
-                            }
-                        }
-                    } else {
-                        for (int i = 0; i < p.d; i++) {
-                            const float qv = __ldg(q + i), xv = __ldg(xr + i);
-                            if (METRIC == KB2_METRIC_L2) {
-                                const float df = qv - xv;
-                                acc = fmaf(df, df, acc);
-                            } else {
-                                acc = fmaf(qv, xv, acc);
-                            }
-                        }
-                    }
-                    ext = fminf(ext, (METRIC == KB2_METRIC_L2) ? acc : -acc);
-                }
-            }
-#pragma unroll
-            for (int l = 0; l < kWarp; l++) {
-                const float v = __shfl_sync(0xffffffffu, ext, l);
-                if (t0 + l < qe) total += v;
-            }
-        }
-    }
-    if (lane != 0) return;
-    if (p.cand) p.out_cand[b * p.per_row + j] = pack_kp(total, (uint32_t)doc);
-    else p.out_all[b * p.lda + j] = total;
-}
-
 // Error bound of the filter's key of list Q against any document, from its tokens' norms and M^2 = max |x|^2 over the
 // base (DESIGN §4.10):  E = sum_t rel(d) a_t + |Q| 2^-22 sum_t a_t,  a_t = |q_t| M (IP, COSINE) or |q_t|^2 + M^2 (L2).
 // rel(d) = fin_cert_rel(d) bounds one approximate distance against its exact value as for FLAT (kb2_topk.cuh); the
 // extremum over a document is then off by at most the same, and the second term covers the fp32 sums over the tokens
-// (filter and exact kernel both: each extremum is at most 2 a_t in magnitude).
+// (filter and re-rank both: each extremum is at most 2 a_t in magnitude).
 __device__ __forceinline__ float
 maxsim_bound(float sum_a, int64_t ntok, int d) {
     return fin_cert_rel(d) * sum_a + (float)ntok * 0x1p-22f * sum_a;
@@ -415,15 +319,6 @@ maxsim_emit_kernel(const EmitParams p) {
     p.cert[2 + atomicAdd(p.cert + 1, 1u)] = (uint32_t)lst;
 }
 
-// Scratch of one emb-list search, reused across calls (per-device BruteForce slot).
-struct Scratch {
-    DevBuf<int64_t> xlims, qlims;
-    DevBuf<int32_t> row_list, seg_off;
-    DevBuf<Item> items;
-    DevBuf<uint64_t> cand, exact, sorted;
-    DevBuf<uint8_t> bits, sort_tmp;
-};
-
 // Work items from the base offsets: consecutive documents packed greedily into one 128-row tile (at most MAXD of them),
 // and each document longer than a tile alone over consecutive tiles.  Empty documents are never scored.
 inline std::vector<Item>
@@ -458,137 +353,19 @@ plan_items(const std::vector<int64_t>& xl) {
     return items;
 }
 
-// The search.  fi holds the base (fi.base, fi.norms = |x|^2, rows normalised for COSINE) and the stream; dq: device query
-// rows (normalised for COSINE); xl / ql: validated host offsets; dbits: device bitset over documents or nullptr; d_ids /
-// d_dist: device [n_lists][k].  metric: KB2_METRIC_L2 or KB2_METRIC_IP.  stats: lists, candidate slots re-ranked, lists
-// scored exactly over all documents.
-inline void
-search(FlatIndex& fi, Scratch& sc, const float* dq, const std::vector<int64_t>& xl, const std::vector<int64_t>& ql, int d,
-       int metric, int k, const uint8_t* dbits, int64_t* d_ids, float* d_dist, int64_t stats[3]) {
-    cudaStream_t st = fi.stream;
-    const int64_t n_docs = (int64_t)xl.size() - 1, n_lists = (int64_t)ql.size() - 1;
-    const int64_t nb = xl.back(), nq_rows = ql.back();
-    const float* X = fi.base.p;
-    const float* xn = fi.norms.p;
-    sc.xlims.ensure(xl.size());
-    sc.qlims.ensure(ql.size());
-    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.xlims.p, xl.data(), xl.size() * 8, cudaMemcpyHostToDevice, st));
-    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.qlims.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice, st));
-    std::vector<int32_t> row_list((size_t)std::max<int64_t>(nq_rows, 1));
-    for (int64_t l = 0; l < n_lists; l++)
-        for (int64_t r = ql[l]; r < ql[l + 1]; r++) row_list[r] = (int32_t)l;
-    sc.row_list.ensure(row_list.size());
-    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.row_list.p, row_list.data(), row_list.size() * 4, cudaMemcpyHostToDevice, st));
-    fi.s_qn.ensure(std::max<int64_t>(nq_rows, 1));
-    if (metric == KB2_METRIC_L2 && nq_rows > 0)
-        row_norms_kernel<<<grid1d(nq_rows * 32, 256), 256, 0, st>>>(dq, nq_rows, d, fi.s_qn.p);
-    fi.s_cert.ensure((size_t)n_lists + 2);
-    KB2_CUDA_CHECK(cudaMemsetAsync(fi.s_cert.p, 0, 8, st));
-    pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, st>>>(xn, nb, fi.s_cert.p);
-
-    CUtensorMap tq, tx;
-    const bool use_tc = nq_rows > 0 && tc::make_tmap(&tq, dq, nq_rows, d) && tc::make_tmap(&tx, X, nb, d);
-    std::vector<Item> items;
-    if (use_tc) {
-        items = plan_items(xl);
-        sc.items.ensure(std::max<size_t>(items.size(), 1));
-        if (!items.empty())
-            KB2_CUDA_CHECK(cudaMemcpyAsync(sc.items.p, items.data(), items.size() * sizeof(Item), cudaMemcpyHostToDevice, st));
-    }
-    const int K = k + 16;
-    const int64_t lds = round_up(n_docs, 4);
-    // lists per chunk: S within the 256 MB key budget of dense_candidates, candidates within the large-k scratch
-    const int64_t L = std::max<int64_t>(1, std::min<int64_t>({n_lists, (64ll << 20) / lds, large_k_group(n_lists, (int64_t)K * 24 + 16)}));
-    fi.s_keys.ensure((size_t)L * lds);
-    sc.cand.ensure((size_t)L * K);
-    sc.exact.ensure((size_t)L * K);
-    sc.sorted.ensure((size_t)L * K);
-    sc.seg_off.ensure((size_t)L + 1);
-    segment_offsets_kernel<<<grid1d(L + 1, 256), 256, 0, st>>>(sc.seg_off.p, L, K);
-    size_t tmp_bytes = 0;
-    cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, sc.exact.p, sc.sorted.p, (int)(L * K), (int)L, sc.seg_off.p,
-                                            sc.seg_off.p + 1, 0, 64, st);
-    sc.sort_tmp.ensure(tmp_bytes);
-    const bool vec4 = (d & 3) == 0 && (reinterpret_cast<uintptr_t>(dq) & 15) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
-
-    auto exact = [&](const uint64_t* cand, int64_t rows, int64_t l0, const uint32_t* qlist) {
-        ExactParams ep{dq, sc.qlims.p, X, sc.xlims.p, d, dbits, l0, qlist, cand, sc.exact.p, fi.s_keys.p, lds,
-                       cand ? (int64_t)K : n_docs, 0};
-        ep.npairs = rows * ep.per_row;
-        if (ep.npairs == 0) return;
-        const unsigned grid = (unsigned)((ep.npairs + 7) / 8);
-        with_metric(metric, [&](auto m) {
-            if (vec4) maxsim_exact_kernel<decltype(m)::value, true><<<grid, 256, 0, st>>>(ep);
-            else maxsim_exact_kernel<decltype(m)::value, false><<<grid, 256, 0, st>>>(ep);
-        });
-        fi.last.launches++;
-        KB2_CUDA_CHECK(cudaGetLastError());
-    };
-    // sort the K entries of each row by (key, document) and emit the rows
-    auto sort_emit = [&](const uint64_t* in, int64_t rows, int64_t l0, const uint32_t* qlist, const uint64_t* approx) {
-        size_t bytes = tmp_bytes;
-        KB2_CUDA_CHECK(cub::DeviceSegmentedRadixSort::SortKeys(sc.sort_tmp.p, bytes, in, sc.sorted.p, (int)(rows * K), (int)rows,
-                                                               sc.seg_off.p, sc.seg_off.p + 1, 0, 64, st));
-        EmitParams pp{sc.sorted.p, approx, K, k, dq, sc.qlims.p, d, fi.s_cert.p, l0, qlist, d_ids, d_dist};
-        with_metric(metric, [&](auto m) { maxsim_emit_kernel<decltype(m)::value><<<(unsigned)rows, 256, 0, st>>>(pp); });
-        fi.last.launches += 2;
-        KB2_CUDA_CHECK(cudaGetLastError());
-    };
-    // exact keys of every document for `rows` lists -> their K best -> sorted, emitted
-    auto exact_all = [&](int64_t rows, int64_t l0, const uint32_t* qlist) {
-        exact(nullptr, rows, l0, qlist);
-        large_k_select<float>(fi, fi.s_keys.p, lds, n_docs, 0u, K, sc.cand.p, K, rows);
-        sort_emit(sc.cand.p, rows, l0, qlist, nullptr);
-    };
-
-    int64_t n_exact = 0;
-    for (int64_t l0 = 0; l0 < n_lists; l0 += L) {
-        const int64_t rows = std::min(L, n_lists - l0);
-        if (!use_tc) {
-            exact_all(rows, l0, nullptr);
-            n_exact += rows;
-            continue;
-        }
-        pqtc::fill_f32_kernel<<<grid1d(rows * lds, 256), 256, 0, st>>>(fi.s_keys.p, rows * lds, INFINITY);
-        FilterParams fp{sc.items.p, (int)items.size(), sc.xlims.p, sc.qlims.p, sc.row_list.p, fi.s_qn.p, xn,
-                        ql[l0], ql[l0 + rows], l0, d, dbits, fi.s_keys.p, lds};
-        if (fp.r1 > fp.r0 && fp.nitems > 0) {
-            const unsigned grid = (unsigned)std::min<int64_t>(num_sms(), fp.nitems);
-            with_metric(metric, [&](auto m) {
-                launch<maxsim_filter_kernel<decltype(m)::value>>(grid, tc::THREADS, SMEM_BYTES, st, tq, tx, fp);
-            });
-            fi.last.launches++;
-            KB2_CUDA_CHECK(cudaGetLastError());
-        }
-        large_k_select<float>(fi, fi.s_keys.p, lds, n_docs, 0u, K, sc.cand.p, K, rows);
-        exact(sc.cand.p, rows, l0, nullptr);
-        sort_emit(sc.exact.p, rows, l0, nullptr, sc.cand.p);
-        stats[1] += rows * K;
-    }
-    int64_t nredo = 0;
-    if (use_tc && n_lists > 0) {
-        uint32_t* hc = (uint32_t*)fi.h_counter.p;
-        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, fi.s_cert.p + 1, 4, cudaMemcpyDeviceToHost, st));
-        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
-        nredo = hc[0];
-        for (int64_t r0 = 0; r0 < nredo; r0 += L) exact_all(std::min(L, nredo - r0), 0, fi.s_cert.p + 2 + r0);
-    }
-    stats[0] += n_lists;
-    stats[2] += n_exact + nredo;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
-// Exact re-rank of gathered candidates (index-level emb-list search, kb2_emb_list_index.cuh; DESIGN §4.11).
+// Exact re-rank of (query list, document) candidates: the BruteForce candidates and all-documents rows (search() below)
+// and the index-level emb-list search (kb2_emb_list_index.cuh; DESIGN §4.10, §4.11).
 //
 // A work item is one query list and a run of its candidate documents: up to RR_MAXD whole documents of at most RR_TR
 // rows in all, or one longer document alone.  One CTA per item.  The list's tokens are taken RR_TQ at a time; for each
 // token block the item's rows are taken RR_TR at a time, and the (token x row) block is contracted like an SGEMM over
 // RR_DK-dimension stages (cp.async 16-byte copies into a double-buffered shared tile when rows are float4-aligned).
-// Each thread owns a 4 x 4 (token x row) register tile and runs every one of its distances as the fmaf chain over
-// dimensions 0..d-1 of maxsim_exact_kernel, so each distance has the same bits; the per-(token, document) extremum is
-// order-free (fminf over the same values), and after each token block one thread per document adds the block's extrema
-// to its running sum in token order, as maxsim_exact_kernel does.  The scores are therefore bit-identical to the
-// BruteForce re-rank.  Rows are read in place (HNSW) or at pos[row] (IVF_FLAT's list-order store).
+// Each thread owns a 4 x 4 (token x row) register tile and runs every one of its distances as one fmaf chain over
+// dimensions 0..d-1 in order (get_sum_max_sim's order); the per-(token, document) extremum is order-free (fminf over the
+// same values), and after each token block one thread per document adds the block's extrema to its running sum in token
+// order.  A score therefore does not depend on how the candidates are packed into items.  Rows are read in place
+// (BruteForce, HNSW) or at pos[row] (IVF_FLAT's list-order store).
 constexpr int RR_TQ = 32;
 constexpr int RR_TR = 128;
 constexpr int RR_DK = 32;
@@ -771,7 +548,7 @@ maxsim_rerank_kernel(const RerankParams p) {
         }
         __syncthreads();
     }
-    // an empty query list or document scores +inf, as in maxsim_exact_kernel
+    // an empty query list or document scores +inf, which no selection keeps
     if (t < it.ndocs)
         p.out[it.c0 + t] = pack_kp(qe > qa && sBeg[t + 1] > sBeg[t] ? sT[t] : INFINITY, (uint32_t)p.cand[it.c0 + t]);
 }
@@ -783,20 +560,33 @@ launch_rerank(bool vec4, unsigned nitems, cudaStream_t st, const RerankParams& r
     else launch<maxsim_rerank_kernel<METRIC, false>>(nitems, RR_THREADS, RR_SMEM, st, rp);
 }
 
-// Items of the candidates of each list (cand_off: [lists + 1] CSR over the candidates, each list's documents in
-// ascending order).  One thread per list packs its documents greedily: consecutive documents while they hold at most
-// RR_TR rows and RR_MAXD documents, a longer document alone.  Pass 1 (items == nullptr) counts each list's items into
-// cnt[l] and adds the list's (document, |Q| x |D|) totals to stats[0..1]; pass 2 writes them at off[l].
+// Items of the candidates of each list.  Row b's candidates are cand[cand_off[b] .. cand_off[b + 1]): documents in the
+// low 32 bits, then possibly kEmpty padding, which is skipped (select_rows_kernel's rows).  Its query list is qlist[b],
+// or l0 + b.  One thread per row packs the documents greedily: consecutive documents while they hold at most RR_TR rows and RR_MAXD documents, a longer document
+// alone.  Pass 1 (items == nullptr) counts each row's items into cnt[b] and, with stats, adds the row's (candidate,
+// |Q| x |D|) totals to stats[0..1]; pass 2 writes them at off[b].
 __global__ void
 rerank_plan_kernel(const int64_t* cand_off, const uint64_t* cand, const int64_t* xlims, const int64_t* qlims, int64_t l0,
-                   int64_t nlists, int32_t* cnt, const int32_t* off, RerankItem* items, unsigned long long* stats) {
+                   const uint32_t* qlist, int64_t nlists, int32_t* cnt, const int32_t* off, RerankItem* items,
+                   unsigned long long* stats) {
     const int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (l >= nlists) return;
-    const int64_t c0 = cand_off[l], c1 = cand_off[l + 1];
+    const int64_t lst = qlist ? (int64_t)qlist[l] : l0 + l;
+    const int64_t c0 = cand_off[l];
+    int64_t c1 = cand_off[l + 1];
+    if (c1 > c0 && cand[c1 - 1] == kEmpty) {   // the padding starts at the first kEmpty: cut it off before the walk
+        int64_t lo = c0, hi = c1 - 1;
+        while (lo < hi) {
+            const int64_t m = (lo + hi) >> 1;
+            if (cand[m] == kEmpty) hi = m;
+            else lo = m + 1;
+        }
+        c1 = lo;
+    }
     int n = 0;
     int64_t o = items ? off[l] : 0;
     unsigned long long rows_all = 0;
-    RerankItem cur{(int32_t)l, 0, 0, 0};
+    RerankItem cur{(int32_t)(lst - l0), 0, 0, 0};
     auto close = [&] {
         if (cur.ndocs == 0) return;
         if (items) items[o++] = cur;
@@ -819,11 +609,217 @@ rerank_plan_kernel(const int64_t* cand_off, const uint64_t* cand, const int64_t*
     close();
     if (!items) {
         cnt[l] = n;
-        if (c1 > c0) {
+        if (stats && c1 > c0) {
             atomicAdd(stats, (unsigned long long)(c1 - c0));
-            atomicAdd(stats + 1, rows_all * (unsigned long long)(qlims[l0 + l + 1] - qlims[l0 + l]));
+            atomicAdd(stats + 1, rows_all * (unsigned long long)(qlims[lst + 1] - qlims[lst]));
         }
     }
+}
+
+// Grow-only scratch of rerank().
+struct RerankScratch {
+    DevBuf<int32_t> cnt, off;
+    DevBuf<RerankItem> items;
+    DevBuf<uint8_t> tmp;
+};
+
+// Exact keys of the candidates of L rows (rerank_plan_kernel's rows: cand = rp.cand, list qlist[b] or rp.l0 + b):
+// out[c] = pack_kp(exact key, document) for every entry c that is not kEmpty padding; the padding's slots are not
+// written.  The plan's count pass, a cub::DeviceScan of the counts, one read-back of the item and candidate counts (the
+// stream's only synchronisation here), the write pass and maxsim_rerank_kernel.  out is grown to the candidate count
+// cand_off[L], which is returned.  stats: as rerank_plan_kernel's, or nullptr; `planned`, when given, is recorded
+// between the plan and the re-rank.
+inline int64_t
+rerank(IndexBase& ix, int metric, bool vec4, RerankParams rp, const int64_t* cand_off, const uint32_t* qlist, int64_t L,
+       DevBuf<uint64_t>& out, RerankScratch& rs, unsigned long long* stats, cudaEvent_t planned = nullptr) {
+    cudaStream_t st = ix.stream;
+    rs.cnt.ensure(L + 1);
+    rs.off.ensure(L + 1);
+    KB2_CUDA_CHECK(cudaMemsetAsync(rs.cnt.p + L, 0, 4, st));
+    rerank_plan_kernel<<<grid1d(L, 128), 128, 0, st>>>(cand_off, rp.cand, rp.xlims, rp.qlims, rp.l0, qlist, L, rs.cnt.p,
+                                                        nullptr, nullptr, stats);
+    size_t bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, bytes, rs.cnt.p, rs.off.p, (int)(L + 1), st);
+    rs.tmp.ensure(bytes);
+    bytes = rs.tmp.n;
+    KB2_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(rs.tmp.p, bytes, rs.cnt.p, rs.off.p, (int)(L + 1), st));
+    unsigned long long* hc = (unsigned long long*)ix.h_counter.p + 12;   // [0] items (int32), [1] candidates
+    KB2_CUDA_CHECK(cudaMemcpyAsync(hc, rs.off.p + L, 4, cudaMemcpyDeviceToHost, st));
+    KB2_CUDA_CHECK(cudaMemcpyAsync(hc + 1, cand_off + L, 8, cudaMemcpyDeviceToHost, st));
+    KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+    const int64_t nitems = (int64_t)*(const int32_t*)hc, ncand = (int64_t)hc[1];
+    rs.items.ensure(std::max<int64_t>(nitems, 1));
+    out.ensure(std::max<int64_t>(ncand, 1));
+    rerank_plan_kernel<<<grid1d(L, 128), 128, 0, st>>>(cand_off, rp.cand, rp.xlims, rp.qlims, rp.l0, qlist, L, nullptr,
+                                                        rs.off.p, rs.items.p, nullptr);
+    KB2_CUDA_CHECK(cudaGetLastError());
+    if (planned) KB2_CUDA_CHECK(cudaEventRecord(planned, st));
+    if (nitems > 0) {
+        rp.items = rs.items.p;
+        rp.out = out.p;
+        with_metric(metric, [&](auto m) { launch_rerank<decltype(m)::value>(vec4, (unsigned)nitems, st, rp); });
+        KB2_CUDA_CHECK(cudaGetLastError());
+    }
+    return ncand;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The BruteForce search.
+
+// Scratch of one emb-list search, reused across calls (per-device BruteForce slot).
+struct Scratch {
+    DevBuf<int64_t> xlims, qlims, seg_off, doc_off;
+    DevBuf<int32_t> row_list;
+    DevBuf<uint32_t> kept;
+    DevBuf<Item> items;
+    DevBuf<uint64_t> cand, exact, sorted;
+    DevBuf<uint8_t> bits, sort_tmp;
+    RerankScratch rr;
+};
+
+// n entries of the all-documents mode's candidate rows: each row holds the n_kept documents kept[0 .. n_kept)
+__global__ void
+all_docs_kernel(const uint32_t* kept, int64_t n_kept, int64_t n, uint64_t* cand) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) cand[i] = kept[i % n_kept];
+}
+
+// fi holds the base (fi.base, fi.norms = |x|^2, rows normalised for COSINE) and the stream; dq: device query rows
+// (normalised for COSINE); xl / ql: validated host offsets; dbits: device bitset over documents or nullptr; d_ids /
+// d_dist: device [n_lists][k].  metric: KB2_METRIC_L2 or KB2_METRIC_IP.  stats: lists, candidate slots re-ranked, lists
+// scored exactly over all documents.
+inline void
+search(FlatIndex& fi, Scratch& sc, const float* dq, const std::vector<int64_t>& xl, const std::vector<int64_t>& ql, int d,
+       int metric, int k, const uint8_t* dbits, int64_t* d_ids, float* d_dist, int64_t stats[3]) {
+    cudaStream_t st = fi.stream;
+    const int64_t n_docs = (int64_t)xl.size() - 1, n_lists = (int64_t)ql.size() - 1;
+    const int64_t nb = xl.back(), nq_rows = ql.back();
+    const float* X = fi.base.p;
+    const float* xn = fi.norms.p;
+    sc.xlims.ensure(xl.size());
+    sc.qlims.ensure(ql.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.xlims.p, xl.data(), xl.size() * 8, cudaMemcpyHostToDevice, st));
+    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.qlims.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice, st));
+    std::vector<int32_t> row_list((size_t)std::max<int64_t>(nq_rows, 1));
+    for (int64_t l = 0; l < n_lists; l++)
+        for (int64_t r = ql[l]; r < ql[l + 1]; r++) row_list[r] = (int32_t)l;
+    sc.row_list.ensure(row_list.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.row_list.p, row_list.data(), row_list.size() * 4, cudaMemcpyHostToDevice, st));
+    fi.s_qn.ensure(std::max<int64_t>(nq_rows, 1));
+    if (metric == KB2_METRIC_L2 && nq_rows > 0)
+        row_norms_kernel<<<grid1d(nq_rows * 32, 256), 256, 0, st>>>(dq, nq_rows, d, fi.s_qn.p);
+    fi.s_cert.ensure((size_t)n_lists + 2);
+    KB2_CUDA_CHECK(cudaMemsetAsync(fi.s_cert.p, 0, 8, st));
+    pqtc::max_abs_kernel<<<2 * num_sms(), 256, 0, st>>>(xn, nb, fi.s_cert.p);
+
+    CUtensorMap tq, tx;
+    const bool use_tc = nq_rows > 0 && tc::make_tmap(&tq, dq, nq_rows, d) && tc::make_tmap(&tx, X, nb, d);
+    const int K = k + 16;
+    const int64_t lds = round_up(n_docs, 4);
+    // lists per chunk: S within the 256 MB key budget of dense_candidates; the candidates, their exact keys, the sorted
+    // rows and the re-rank items (at most one per candidate) within the large-k scratch
+    const int64_t L = std::max<int64_t>(1, std::min<int64_t>({n_lists, (64ll << 20) / lds, large_k_group(n_lists, (int64_t)K * 40 + 16)}));
+    // lists per all-documents group (at most L, so the K-entry buffers fit): the key rows within the same 64 M entries,
+    // the candidate rows and their items within the large-k scratch; rows x n_docs < 2^31 as RerankItem::c0 is int32
+    const int64_t La = std::max<int64_t>(1, std::min<int64_t>({L, (64ll << 20) / n_docs, large_k_group(n_lists, n_docs * 24)}));
+    std::vector<Item> items;
+    if (use_tc) {
+        items = plan_items(xl);
+        sc.items.ensure(std::max<size_t>(items.size(), 1));
+        if (!items.empty())
+            KB2_CUDA_CHECK(cudaMemcpyAsync(sc.items.p, items.data(), items.size() * sizeof(Item), cudaMemcpyHostToDevice, st));
+        fi.s_keys.ensure((size_t)L * lds);
+    }
+    sc.cand.ensure((size_t)L * K);
+    sc.sorted.ensure((size_t)L * K);
+    sc.seg_off.ensure((size_t)L + 1);
+    segment_offsets_kernel<<<grid1d(L + 1, 256), 256, 0, st>>>(sc.seg_off.p, L, K);
+    size_t tmp_bytes = 0;
+    cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, sc.cand.p, sc.sorted.p, (int)(L * K), (int)L, sc.seg_off.p,
+                                            sc.seg_off.p + 1, 0, 64, st);
+    sc.sort_tmp.ensure(tmp_bytes);
+    const bool vec4 = (d & 3) == 0 && (reinterpret_cast<uintptr_t>(dq) & 15) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
+
+    // exact keys of `rows` candidate rows of n entries in all into sc.exact; the slots of kEmpty padding stay kEmpty
+    auto exact = [&](const uint64_t* cand, const int64_t* cand_off, int64_t n, int64_t rows, int64_t l0, const uint32_t* qlist) {
+        sc.exact.ensure(n);
+        KB2_CUDA_CHECK(cudaMemsetAsync(sc.exact.p, 0xFF, n * 8, st));
+        const RerankParams rp{dq, sc.qlims.p, X, nullptr, sc.xlims.p, d, l0, nullptr, cand, nullptr};
+        rerank(fi, metric, vec4, rp, cand_off, qlist, rows, sc.exact, sc.rr, nullptr);
+        fi.last.launches += 4;
+    };
+    // sort the K entries of each row by (key, document) and emit the rows
+    auto sort_emit = [&](const uint64_t* in, int64_t rows, int64_t l0, const uint32_t* qlist, const uint64_t* approx) {
+        size_t bytes = tmp_bytes;
+        KB2_CUDA_CHECK(cub::DeviceSegmentedRadixSort::SortKeys(sc.sort_tmp.p, bytes, in, sc.sorted.p, (int)(rows * K), (int)rows,
+                                                               sc.seg_off.p, sc.seg_off.p + 1, 0, 64, st));
+        EmitParams pp{sc.sorted.p, approx, K, k, dq, sc.qlims.p, d, fi.s_cert.p, l0, qlist, d_ids, d_dist};
+        with_metric(metric, [&](auto m) { maxsim_emit_kernel<decltype(m)::value><<<(unsigned)rows, 256, 0, st>>>(pp); });
+        fi.last.launches += 2;
+        KB2_CUDA_CHECK(cudaGetLastError());
+    };
+    // exact keys of every document the bitset keeps for `rows` lists (at most La) -> their K best -> sorted, emitted.
+    // The kept documents are listed on the host the first time: filtered ones are never scored.
+    std::vector<uint32_t> kept;
+    bool listed = false;
+    auto exact_all = [&](int64_t rows, int64_t l0, const uint32_t* qlist) {
+        if (!listed) {
+            std::vector<uint8_t> bits(dbits ? (size_t)((n_docs + 7) / 8) : 0);
+            if (dbits) {
+                KB2_CUDA_CHECK(cudaMemcpyAsync(bits.data(), dbits, bits.size(), cudaMemcpyDeviceToHost, st));
+                KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+            }
+            for (int64_t j = 0; j < n_docs; j++)
+                if (!dbits || !((bits[j >> 3] >> (j & 7)) & 1)) kept.push_back((uint32_t)j);
+            sc.kept.ensure(std::max<size_t>(kept.size(), 1));
+            KB2_CUDA_CHECK(cudaMemcpyAsync(sc.kept.p, kept.data(), kept.size() * 4, cudaMemcpyHostToDevice, st));
+            listed = true;
+        }
+        const int64_t n_kept = (int64_t)kept.size(), n = rows * n_kept;
+        sc.cand.ensure(n);
+        sc.doc_off.ensure(rows + 1);
+        if (n > 0) all_docs_kernel<<<grid1d(n, 256), 256, 0, st>>>(sc.kept.p, n_kept, n, sc.cand.p);
+        segment_offsets_kernel<<<grid1d(rows + 1, 256), 256, 0, st>>>(sc.doc_off.p, rows, n_kept);
+        fi.last.launches += 2;
+        exact(sc.cand.p, sc.doc_off.p, n, rows, l0, qlist);
+        large_k_select<uint64_t>(fi, sc.exact.p, n_kept, n_kept, 0u, K, sc.cand.p, K, rows);
+        sort_emit(sc.cand.p, rows, l0, qlist, nullptr);
+    };
+
+    if (!use_tc) {
+        for (int64_t l0 = 0; l0 < n_lists; l0 += La) exact_all(std::min(La, n_lists - l0), l0, nullptr);
+        stats[0] += n_lists;
+        stats[2] += n_lists;
+        return;
+    }
+    for (int64_t l0 = 0; l0 < n_lists; l0 += L) {
+        const int64_t rows = std::min(L, n_lists - l0);
+        pqtc::fill_f32_kernel<<<grid1d(rows * lds, 256), 256, 0, st>>>(fi.s_keys.p, rows * lds, INFINITY);
+        FilterParams fp{sc.items.p, (int)items.size(), sc.xlims.p, sc.qlims.p, sc.row_list.p, fi.s_qn.p, xn,
+                        ql[l0], ql[l0 + rows], l0, d, dbits, fi.s_keys.p, lds};
+        if (fp.r1 > fp.r0 && fp.nitems > 0) {
+            const unsigned grid = (unsigned)std::min<int64_t>(num_sms(), fp.nitems);
+            with_metric(metric, [&](auto m) {
+                launch<maxsim_filter_kernel<decltype(m)::value>>(grid, tc::THREADS, SMEM_BYTES, st, tq, tx, fp);
+            });
+            fi.last.launches++;
+            KB2_CUDA_CHECK(cudaGetLastError());
+        }
+        large_k_select<float>(fi, fi.s_keys.p, lds, n_docs, 0u, K, sc.cand.p, K, rows);
+        exact(sc.cand.p, sc.seg_off.p, rows * K, rows, l0, nullptr);
+        sort_emit(sc.exact.p, rows, l0, nullptr, sc.cand.p);
+        stats[1] += rows * K;
+    }
+    int64_t nredo = 0;
+    if (n_lists > 0) {
+        uint32_t* hc = (uint32_t*)fi.h_counter.p;
+        KB2_CUDA_CHECK(cudaMemcpyAsync(hc, fi.s_cert.p + 1, 4, cudaMemcpyDeviceToHost, st));
+        KB2_CUDA_CHECK(cudaStreamSynchronize(st));
+        nredo = hc[0];
+        for (int64_t r0 = 0; r0 < nredo; r0 += La) exact_all(std::min(La, nredo - r0), 0, fi.s_cert.p + 2 + r0);
+    }
+    stats[0] += n_lists;
+    stats[2] += nredo;
 }
 
 }  // namespace msim

@@ -1,7 +1,7 @@
 """Emb-list (multi-vector) search on HNSW and IVF_FLAT (TokenANN, DESIGN §4.11): time per search and per stage, candidates
-per list, the re-rank's useful FLOP/s, recall@k against the exact BruteForce emb-list search, and the re-rank kernel
-against the BruteForce re-rank kernel on the same (list, document) pairs.  One JSON line per measurement; with --out
-the whole record also goes to that file.  Needs an H100.
+per list, the re-rank's useful FLOP/s, recall@k against the exact BruteForce emb-list search, and a torch.profiler
+trace of one k = 100 search.  One JSON line per measurement; with --out the whole record also goes to that file.  Needs
+an H100.
 
 Workload (defaults): 20 000 documents of 32..256 rows of datagen.clustered (d = 128, ~2.9M rows), MAX_SIM_IP; HNSW
 (M 16, efConstruction 100, built on the GPU) and IVF_FLAT (nlist 2048); 1000 query lists of 32 tokens, each token a row
@@ -121,41 +121,6 @@ def main():
         rec["results"].append({"index": itype, "profile_k100_kernel_ms": top})
         print(json.dumps({"index": itype, "profile_k100_kernel_ms": top}), flush=True)
 
-        # the re-rank kernel against maxsim_exact_kernel on this index's candidates at k = 100, ratio 3: the search at
-        # k = 16384 with the same vec_topk (300) returns every candidate of each list.  HNSW needs ef >= k, so its pairs
-        # come from a beam of 16384, wider than the timed searches' max(ef, 300): candidates of the same kind, not the same sets
-        vt = int(np.float32(100) * np.float32(3.0))
-        cfg = dict(base_cfg, retrieval_ann_ratio=(vt + 0.5) / 16384)
-        if itype == "HNSW":
-            cfg["ef"] = 16384
-        nl = min(a.lists, 200)
-        try:
-            ids, _ = ix.search_emb_list(xq[:nl * a.tokens], ql[:nl + 1], 16384, cfg)
-            ids = ids.cpu().numpy()
-        except kb.KnowhereError as e:
-            print(json.dumps({"index": itype, "pairs_skipped": str(e)}), flush=True)
-            continue
-        pl, docs = [0], []
-        for l in range(nl):
-            c = np.sort(ids[l][ids[l] >= 0])
-            docs.append(c)
-            pl.append(pl[-1] + c.size)
-        pd = torch.as_tensor(np.concatenate(docs).astype(np.int32), device=dev)
-        t_rr, t_ex = [], []
-        for _ in range(3):
-            s1, ms1 = kb.debug_maxsim_pairs(xq, ql[:nl + 1], xb, xl, np.array(pl), pd, "IP", use_rerank=True)
-            s0, ms0 = kb.debug_maxsim_pairs(xq, ql[:nl + 1], xb, xl, np.array(pl), pd, "IP", use_rerank=False)
-            t_rr.append(ms1)
-            t_ex.append(ms0)
-        same = bool(torch.equal(s1.view(torch.int32), s0.view(torch.int32)))
-        pairs = int(pl[-1])
-        dist_n = int(sum((xl[c + 1] - xl[c]).sum() for c in docs)) * a.tokens
-        r = {"index": itype, "pairs": pairs, "lists": nl, "rerank_kernel_ms": float(np.median(t_rr)),
-             "exact_kernel_ms": float(np.median(t_ex)), "bit_identical": same,
-             "rerank_useful_tflops": 2.0 * a.dim * dist_n / (np.median(t_rr) * 1e-3) / 1e12,
-             "exact_useful_tflops": 2.0 * a.dim * dist_n / (np.median(t_ex) * 1e-3) / 1e12}
-        rec["results"].append(r)
-        print(json.dumps(r), flush=True)
         del ix
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)

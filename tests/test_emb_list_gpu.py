@@ -17,7 +17,8 @@ Paths: d % 4 == 0 runs the tensor-core filter (maxsim_filter_kernel), the K = k 
 certification; k >= 1009 has K > 1024 (the same path, no other selection kernel exists here); d % 4 != 0 runs the exact
 all-documents mode for every list (stats[2] == n_lists); data with a large common offset under MAX_SIM_L2 makes the filter's
 bound too wide to certify and runs the exact redo of those lists (stats[2] > 0).  Documents longer than 128 rows span
-several filter tiles, query lists longer than 128 tokens several query blocks.
+several filter tiles, query lists longer than 128 tokens several query blocks.  The candidate re-rank and the
+all-documents mode both run maxsim_rerank_kernel; test_rerank_shapes takes each across its row tiles and token blocks.
 """
 import os
 import subprocess
@@ -215,6 +216,34 @@ def test_fallback_large_offset_l2(kb):
     assert st[2] > 0, st
     S, B = oracle(xb, xl, xq, ql, "MAX_SIM_L2")
     check_emb(ids, dist, S, B, "MAX_SIM_L2", what="offset")
+
+
+# the re-rank's shapes: documents of 0, 1, 128, 129 and 300 rows (several 128-row tiles), query lists of 0, 1 and 200
+# tokens (several 32-token blocks)
+RR_DOC_LEN = np.concatenate([[0, 1, 129, 300, 0, 128], np.random.default_rng(27).integers(0, 60, 200)])
+RR_Q_LEN = np.array([200, 1, 37, 0, 5, 64])
+
+
+@pytest.mark.parametrize("metric,offset", [("MAX_SIM_IP", 0.0), ("MAX_SIM_L2", 0.0), ("MAX_SIM_L2", 200.0)])
+@pytest.mark.parametrize("d", [30, 128, 768])
+@pytest.mark.parametrize("keep", [1.0, 0.5])
+def test_rerank_shapes(kb, metric, offset, d, keep):
+    """d = 30 re-ranks every document of every list with scalar loads; d = 128 and 768 re-rank the filter's candidates
+    with float4 loads, and with the large common offset under MAX_SIM_L2 also every document of the uncertified lists.
+    With keep = 0.5 half the documents are filtered out and skipped inside each all-documents row."""
+    xb, xl = _data(RR_DOC_LEN, d, 28 + d, offset=offset, scale=0.05 if offset else 1.0)
+    xq, ql = _data(RR_Q_LEN, d, 29 + d, offset=offset, scale=0.05 if offset else 1.0)
+    filt = np.random.default_rng(30).random(len(RR_DOC_LEN)) >= keep
+    k = 10
+    ids, dist, st = kb.brute_force_search_emb_list(xb, xl, xq, ql, k, metric, bitset=np.packbits(filt, bitorder="little"),
+                                                   stats=True)
+    S, B = oracle(xb, xl, xq, ql, metric)
+    check_emb(ids, dist, S, B, metric, valid=~filt, what=f"{metric} d={d} offset={offset} keep={keep}")
+    if d % 4:
+        assert st[1] == 0 and st[2] == len(RR_Q_LEN), st           # all-documents mode
+    else:
+        assert st[1] == len(RR_Q_LEN) * (k + 16), st                # the filter's candidates
+        assert st[2] > 0 or offset == 0, st                         # the redo of uncertified lists
 
 
 @pytest.mark.parametrize("metric,single", [("MAX_SIM_IP", "IP"), ("MAX_SIM_L2", "L2")])

@@ -4,7 +4,8 @@ Expected results come from a numpy restatement of TokenANN applied to the refere
 token's vec_topk = min(max(int32(fp32(k) * fp32(ratio)), 1), rows) hits, the distinct documents of a list's hits as its
 candidates, their MaxSim scores in float64, the k best by (score, document id), padded with id -1 and -FLT_MAX (IP) or
 FLT_MAX (L2).  HNSW runs on small-integer vectors, where every distance and every score is exact in fp32, so ids and
-distance bits must be equal.  The re-rank kernel is held to maxsim_exact_kernel (the BruteForce re-rank) bit for bit.
+distance bits must be equal.  The re-rank is the BruteForce re-rank: with every document a candidate, the result is the
+BruteForce emb-list result, ids and distance bits.
 """
 import functools
 import os
@@ -196,30 +197,6 @@ def test_ivf_flat_exact_stage1_equals_bruteforce(kb, ref, metric):
     assert np.array_equal(v, bi >= 0)
     assert np.array_equal(ids[v], bi[v])
     assert np.array_equal(dist[v].view(np.uint32), bd[v].view(np.uint32))
-
-
-# ---------------------------------------------------------------- the re-rank kernel against maxsim_exact_kernel
-@pytest.mark.parametrize("metric", ["L2", "IP"])
-@pytest.mark.parametrize("d", [30, 128, 768])
-def test_rerank_kernel_bit_identical_to_exact_kernel(kb, metric, d):
-    rng = np.random.default_rng(d)
-    doc_len = np.concatenate([[0, 1, 129, 300, 0, 128], rng.integers(0, 60, 200)])
-    xl = _lims(doc_len)
-    ql = _lims([200, 1, 37, 0, 5, 64])
-    xb = torch.randn(int(xl[-1]), d, device="cuda")
-    xq = torch.randn(int(ql[-1]), d, device="cuda")
-    pl = [0]
-    docs = []
-    for l in range(len(ql) - 1):
-        c = np.sort(rng.choice(len(doc_len), int(rng.integers(1, 120)), replace=False))
-        docs.append(c)
-        pl.append(pl[-1] + c.size)
-    pd = torch.as_tensor(np.concatenate(docs).astype(np.int32), device="cuda")
-    a, _ = kb.debug_maxsim_pairs(xq, ql, xb, xl, np.array(pl), pd, metric, use_rerank=True)
-    b, _ = kb.debug_maxsim_pairs(xq, ql, xb, xl, np.array(pl), pd, metric, use_rerank=False)
-    a, b = a.cpu().numpy(), b.cpu().numpy()
-    assert np.isfinite(a).sum() > 0
-    assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), f"{(a != b).sum()} of {a.size} scores differ"
 
 
 @pytest.mark.parametrize("metric", [0, 1])
