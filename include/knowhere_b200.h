@@ -372,6 +372,14 @@ int kb2_index_last_stage_info(kb2_index_t h, float* out4);
 int kb2_debug_gemm_keys(const float* q, int64_t nq, const float* x, int64_t nb, int dim, int metric, int use_tc,
                         float* out_keys, int device);
 
+/* validation hook: the k-means of the IVF build (the coarse quantizer and every PQ sub-quantizer are trained by it) over
+ * the n rows x (device, n x dim fp32): k centroids, metric KB2_METRIC_L2 or KB2_METRIC_IP, niter Lloyd iterations from a
+ * std::mt19937_64 seeded with seed (IVF build: niter 25, seed 1234).  niter = 0 returns the initial centroids.
+ * out_centroids: device, k x dim fp32.  n < k: KB2_INVALID_ARGS.  Used by tests to hold each Lloyd step to a numpy
+ * model (DESIGN §4.8). */
+int kb2_debug_kmeans(const float* x, int64_t n, int dim, int k, int metric, int niter, uint64_t seed,
+                     float* out_centroids, int device);
+
 /* validation hook: step 1 of the GPU_CAGRA build alone (DESIGN §4.12) over the n rows x (device, n x dim fp32), with
  * the build keys of json (intermediate_graph_degree, build_algo, nn_descent_niter; errors as kb2_index_create).  metric:
  * KB2_METRIC_L2 or KB2_METRIC_IP.  m = min(intermediate_graph_degree, n - 1); out_ids (device, n x m int32) receives

@@ -972,6 +972,23 @@ kb2_debug_gemm_keys(const float* q, int64_t nq, const float* x, int64_t nb, int 
     });
 }
 
+// ---------------------------------------------------------------- validation hook for the IVF build's k-means
+int
+kb2_debug_kmeans(const float* x, int64_t n, int dim, int k, int metric, int niter, uint64_t seed, float* out_centroids,
+                 int device) {
+    return guarded([&] {
+        require_device(device);
+        KB2_REQUIRE(x && out_centroids, KB2_INVALID_ARGS, "null buffer");
+        KB2_REQUIRE(is_device_ptr(x) && is_device_ptr(out_centroids), KB2_INVALID_ARGS, "debug_kmeans takes device pointers");
+        KB2_REQUIRE(metric == KB2_METRIC_L2 || metric == KB2_METRIC_IP, KB2_INVALID_METRIC_TYPE, "metric must be L2 or IP");
+        KB2_REQUIRE(dim > 0 && k > 0 && niter >= 0 && n < (1ll << 31), KB2_INVALID_ARGS, "bad sizes");
+        KB2_CUDA_CHECK(cudaDeviceSynchronize());   // the caller's rows are ready before the default stream reads them
+        kmeans_train(x, n, dim, k, metric, niter, seed, out_centroids, nullptr);
+        KB2_CUDA_CHECK(cudaDeviceSynchronize());
+        KB2_CUDA_CHECK(cudaGetLastError());
+    });
+}
+
 // ---------------------------------------------------------------- validation hook for GPU_CAGRA's intermediate graph
 int
 kb2_debug_cagra_knn_graph(const float* x, int64_t n, int dim, int metric, const char* json, int32_t* out_ids, float* out_keys,

@@ -894,6 +894,12 @@ struct IvfIndex : IndexBase {
     train(const float* x, int64_t n) override {
         KB2_REQUIRE(!trained, KB2_INDEX_ALREADY_TRAINED, "index already trained");
         KB2_REQUIRE(n > 0, KB2_INVALID_ARGS, "empty training set");
+        // refused before anything changes, so that a refused train() leaves the configured nlist for the next one
+        if (is_pq) {
+            KB2_REQUIRE(nbits == 8, KB2_NOT_IMPLEMENTED, "IVF_PQ: only nbits=8 is implemented on the GPU path");
+            KB2_REQUIRE(M > 0 && dim % M == 0, KB2_INVALID_ARGS, "IVF_PQ: dim must be a multiple of m");
+            KB2_REQUIRE(n >= 256, KB2_INVALID_ARGS, "IVF_PQ: need at least 256 training rows for nbits=8");
+        }
         // MatchNlist (ivf.cc:479-489)
         if (nlist * 39 > n) nlist = std::max<int64_t>(1, n / 39);
         DevBuf<float> xbuf;
@@ -902,9 +908,6 @@ struct IvfIndex : IndexBase {
         kmeans_train(dx, n, dim, (int)nlist, metric, 25, 1234, centroids.p, stream);
         set_centroids_common();
         if (is_pq) {
-            KB2_REQUIRE(nbits == 8, KB2_NOT_IMPLEMENTED, "IVF_PQ: only nbits=8 is implemented on the GPU path");
-            KB2_REQUIRE(M > 0 && dim % M == 0, KB2_INVALID_ARGS, "IVF_PQ: dim must be a multiple of m");
-            KB2_REQUIRE(n >= 256, KB2_INVALID_ARGS, "IVF_PQ: need at least 256 training rows for nbits=8");
             dsub = dim / M;
             // residuals of (a subsample of) the training set: F/IndexIVF.cpp:1307-1329, IndexIVFPQ.cpp:76-95
             const int64_t nt = std::min<int64_t>(n, 256 * 256);
