@@ -319,8 +319,26 @@ int kb2_index_emb_list_offsets(kb2_index_t h, int64_t* n_docs, int64_t* lims);
 int kb2_index_search_emb_list(kb2_index_t h, const float* queries, const int64_t* query_lims, int64_t n_lists, int k,
                               const char* json, const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids,
                               float* out_dist, int64_t* out_stats);
-/* device ms of the stages of the last kb2_index_search_emb_list on this handle (with kb2_index_enable_kernel_timing):
- * out4 = stage 1 (base search), candidates, re-rank, select + emit */
+/* ---- the MUVERA strategy (src/index/emb_list/emb_list_strategy_muvera.cc; DESIGN §4.11): an HNSW or IVF_FLAT handle
+ * created with "emb_list_strategy": "muvera" (default, or an empty string: "tokenann"; "lemur": KB2_NOT_IMPLEMENTED; any
+ * other string: KB2_INVALID_ARGS; other index types do not read these keys and refuse kb2_index_set_emb_list), "muvera_num_projections" P (1..7, default 4), "muvera_num_repeats" R (1..32, default 7) and
+ * "muvera_seed" S (int32, default 42; out of range: KB2_OUT_OF_RANGE_IN_JSON).  With token dimension d, B = 2^P buckets
+ * and E = R * B * d encoded dimensions.  On such a handle kb2_index_add keeps the token rows (raw, also under COSINE),
+ * kb2_index_train does nothing and kb2_index_count is the token-row count; kb2_index_search / _range_search return
+ * KB2_EMB_LIST_INNER_ERROR and kb2_hnsw_* / kb2_ivf_* KB2_NOT_IMPLEMENTED.  kb2_index_set_emb_list (same checks as
+ * above) encodes every document into its Fixed Dimensional Encoding (per repeat and bucket the mean of its tokens in
+ * the bucket) and builds the base index of the handle's type over the n_docs encoded rows (IVF_FLAT: its k-means and
+ * nlist cap; HNSW: its build); a second kb2_index_set_emb_list on such a handle is KB2_NOT_IMPLEMENTED.  A base that cannot serve E fails here or at search with its own error (limits:
+ * kb2_emb_list_index.cuh).  kb2_index_search_emb_list encodes each query list (the sum of its tokens per bucket),
+ * searches the base for ann_k documents and, with "emb_list_rerank" true (default), re-ranks them by exact MaxSim as
+ * above: ann_k = min(max(int(k * ratio), 1), n_docs); the bitset filters documents of the base directly; a list gets
+ * the k best of its candidates, empty documents skipped, padded as above.  With emb_list_rerank false: ann_k =
+ * min(k, n_docs), the base's ids and distances as they are, padded with -1 and -inf (MAX_SIM_IP / _COSINE) or +inf.
+ * The "KB2I" blob holds the base, P, R, S, d, the offsets and the token rows; the faiss stream: KB2_NOT_IMPLEMENTED.
+ * GetIndexMeta adds emb_list_strategy, muvera_num_projections, muvera_num_repeats, muvera_seed and muvera_encoded_dim.
+ *
+ * device ms of the stages of the last kb2_index_search_emb_list on this handle (with kb2_index_enable_kernel_timing):
+ * out4 = stage 1 (base search; MUVERA: encode + base search), candidates, re-rank, select + emit */
 int kb2_index_emb_list_stage_ms(kb2_index_t h, float* out4);
 
 /* ---- multi-GPU: one process per GPU, inverted lists sharded (kb2_index_set_shard), collectives over NCCL/NVLink
@@ -379,6 +397,14 @@ int kb2_debug_gemm_keys(const float* q, int64_t nq, const float* x, int64_t nb, 
  * model (DESIGN §4.8). */
 int kb2_debug_kmeans(const float* x, int64_t n, int dim, int k, int metric, int niter, uint64_t seed,
                      float* out_centroids, int device);
+
+/* validation hook: the MUVERA encoder (DESIGN §4.11) over n_items items, item i being the rows [lims[i], lims[i+1]) of x
+ * (n x dim fp32; x and lims host or device).  out_projections (nullable, host or device, R x P x dim fp32): the
+ * projections drawn from num_projections P, num_repeats R and seed; out_fde (nullable, host or device, n_items x E fp32,
+ * E = R * 2^P * dim): the encodings, mean != 0 as documents (kb2_index_set_emb_list), 0 as query lists.  Used by tests to
+ * hold the projections to the C++ standard library and the encodings to a numpy model. */
+int kb2_debug_muvera_encode(const float* x, const int64_t* lims, int64_t n_items, int dim, int num_projections,
+                            int num_repeats, int seed, int mean, float* out_projections, float* out_fde, int device);
 
 /* validation hook: step 1 of the GPU_CAGRA build alone (DESIGN §4.12) over the n rows x (device, n x dim fp32), with
  * the build keys of json (intermediate_graph_degree, build_algo, nn_descent_niter; errors as kb2_index_create).  metric:

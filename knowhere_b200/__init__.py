@@ -96,6 +96,7 @@ def _declare(L):
                                                 c.POINTER(vp), c.POINTER(vp), c.POINTER(vp)]
     L.kb2_bruteforce_search_sparse.argtypes = [vp, vp, vp, i64, vp, vp, vp, i64, i32, i32, c.c_char_p, vp, i64, vp, vp, i32]
     L.kb2_debug_cagra_knn_graph.argtypes = [vp, i64, i32, i32, c.c_char_p, vp, vp, vp, vp, i32, vp, i32]
+    L.kb2_debug_muvera_encode.argtypes = [vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i32]
     if hasattr(L, "kb2_faiss_describe"):
         L.kb2_faiss_describe.argtypes = [vp, c.c_size_t, i32, vp, c.c_size_t]
         L.kb2_faiss_rewrite.argtypes = [vp, c.c_size_t, i32, c.POINTER(vp), c.POINTER(c.c_size_t)]
@@ -344,10 +345,13 @@ class Index:
         _check(self.L.kb2_index_get_meta(self.h, ctypes.cast(buf, ctypes.c_void_p), 1024))
         return json.loads(buf.value.decode())
 
-    # -- emb-lists (multi-vector documents) on HNSW / IVF_FLAT: the reference's TokenANN strategy (DESIGN §4.11)
+    # -- emb-lists (multi-vector documents) on HNSW / IVF_FLAT: the reference's TokenANN strategy, or MUVERA with the create
+    #    keys {"emb_list_strategy": "muvera", "muvera_num_projections": P, "muvera_num_repeats": R, "muvera_seed": S}
+    #    (DESIGN §4.11)
     def set_emb_list(self, lims, metric):
         """attach document offsets (int64 [n_docs + 1], ending at count()) and the MAX_SIM metric that pairs with the
-        index metric (MAX_SIM_L2 - L2, MAX_SIM_IP - IP, MAX_SIM / MAX_SIM_COSINE - COSINE)"""
+        index metric (MAX_SIM_L2 - L2, MAX_SIM_IP - IP, MAX_SIM / MAX_SIM_COSINE - COSINE); on a MUVERA index this
+        encodes the documents and builds the base index over them"""
         lims = lims if _is_torch(lims) else np.ascontiguousarray(lims, np.int64)
         _check(self.L.kb2_index_set_emb_list(self.h, _ptr(lims), int(lims.shape[0]) - 1,
                                              _EMB_METRICS.get(str(metric).upper(), -1)))
@@ -362,8 +366,8 @@ class Index:
     def search_emb_list(self, q, q_lims, k, config=None, bitset=None, stats=False):
         """q: [rows, dim] float32 query tokens, q_lims: int64 [n_lists + 1] (numpy or CUDA tensors).  Returns (ids, dist)
         [n_lists, k] (CUDA tensors when q is), documents best first; with stats=True also int64 [query lists,
-        candidates re-ranked, token x row distances].  config: retrieval_ann_ratio (default 3) and the base search keys;
-        bitset: one bit per document."""
+        candidates re-ranked, token x row distances].  config: retrieval_ann_ratio (default 3), emb_list_rerank (MUVERA,
+        default true) and the base search keys; bitset: one bit per document."""
         if not _is_torch(q_lims):
             q_lims = np.ascontiguousarray(q_lims, np.int64)
         n_lists = int(q_lims.shape[0]) - 1
@@ -566,6 +570,20 @@ def brute_force_search(base, queries, k, metric="L2", bitset=None, device=0, str
 # emb-list metrics (reference index_param.h:280-285; names are case-insensitive, "MAX_SIM" is MAX_SIM_COSINE).  Names the
 # library has no metric for (MAX_SIM_HAMMING, MAX_SIM_JACCARD) go through as -1, which it rejects as an invalid metric.
 _EMB_METRICS = {"MAX_SIM": 5, "MAX_SIM_COSINE": 5, "MAX_SIM_IP": 4, "MAX_SIM_L2": 3}
+
+
+def debug_muvera_encode(x, lims, num_projections=4, num_repeats=7, seed=42, mean=True, device=0):
+    """The MUVERA encoder on the device (validation hook): (projections [R, P, dim], encodings [n_items, R * 2^P * dim])
+    of the items lims[i] .. lims[i + 1] of the float32 rows x; mean=True encodes documents, False query lists."""
+    L = lib()
+    x = np.ascontiguousarray(x, np.float32)
+    lims = np.ascontiguousarray(lims, np.int64)
+    n_items, dim = lims.shape[0] - 1, x.shape[1]
+    proj = np.empty((num_repeats, num_projections, dim), np.float32)
+    fde = np.empty((n_items, num_repeats * (1 << num_projections) * dim), np.float32)
+    _check(L.kb2_debug_muvera_encode(_ptr(x), _ptr(lims), n_items, dim, num_projections, num_repeats, seed, 1 if mean else 0,
+                                     _ptr(proj), _ptr(fde), device))
+    return proj, fde
 
 
 def brute_force_search_emb_list(base, base_lims, queries, query_lims, k, metric="MAX_SIM", bitset=None, device=0,

@@ -13,8 +13,13 @@ NVCC_FLAGS = [
 ]
 
 
+# the translation units of the library, in link order: every build of it (also scripts/filter_stalls.py) compiles these.
+# kb2_muvera_proj.cpp is a host unit of its own, compiled without FMA contraction (see its header).
+UNITS = [os.path.join(CSRC, "kb2_capi.cu"), os.path.join(CSRC, "kb2_muvera_proj.cpp")]
+
+
 def sources():
-    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh", ".h")))
+    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh", ".h", ".cpp")))
 
 
 def needs_build():
@@ -30,7 +35,7 @@ def build(force=False, verbose=False):
     if not force and not needs_build():
         return LIB
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    cmd = [nvcc] + NVCC_FLAGS + ["-o", LIB, os.path.join(CSRC, "kb2_capi.cu"), "-lgomp", "-ldl"]
+    cmd = [nvcc] + NVCC_FLAGS + ["-o", LIB] + UNITS + ["-lgomp", "-ldl"]
     if verbose:
         cmd += ["-Xptxas", "-v"]
     r = subprocess.run(cmd, capture_output=True, text=True)

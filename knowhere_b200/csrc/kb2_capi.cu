@@ -91,6 +91,8 @@ template <typename T>
 inline T*
 ix_as(kb2_index_t h, const char* what) {
     T* p = dynamic_cast<T*>(ix_of(h));
+    KB2_REQUIRE(p != nullptr || !dynamic_cast<MuveraIndex*>(ix_of(h)), KB2_NOT_IMPLEMENTED,
+                std::string(what) + " calls on a MUVERA emb-list index (its base holds the documents' encodings)");
     KB2_REQUIRE(p != nullptr, KB2_INVALID_ARGS, std::string("handle is not an ") + what + " index");
     return p;
 }
@@ -190,6 +192,10 @@ kb2_index_create(const char* index_type, int metric, int dim, const char* json_c
         require_device(device);
         std::unique_ptr<IndexBase> ix = make_index(t);
         KB2_REQUIRE(ix, KB2_INVALID_ARGS, "unknown index type " + t);
+        // emb_list_strategy muvera: the handle keeps the token rows and builds its base at kb2_index_set_emb_list.  The
+        // strategy is read on the types that take emb-lists only; the others refuse kb2_index_set_emb_list, as for TokenANN
+        MuveraParams mp;
+        if (ix->takes_emb_list() && muvera_params_of(cfg, mp)) ix = std::make_unique<MuveraIndex>();
         // COSINE = inner product of L2-normalised vectors: data is normalised when it enters the index and
         // queries when they are searched (what the reference does for IVF_PQ, ivf.cc:557-565,1067-1071; for FLAT
         // the reference keeps inverse norms instead, flat.cc:57-62 — same similarities)
@@ -270,7 +276,7 @@ kb2_index_train_typed(kb2_index_t h, const void* x, int dtype, int64_t n) {
         KB2_REQUIRE(!ix->emb_list, KB2_NOT_IMPLEMENTED, "Train on an emb-list index");
         ix->wait_caller_work();
         const float* xf = widen_to_f32(ix, x, dtype, n * ix->dim);
-        ix->train(ix->cosine ? ix->normalized(xf, n) : xf, n);
+        ix->train(ix->cosine && !ix->raw_rows_on_entry() ? ix->normalized(xf, n) : xf, n);
     });
 }
 int
@@ -285,7 +291,7 @@ kb2_index_add_typed(kb2_index_t h, const void* x, int dtype, int64_t n, const in
         KB2_REQUIRE(!ix->emb_list, KB2_NOT_IMPLEMENTED, "AddEmbList is not implemented: rows cannot be added to an emb-list index");
         ix->wait_caller_work();
         const float* xf = widen_to_f32(ix, x, dtype, n * ix->dim);
-        ix->add(ix->cosine ? ix->normalized(xf, n) : xf, n, ids);
+        ix->add(ix->cosine && !ix->raw_rows_on_entry() ? ix->normalized(xf, n) : xf, n, ids);
     });
 }
 int
@@ -986,6 +992,38 @@ kb2_debug_kmeans(const float* x, int64_t n, int dim, int k, int metric, int nite
         kmeans_train(x, n, dim, k, metric, niter, seed, out_centroids, nullptr);
         KB2_CUDA_CHECK(cudaDeviceSynchronize());
         KB2_CUDA_CHECK(cudaGetLastError());
+    });
+}
+
+// ---------------------------------------------------------------- validation hook for the MUVERA encoder
+int
+kb2_debug_muvera_encode(const float* x, const int64_t* lims, int64_t n_items, int dim, int num_projections, int num_repeats,
+                        int seed, int mean, float* out_projections, float* out_fde, int device) {
+    return guarded([&] {
+        require_device(device);
+        KB2_REQUIRE(lims && n_items >= 0 && dim > 0, KB2_INVALID_ARGS, "bad sizes");
+        KB2_REQUIRE(num_projections >= 1 && num_projections <= 7 && num_repeats >= 1 && num_repeats <= 32, KB2_OUT_OF_RANGE_IN_JSON,
+                    "muvera_num_projections (1..7) or muvera_num_repeats (1..32) out of range");
+        const MuveraParams mp{num_projections, num_repeats, seed};
+        const std::vector<int64_t> hl = read_lims(lims, n_items, "item");
+        const int64_t ntok = hl.back(), E = (int64_t)num_repeats * (1ll << num_projections) * dim;
+        KB2_REQUIRE(x || ntok == 0, KB2_INVALID_ARGS, "null rows");
+        const std::vector<float> hp = muvera_projections(mp, dim);
+        if (out_projections) KB2_CUDA_CHECK(cudaMemcpy(out_projections, hp.data(), hp.size() * 4, cudaMemcpyDefault));
+        if (!out_fde || n_items == 0) return;
+        DevBuf<float> dp, dx, dout;
+        DevBuf<int64_t> dl;
+        DevBuf<uint8_t> bucket;
+        dp.ensure(hp.size());
+        dl.ensure(hl.size());
+        dx.ensure((size_t)std::max<int64_t>(ntok, 1) * dim);
+        dout.ensure((size_t)n_items * E);
+        KB2_CUDA_CHECK(cudaMemcpy(dp.p, hp.data(), hp.size() * 4, cudaMemcpyHostToDevice));
+        KB2_CUDA_CHECK(cudaMemcpy(dl.p, hl.data(), hl.size() * 8, cudaMemcpyHostToDevice));
+        if (ntok) KB2_CUDA_CHECK(cudaMemcpy(dx.p, x, (size_t)ntok * dim * 4, cudaMemcpyDefault));
+        muvera_encode(mp, dim, dp.p, dx.p, ntok, dl.p, 0, n_items, mean != 0, bucket, dout.p, nullptr);
+        KB2_CUDA_CHECK(cudaDeviceSynchronize());
+        KB2_CUDA_CHECK(cudaMemcpy(out_fde, dout.p, (size_t)n_items * E * 4, cudaMemcpyDefault));
     });
 }
 

@@ -302,6 +302,8 @@ struct IndexBase {
         throw Error(KB2_NOT_IMPLEMENTED, "RangeSearch: unknown index class");
     }
     virtual bool takes_emb_list() const { return false; }   // kb2_index_set_emb_list
+    // rows reach add() / train() as the caller gave them, also under COSINE (a MUVERA emb-list index encodes raw tokens)
+    virtual bool raw_rows_on_entry() const { return false; }
     // emb-lists (kb2_emb_list_index.cuh): the fp32 rows the MaxSim re-rank reads, and each row's position among them (null:
     // row order)
     virtual std::pair<const float*, const int32_t*>

@@ -150,13 +150,34 @@ make_index(const std::string& type) {
 
 inline void
 serialize_index(IndexBase& ix, std::vector<uint8_t>& blob) {
+    // a MUVERA index is stored as its base (the documents' FDE rows) followed by its emb-list section
+    auto* mv = dynamic_cast<MuveraIndex*>(&ix);
+    KB2_REQUIRE(!mv || ix.emb_list, KB2_INVALID_ARGS, "a MUVERA index is serialised once its documents are attached (kb2_index_set_emb_list)");
+    IndexBase& body = mv ? mv->base_index() : ix;
     BlobWriter w{blob};
     w.put<uint32_t>(0x4932424b);  // "KB2I"
     w.put<uint32_t>(1);
-    w.put_str(ix.type);
-    w.put<int32_t>(ix.cosine ? KB2_METRIC_COSINE : ix.metric);
-    w.put<int32_t>(ix.dim);
-    ix.save(w);
+    w.put_str(body.type);
+    w.put<int32_t>(body.cosine ? KB2_METRIC_COSINE : body.metric);
+    w.put<int32_t>(body.dim);
+    body.save(w);
+    // MUVERA: "ELMV", the strategy (1: MUVERA), the MAX_SIM metric, P, R, S, the token dimension, n_docs,
+    // offsets[n_docs + 1] and the token rows [offsets[n_docs]][d] as added; the projections are drawn again on load
+    if (mv) {
+        w.put<uint32_t>(kEmbListMuveraTag);
+        w.put<int32_t>(1);
+        w.put<int32_t>(ix.emb_list->metric);
+        w.put<int32_t>(mv->mp.P);
+        w.put<int32_t>(mv->mp.R);
+        w.put<int32_t>(mv->mp.S);
+        w.put<int32_t>(ix.dim);
+        w.put<int64_t>(ix.emb_list->n_docs());
+        w.put_bytes(ix.emb_list->lims.data(), ix.emb_list->lims.size() * 8);
+        std::vector<float> t((size_t)ix.count() * ix.dim);
+        if (!t.empty()) KB2_CUDA_CHECK(cudaMemcpy(t.data(), mv->tokens.p, t.size() * 4, cudaMemcpyDeviceToHost));
+        w.put_bytes(t.data(), t.size() * 4);
+        return;
+    }
     // optional trailing section of an emb-list index: "ELST", the MAX_SIM metric, n_docs, offsets[n_docs + 1]
     if (ix.emb_list) {
         w.put<uint32_t>(kEmbListTag);
@@ -187,15 +208,40 @@ deserialize_index(const uint8_t* blob, size_t size, int device) {
     ix->init(type, metric, dim, device);   // COSINE: the stored vectors are already normalised; queries will be
     ix->load(r);
     if (r.o < r.n) {
-        KB2_REQUIRE(r.get<uint32_t>() == kEmbListTag, KB2_INVALID_BINARY_SET, "unknown section after the index in blob");
+        const uint32_t tag = r.get<uint32_t>();
+        KB2_REQUIRE(tag == kEmbListTag || tag == kEmbListMuveraTag, KB2_INVALID_BINARY_SET, "unknown section after the index in blob");
+        MuveraParams mp;
+        int d = 0;
+        if (tag == kEmbListMuveraTag) {
+            KB2_REQUIRE(r.get<int32_t>() == 1, KB2_INVALID_BINARY_SET, "unknown emb-list strategy in blob");
+        }
         const int el_metric = r.get<int32_t>();
+        if (tag == kEmbListMuveraTag) {
+            mp.P = r.get<int32_t>();
+            mp.R = r.get<int32_t>();
+            mp.S = r.get<int32_t>();
+            d = r.get<int32_t>();
+            KB2_REQUIRE(ix->takes_emb_list() && mp.P >= 1 && mp.P <= 7 && mp.R >= 1 && mp.R <= 32 && d > 0 && (int64_t)mp.R * (1 << mp.P) * d == dim,
+                        KB2_INVALID_BINARY_SET, "bad MUVERA parameters in blob");
+        }
         const int64_t nd = r.get<int64_t>();
         KB2_REQUIRE(nd >= 1 && (uint64_t)nd < (r.n - r.o) / 8, KB2_INVALID_BINARY_SET, "bad emb-list document count in blob");
         std::vector<int64_t> lims((size_t)nd + 1);
         memcpy(lims.data(), r.get_bytes(lims.size() * 8), lims.size() * 8);
         KB2_REQUIRE(lims[0] == 0, KB2_INVALID_BINARY_SET, "bad emb-list offsets in blob");
         for (int64_t i = 0; i < nd; i++) KB2_REQUIRE(lims[i + 1] >= lims[i], KB2_INVALID_BINARY_SET, "bad emb-list offsets in blob");
-        set_emb_list(*ix, std::move(lims), el_metric);
+        if (tag == kEmbListTag) {
+            set_emb_list(*ix, std::move(lims), el_metric);
+            return ix;
+        }
+        KB2_REQUIRE(lims[nd] >= 1 && (uint64_t)lims[nd] <= (r.n - r.o) / ((size_t)d * 4), KB2_INVALID_BINARY_SET,
+                    "bad MUVERA token count in blob");
+        auto mv = std::make_unique<MuveraIndex>();
+        mv->init(type, metric, d, device);
+        mv->mp = mp;
+        mv->add((const float*)r.get_bytes((size_t)lims[nd] * d * 4), lims[nd], nullptr);
+        set_emb_list(*mv, std::move(lims), el_metric, std::move(ix));
+        return mv;
     }
     return ix;
 }

@@ -28,8 +28,7 @@ def build_lib(out_dir):
     from knowhere_b200 import _build
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     lib = os.path.join(out_dir, "libknowhere_b200_stalls.so")
-    cmd = [nvcc] + _build.NVCC_FLAGS + ["-DKB2_FILTER_STALLS", "-o", lib, os.path.join(_build.CSRC, "kb2_capi.cu"),
-                                        "-lgomp", "-ldl"]
+    cmd = [nvcc] + _build.NVCC_FLAGS + ["-DKB2_FILTER_STALLS", "-o", lib] + _build.UNITS + ["-lgomp", "-ldl"]
     subprocess.run(cmd, check=True)
     return lib
 
