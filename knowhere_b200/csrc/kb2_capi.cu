@@ -740,16 +740,7 @@ kb2_bruteforce_search_emb_list(const float* base, const int64_t* base_lims, int6
         FlatIndex& fi = bf_prepare(slot, device, inner, dim, cuda_stream, base, nb);
         const int64_t nq_rows = ql.back();
         const float* dq = fi.cosine ? fi.normalized(queries, nq_rows) : fi.to_device(queries, (size_t)nq_rows * dim, fi.s_q);
-        const uint8_t* dbits = nullptr;
-        if (bitset && bitset_nbits > 0) {
-            dbits = bitset;
-            if (!is_device_ptr(bitset)) {
-                const size_t nbytes = (size_t)((n_docs + 7) / 8);
-                slot.el.bits.ensure(nbytes);
-                KB2_CUDA_CHECK(cudaMemcpyAsync(slot.el.bits.p, bitset, nbytes, cudaMemcpyHostToDevice, fi.stream));
-                dbits = slot.el.bits.p;
-            }
-        }
+        const uint8_t* dbits = msim::doc_bits_to_device(bitset, bitset_nbits, n_docs, slot.el.bits, fi.stream);
         int64_t* d_ids;
         float* d_dist;
         fi.device_out(n_lists, k, out_ids, out_dist, d_ids, d_dist);

@@ -664,6 +664,33 @@ rerank(IndexBase& ix, int metric, bool vec4, RerankParams rp, const int64_t* can
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Host set-up of every emb-list search: the BruteForce search below and the index-level one (kb2_emb_list_index.cuh).
+
+// The document bitset (host or device bits; none when null or nbits <= 0) on the device: checked to cover n_docs
+// documents, a host bitset copied into buf
+inline const uint8_t*
+doc_bits_to_device(const uint8_t* bitset, int64_t nbits, int64_t n_docs, DevBuf<uint8_t>& buf, cudaStream_t st) {
+    if (!bitset || nbits <= 0) return nullptr;
+    KB2_REQUIRE(nbits >= n_docs, KB2_INVALID_ARGS, "bitset has fewer bits than the index has documents");
+    if (is_device_ptr(bitset)) return bitset;
+    buf.ensure((size_t)((n_docs + 7) / 8));
+    KB2_CUDA_CHECK(cudaMemcpyAsync(buf.p, bitset, (size_t)((n_docs + 7) / 8), cudaMemcpyHostToDevice, st));
+    return buf.p;
+}
+
+// Uploads into buf the list of every query row (ql: validated host offsets; at least one entry).  The returned host
+// array is the copy's source: keep it until the stream has synchronised.
+[[nodiscard]] inline std::vector<int32_t>
+upload_row_list(const std::vector<int64_t>& ql, DevBuf<int32_t>& buf, cudaStream_t st) {
+    std::vector<int32_t> row_list((size_t)std::max<int64_t>(ql.back(), 1));
+    for (size_t l = 0; l + 1 < ql.size(); l++)
+        for (int64_t r = ql[l]; r < ql[l + 1]; r++) row_list[r] = (int32_t)l;
+    buf.ensure(row_list.size());
+    KB2_CUDA_CHECK(cudaMemcpyAsync(buf.p, row_list.data(), row_list.size() * 4, cudaMemcpyHostToDevice, st));
+    return row_list;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // The BruteForce search.
 
 // Scratch of one emb-list search, reused across calls (per-device BruteForce slot).
@@ -700,11 +727,7 @@ search(FlatIndex& fi, Scratch& sc, const float* dq, const std::vector<int64_t>& 
     sc.qlims.ensure(ql.size());
     KB2_CUDA_CHECK(cudaMemcpyAsync(sc.xlims.p, xl.data(), xl.size() * 8, cudaMemcpyHostToDevice, st));
     KB2_CUDA_CHECK(cudaMemcpyAsync(sc.qlims.p, ql.data(), ql.size() * 8, cudaMemcpyHostToDevice, st));
-    std::vector<int32_t> row_list((size_t)std::max<int64_t>(nq_rows, 1));
-    for (int64_t l = 0; l < n_lists; l++)
-        for (int64_t r = ql[l]; r < ql[l + 1]; r++) row_list[r] = (int32_t)l;
-    sc.row_list.ensure(row_list.size());
-    KB2_CUDA_CHECK(cudaMemcpyAsync(sc.row_list.p, row_list.data(), row_list.size() * 4, cudaMemcpyHostToDevice, st));
+    const std::vector<int32_t> row_list = upload_row_list(ql, sc.row_list, st);
     fi.s_qn.ensure(std::max<int64_t>(nq_rows, 1));
     if (metric == KB2_METRIC_L2 && nq_rows > 0)
         row_norms_kernel<<<grid1d(nq_rows * 32, 256), 256, 0, st>>>(dq, nq_rows, d, fi.s_qn.p);

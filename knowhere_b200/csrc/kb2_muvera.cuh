@@ -141,10 +141,9 @@ struct MuveraIndex : IndexBase {
     DevBuf<float> tokens, tokens_n;    // token rows as added; under COSINE their normalised copy, which the re-rank reads
     size_t tokens_used = 0;
     DevBuf<float> proj;                // [R][P][d], uploaded at attach
-    // search scratch: the encoded query lists of a chunk, their tokens' buckets, candidates per list
+    // search scratch: the encoded query lists of a chunk and their tokens' buckets (the attach's buckets too)
     DevBuf<float> fde;
     DevBuf<uint8_t> bucket;
-    DevBuf<int64_t> cand_cnt;
 
     int64_t E() const { return (int64_t)mp.R * ((int64_t)1 << mp.P) * dim; }
     // an empty base of the handle's type over E-dimensional rows, on the handle's stream

@@ -199,8 +199,8 @@ def test_ivf_flat_exact_stage1_equals_bruteforce(kb, ref, metric):
     assert np.array_equal(dist[v].view(np.uint32), bd[v].view(np.uint32))
 
 
-@pytest.mark.parametrize("metric", [0, 1])
-def test_exact_branch_equals_bruteforce(kb, metric):
+@pytest.mark.parametrize("metric,chunks", [(0, 1), (1, 1), (0, 2), (1, 2)], ids=["0", "1", "0-2chunks", "1-2chunks"])
+def test_exact_branch_equals_bruteforce(kb, metric, chunks):
     """vec_topk = rows: HNSW takes its exact branch and every non-empty document is a candidate, so the result is the
     BruteForce emb-list result, ids and score bits"""
     rng = np.random.default_rng(7 + metric)
@@ -208,7 +208,10 @@ def test_exact_branch_equals_bruteforce(kb, metric):
     xl = _lims(np.concatenate([[0, 3], rng.integers(0, 40, 500)]))
     xb = rng.standard_normal((int(xl[-1]), d)).astype(np.float32)
     assert xl[-1] <= 16384
-    ql = _lims([32, 5, 0, 150])
+    # chunks = 2: 32 + 5 + 0 + 150 + 24 * 40 = 1147 tokens x vec_topk = rows (10 089 at L2, 9 923 at IP) make 11.4 to 11.6 M
+    # stage-1 entries, above the 8 M (2^23) of one chunk: a chunk takes at most 845 of the tokens, so two chunks
+    ql = _lims([32, 5, 0, 150] + [40] * 24 * (chunks - 1))
+    assert chunks == 1 or ql[-1] * xl[-1] > 8 << 20
     xq = rng.standard_normal((int(ql[-1]), d)).astype(np.float32)
     ix = kb.Index("HNSW", NAMES[metric][0], d, {"M": 16, "efConstruction": 64})
     ix.add(xb)

@@ -117,11 +117,18 @@ def test_encoder_matches_the_model(kb, P, R, d):
 
 
 # ---------------------------------------------------------------- end to end, exact stage 1
-@pytest.mark.parametrize("typ", ["IVF_FLAT", "HNSW"])
-@pytest.mark.parametrize("metric", ["L2", "IP", "COSINE"])
-def test_exact_stage1_then_bruteforce_rerank(kb, typ, metric):
-    P, R, S, n_docs, k, ratio = 3, 5, 7, 300, 10, 3.0
-    xb, xl, xq, ql = corpus(21, n_docs, 32)
+EXACT = [(m, t, 1) for m in ("L2", "IP", "COSINE") for t in ("IVF_FLAT", "HNSW")] + [("IP", "IVF_FLAT", 2),
+                                                                                     ("COSINE", "IVF_FLAT", 2)]
+
+
+@pytest.mark.parametrize("metric,typ,chunks", EXACT, ids=[f"{m}-{t}" + ("-2chunks" if c > 1 else "") for m, t, c in EXACT])
+def test_exact_stage1_then_bruteforce_rerank(kb, metric, typ, chunks):
+    P, R, S, n_docs, k, ratio, d, nq = 3, 5, 7, 300, 10, 3.0, 32, 24
+    if chunks > 1:
+        # E = R * 2^P * d = 8 * 32 * 64 = 16 384 floats per encoded list: a chunk takes at most 16 M (2^24) / 16 384 =
+        # 1 024 lists, so 1 100 lists span two chunks
+        P, R, d, nq = 5, 8, 64, 1100
+    xb, xl, xq, ql = corpus(21, n_docs, d, nq=nq)
     build = {"nlist": 4} if typ == "IVF_FLAT" else {"M": 16, "efConstruction": 200}
     ix = muvera_index(kb, typ, metric, xb, xl, P, R, S, **build)
     search = {"nprobe": 4} if typ == "IVF_FLAT" else {"ef": 512}
