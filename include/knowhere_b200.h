@@ -150,9 +150,11 @@ int kb2_index_search_typed(kb2_index_t h, const void* queries, int dtype, int64_
  * refine_k (ivf_config.h:33-45,97-128; base_hnsw_config.h:40-71).
  * out_ids[nq*k], out_dist[nq*k] are caller-allocated (like BruteForce::SearchWithBuf,
  * include/knowhere/comp/brute_force.h:33-36).
- * k range: FLAT 1..16384; IVF_FLAT / IVF_PQ k (x refine_k with refine) <= 16384, nprobe <= 1008; HNSW 1..16384 when the
+ * k range: FLAT 1..16384; IVF_FLAT / IVF_PQ k (x refine_k with refine) <= 16384; HNSW 1..16384 when the
  * exact branch runs (k >= n/2 or an almost fully filtered bitset), otherwise as far as the beam (ef) fits; sharded
- * searches world * k <= 8192 and k (x refine_k) <= 1024.  Beyond: KB2_INVALID_ARGS.  Same for kb2_index_search_typed. */
+ * searches world * k <= 8192 and k (x refine_k) <= 1024.  Beyond: KB2_INVALID_ARGS.  IVF nprobe (Search, RangeSearch):
+ * above 65536 KB2_OUT_OF_RANGE_IN_JSON, else clamped to [1, nlist]; a sharded Search takes at most 1008 probes
+ * (KB2_OUT_OF_RANGE_IN_JSON beyond).  Same for kb2_index_search_typed. */
 int kb2_index_search(kb2_index_t h, const float* queries, int64_t nq, int k, const char* json,
                      const uint8_t* bitset, int64_t bitset_nbits, int64_t* out_ids, float* out_dist);
 

@@ -28,6 +28,14 @@ constexpr int kMaxSortEntries = 8192;  // finalize sorts at most this many candi
 constexpr int kMaxLargeK = 16384;      // largest candidate window of the large-k path (DESIGN §4.9)
 // scratch of the large-k path beyond the buffers every search uses: queries are processed in groups that fit it, whatever nq
 constexpr int64_t kLargeKScratch = 1ll << 30;
+// IVF probes (DESIGN §4.9.1).  Up to kMaxWindowProbes the coarse stage selects them in one kMaxK window and one scan CTA holds
+// a query's share of them in shared memory; above, up to kMaxNprobe (the reference's range), the coarse stage takes the
+// large-k selection, no scan CTA holds more than kScanSliceProbes probes, and the queries run in groups whose probe arrays
+// and scan scratch fit kProbeScratch.
+constexpr int kMaxWindowProbes = kMaxK - 16;   // 1008
+constexpr int kMaxNprobe = 65536;
+constexpr int kScanSliceProbes = 1024;
+constexpr int64_t kProbeScratch = 1ll << 30;
 
 struct Counters {
     int64_t launches = 0, codes = 0, code_bytes = 0, pairs = 0, h2d = 0, d2h = 0;
@@ -1289,12 +1297,21 @@ struct IvfIndex : IndexBase {
         return {s_log.p, s_logcnt.p, cap};
     }
 
+    // probe slices of the redo of a flagged query: their Ksel-entry outputs fill its kTcCandCap-entry candidate row
+    static int
+    tc_redo_split(int nprobe, int Ksel) {
+        return std::max(1, std::min(kTcCandCap / Ksel, nprobe));
+    }
+
     bool
     use_tc_engine(int64_t nq, int nprobe, int Ksel) const {
         if (!is_pq || !(tc_geom_18() || tc_geom_32())) return false;
         const char* e = getenv("KB2_PQ_ENGINE");
         if (e && !strcmp(e, "lut")) return false;
         if (nprobe < 8 || Ksel > kTcCandCap / 2) return false;
+        // the redo of a flagged query splits its probes over the kTcCandCap / Ksel slices of its candidate row: above
+        // kScanSliceProbes per slice the scan kernels' probe arrays would not fit, so those searches stay query-major
+        if ((nprobe + tc_redo_split(nprobe, Ksel) - 1) / tc_redo_split(nprobe, Ksel) > kScanSliceProbes) return false;
         if (e && !strcmp(e, "tc")) return true;
         // the decode of a list is amortised over the queries that probe it.  Measured at C5 (100M x 96, nlist 65536, 19.5
         // queries per list on average): the query-major LUT engine needs 34.5 ms per 10000-query batch on two GPUs, so the
@@ -1489,7 +1506,7 @@ struct IvfIndex : IndexBase {
         // ---- flagged queries (no bound / buffer overflow): complete LUT scan into their candidate rows
         {
             IvfScanParams f = sp;
-            f.nsplit = std::max(1, std::min(kTcCandCap / Ksel, nprobe));   // probe slices per flagged query: their lists fill the row
+            f.nsplit = tc_redo_split(nprobe, Ksel);   // probe slices per flagged query: their lists fill the row
             f.partial = s_cand.p;
             f.partial_stride = kTcCandCap;
             f.clear_to = kTcCandCap - (f.nsplit - 1) * Ksel;   // == Ksel (nothing to clear) when the slices fill the row
@@ -1531,6 +1548,9 @@ struct IvfIndex : IndexBase {
         const char* e = getenv("KB2_FLAT_ENGINE");
         if (e && !strcmp(e, "scan")) return false;
         if (k + 16 > kTcCandCap / 2) return false;
+        // every (query, probe) pair gets its own split copy of the query (8 bytes per dimension): above kMaxWindowProbes
+        // probes the engine is taken only where those copies fit the group's scratch
+        if (nprobe > kMaxWindowProbes && ((double)nq * nprobe + fltc::NQ_ITEM) * dim * 8 > (double)kProbeScratch) return false;
         if (e && !strcmp(e, "tc")) return true;
         // a list tile is amortised over the queries probing it
         return (double)nq * nprobe >= 8.0 * (double)nlist && nq >= 64;
@@ -1657,6 +1677,7 @@ struct IvfIndex : IndexBase {
         rp.dense_ld = L;
         rp.scanned = d_counter.p;
         sp.nsplit = (g < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + g - 1) / g) : 1;
+        sp.nsplit = std::max(sp.nsplit, (nprobe + kScanSliceProbes - 1) / kScanSliceProbes);
         const int np_max = (nprobe + sp.nsplit - 1) / sp.nsplit;
         const size_t smem = (size_t)dim * 4 + 64 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12 + (is_pq ? (size_t)M * 1024 : 0);
         KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "large-k search: m too large");
@@ -1705,9 +1726,10 @@ struct IvfIndex : IndexBase {
         KB2_REQUIRE(trained, KB2_INDEX_NOT_TRAINED, "index not trained");
         KB2_REQUIRE(n_total > 0, KB2_EMPTY_INDEX, "index is empty");
         seal();
-        int nprobe = (int)cfg.get_int("nprobe", 8);
-        nprobe = (int)std::min<int64_t>(std::max(nprobe, 1), nlist);
-        KB2_REQUIRE(nprobe <= kMaxK - 16, KB2_OUT_OF_RANGE_IN_JSON, "nprobe too large for the GPU path (max 1008)");
+        const int nprobe = search_nprobe(cfg);
+        // a sharded search all-gathers the probes of one kMaxK window per query
+        KB2_REQUIRE(nprobe <= kMaxWindowProbes || shard_world == 1, KB2_OUT_OF_RANGE_IN_JSON,
+                    "nprobe too large for the GPU path (max 1008)");
         const bool use_refine = is_pq && refine;
         const double refine_k = cfg.get_num("refine_k", 1.0);
         KB2_REQUIRE(refine_k >= 1.0, KB2_OUT_OF_RANGE_IN_JSON, "refine_k must be >= 1");
@@ -1725,6 +1747,11 @@ struct IvfIndex : IndexBase {
         int64_t* d_ids;
         float* d_dist;
         device_out(nq, k, out_ids, out_dist, d_ids, d_dist);
+        if (nprobe > kMaxWindowProbes) {
+            search_many_probes(dq, nq, nprobe, k, k_base, use_refine, dbits, d_ids, d_dist);
+            results_out(nq, k, out_ids, out_dist, d_ids, d_dist);
+            return;
+        }
 
         // ---- coarse quantizer.  With a communicator every rank ranks the centroids for its slice of the batch only and the
         //      probe lists are all-gathered (in place; slices padded to the same length).
@@ -1742,7 +1769,70 @@ struct IvfIndex : IndexBase {
         } else {
             coarse_probes(dq, 0, nq, nprobe);
         }
+        scan_probes(dq, nq, nprobe, k, k_base, use_refine, dbits, d_ids, d_dist, out_ids, out_dist);
+    }
 
+    // nprobe of a search config: the reference's range check (1..kMaxNprobe), then clamped to [1, nlist]
+    int
+    search_nprobe(const JsonObj& cfg) const {
+        const long long v = cfg.get_int("nprobe", 8);
+        KB2_REQUIRE(v <= kMaxNprobe, KB2_OUT_OF_RANGE_IN_JSON, "nprobe out of range (1..65536)");
+        return (int)std::min<int64_t>(std::max<long long>(v, 1), nlist);
+    }
+
+    // Search above kMaxWindowProbes probes: the queries run in groups, one host iteration each, whose probe arrays
+    // (12 bytes a probe), list-major pairs (8 bytes a probe), scan slices and candidate rows fit kProbeScratch.  Each group
+    // ranks its probes (coarse_probes: the large-k selection) and runs scan_probes on them, which picks the engine as it
+    // does for any batch; the results land in the group's rows of d_ids / d_dist.
+    void
+    search_many_probes(const float* dq, int64_t nq, int nprobe, int k, int k_base, bool use_refine, const uint8_t* dbits,
+                       int64_t* d_ids, float* d_dist) {
+        const int Ksel = next_pow2(std::max(32, k_base));
+        const int64_t slices = (nprobe + kScanSliceProbes - 1) / kScanSliceProbes;
+        const int64_t per_query = (int64_t)nprobe * 20 + (slices + 1) * Ksel * 8 + (int64_t)kTcCandCap * 8 + 4096 * 4 + dim * 2;
+        const int64_t g = std::max<int64_t>(1, std::min<int64_t>(nq, kProbeScratch / per_query));
+        s_probe_ids.ensure((size_t)g * nprobe);
+        s_probe_dis.ensure((size_t)g * nprobe);
+        Counters sum{};
+        float stage_ms = 0.f, kernel_ms = 0.f;
+        int engine = 0;
+        for (int64_t q0 = 0; q0 < nq; q0 += g) {
+            const int64_t rows = std::min(g, nq - q0);
+            const float* gq = dq + q0 * dim;
+            coarse_probes(gq, 0, rows, nprobe);
+            int64_t* gi = d_ids + q0 * k;
+            float* gd = d_dist + q0 * k;
+            scan_probes(gq, rows, nprobe, k, k_base, use_refine, dbits, gi, gd, gi, gd);
+            sum.codes += last.codes;
+            sum.code_bytes += last.code_bytes;
+            sum.pairs += last.pairs;
+            sum.survivors += last.survivors;
+            sum.flagged += last.flagged;
+            stage_ms += last_stage_ms;
+            kernel_ms += last_kernel_ms;
+            engine = std::max(engine, last_engine);   // a batch some of whose groups went list-major reports the list-major engine
+        }
+        last.codes = sum.codes;
+        last.code_bytes = sum.code_bytes;
+        last.pairs = sum.pairs;
+        last.survivors = sum.survivors;
+        last.flagged = sum.flagged;
+        last_engine = engine;
+        if (timing) {
+            last_stage_ms = stage_ms;
+            last_kernel_ms = kernel_ms;
+            last_comm_ms = 0.f;
+        }
+    }
+
+    // Scan of the nq queries' probes in s_probe_ids / s_probe_dis (rows [0, nq)) and the finalize into d_ids / d_dist, which
+    // results_out copies to out_ids / out_dist.  The engine: the large-k path for windows k_base > kMaxK, else the list-major
+    // tensor-core engines where use_tc_engine / use_flat_tc_engine take them, else the query-major scan kernels.
+    void
+    scan_probes(const float* dq, int64_t nq, int nprobe, int k, int k_base, bool use_refine, const uint8_t* dbits, int64_t* d_ids,
+                float* d_dist, int64_t* out_ids, float* out_dist) {
+        cudaStream_t st = stream;
+        const bool dist = distributed();
         if (k_base > kMaxK) {
             KB2_REQUIRE(!dist, KB2_NOT_IMPLEMENTED, "sharded search with k (x refine_k) above 1024");
             search_large(dq, nq, nprobe, k, k_base, use_refine, dbits, d_ids, d_dist);
@@ -1779,6 +1869,10 @@ struct IvfIndex : IndexBase {
         if (nq < 2 * num_sms()) nsplit = (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq);
         const int Ksel = next_pow2(std::max(32, k_base));
         while ((int64_t)nsplit * Ksel > kMaxSortEntries) nsplit--;
+        // no CTA holds more than kScanSliceProbes probes; slices whose outputs exceed what finalize sorts are cut to the
+        // Ksel best of each query first (select_rows_kernel)
+        nsplit = std::max(nsplit, (nprobe + kScanSliceProbes - 1) / kScanSliceProbes);
+        const bool cut_slices = (int64_t)nsplit * Ksel > kMaxSortEntries;
         const int np_max = (nprobe + nsplit - 1) / nsplit;
         s_partial2.ensure((size_t)nq * nsplit * Ksel);
         KB2_CUDA_CHECK(cudaMemsetAsync(d_counter.p, 0, 64, st));
@@ -1811,6 +1905,13 @@ struct IvfIndex : IndexBase {
             fin_counts = s_cand_cnt.p;
         } else {
             launch_scan(sp, grid, Ksel, np_max, dbits != nullptr);
+            if (cut_slices) {
+                s_partial.ensure((size_t)nq * Ksel);
+                large_k_select<uint64_t>(*this, s_partial2.p, fin_stride, fin_stride, 0u, Ksel, s_partial.p, Ksel, nq);
+                fin_partial = s_partial.p;
+                fin_stride = Ksel;
+                fin_n = Ksel;
+            }
         }
         if (timing) KB2_CUDA_CHECK(cudaEventRecord(ev1, st));
 
@@ -2176,22 +2277,37 @@ struct IvfIndex : IndexBase {
         KB2_REQUIRE(trained, KB2_INDEX_NOT_TRAINED, "index not trained");
         seal();
         const int64_t nq = q.sp.nq;
-        nprobe = (int)std::min<int64_t>(std::max<int64_t>(cfg.get_int("nprobe", 8), 1), nlist);
-        s_probe_ids.ensure((size_t)nq * nprobe);
-        s_probe_dis.ensure((size_t)nq * nprobe);
-        coarse_probes(q.sp.queries, 0, nq, nprobe);
-        RangeParams rp = list_params(q.sp.queries, nq, nprobe, q.sp.bitset);
-        rp.radius = q.radius;
-        rp.range_filter = q.range_filter;
-        // with max_empty_result_buckets on, a probe is empty when it adds no hit inside the radius, whatever range_filter
-        // says (faiss range_search_preassigned): the scan emits the radius hits and range_search_index filters after the cut
-        rp.has_filter = range_max_empty(cfg) > 0 ? 0 : q.has_filter;
-        rp.sp.nsplit = (nq < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + nq - 1) / nq) : 1;
-        const int np_max = (nprobe + rp.sp.nsplit - 1) / rp.sp.nsplit;
-        size_t smem = (size_t)dim * 4 + 64 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12;
-        if (is_pq) smem += (size_t)M * 1024;
-        KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "range search: m too large");
-        std::vector<RangeHit> h = range_scan(*this, rp, smem);
+        nprobe = search_nprobe(cfg);
+        // above kMaxWindowProbes the queries run in groups whose probe arrays fit kProbeScratch
+        const int64_t g = (nprobe > kMaxWindowProbes) ? std::max<int64_t>(1, std::min<int64_t>(nq, kProbeScratch / ((int64_t)nprobe * 12)))
+                                                      : nq;
+        s_probe_ids.ensure((size_t)g * nprobe);
+        s_probe_dis.ensure((size_t)g * nprobe);
+        std::vector<RangeHit> h;
+        for (int64_t q0 = 0; q0 < nq; q0 += g) {
+            const int64_t rows = std::min(g, nq - q0);
+            const float* gq = q.sp.queries + q0 * dim;
+            coarse_probes(gq, 0, rows, nprobe);
+            RangeParams rp = list_params(gq, rows, nprobe, q.sp.bitset);
+            rp.radius = q.radius;
+            rp.range_filter = q.range_filter;
+            // with max_empty_result_buckets on, a probe is empty when it adds no hit inside the radius, whatever range_filter
+            // says (faiss range_search_preassigned): the scan emits the radius hits and range_search_index filters after the cut
+            rp.has_filter = range_max_empty(cfg) > 0 ? 0 : q.has_filter;
+            rp.sp.nsplit = (rows < 2 * num_sms()) ? (int)std::min<int64_t>(nprobe, (2 * num_sms() + rows - 1) / rows) : 1;
+            rp.sp.nsplit = std::max(rp.sp.nsplit, (nprobe + kScanSliceProbes - 1) / kScanSliceProbes);
+            const int np_max = (nprobe + rp.sp.nsplit - 1) / rp.sp.nsplit;
+            size_t smem = (size_t)dim * 4 + 64 + (size_t)(np_max + 1) * 4 + (size_t)np_max * 12;
+            if (is_pq) smem += (size_t)M * 1024;
+            KB2_REQUIRE(smem <= (size_t)kMaxDynSmem, KB2_NOT_IMPLEMENTED, "range search: m too large");
+            std::vector<RangeHit> hg = range_scan(*this, rp, smem);
+            if (q0 == 0) {
+                h = std::move(hg);
+            } else {
+                for (RangeHit& e : hg) e.q += (int32_t)q0;   // the group's queries are numbered from 0
+                h.insert(h.end(), hg.begin(), hg.end());
+            }
+        }
         std::vector<int32_t> hrows(npad);
         KB2_CUDA_CHECK(cudaMemcpy(hrows.data(), rows.p, npad * 4, cudaMemcpyDeviceToHost));
         for (RangeHit& e : h) e.pos = (uint32_t)hrows[e.pos];

@@ -632,11 +632,21 @@ range_scan_kernel(RangeParams rp) {
         const int j1 = min(p.nprobe, j0 + np_max);
         nchunks = setup_probes(p, q, j0, j1, ps);
         if (rp.dense) {
+            // block-wide sum over the probes before j0 (up to 65535 of them), accumulated in the word after the probe
+            // arrays (inside the 64 bytes every IVF launch adds to them; no static shared memory, so that the launch
+            // helper may raise the dynamic limit to kMaxDynSmem)
+            uint32_t* s_chunk_base = (uint32_t*)(ps.dis0 + np_max);
+            if (threadIdx.x == 0) *s_chunk_base = 0;
+            __syncthreads();
             const int64_t pstride = p.probe_stride ? p.probe_stride : p.nprobe;
-            for (int j = 0; j < j0; j++) {   // every thread the same serial sum (j0 <= nprobe <= 1008)
+            uint32_t part = 0;
+            for (int j = threadIdx.x; j < j0; j += blockDim.x) {
                 const int64_t l = p.probe_ids[q * pstride + j];
-                if (l >= 0) chunk_base += (uint32_t)((p.list_len[l] + 31) >> 5);
+                if (l >= 0) part += (uint32_t)((p.list_len[l] + 31) >> 5);
             }
+            if (part) atomicAdd(s_chunk_base, part);
+            __syncthreads();
+            chunk_base = *s_chunk_base;
         }
     }
     if (rp.kind != 0) {
