@@ -20,6 +20,7 @@
 #include <omp.h>
 
 #include <cmath>
+#include <cub/cub.cuh>
 #include <queue>
 
 #include "kb2_blob.h"
@@ -958,11 +959,13 @@ hnsw_wide_kernel(HnswWideParams w) {
 // shrink_neighbor_list, :302-420 add_links_starting_from).  The reference inserts one node at a time under per-node locks;
 // here every level is built by BATCHED insertion in the reference's order (levels descending): for a batch of new nodes
 //   1. hnsw_search_kernel (beam on that level, ef = efConstruction, entry from the finished upper levels) -> candidates
-//   2. hnsw_select_kernel: the heuristic of shrink_neighbor_list (keep c unless some kept s has dist(c,s) < dist(c,q))
-//   3. hnsw_link_kernel: reverse links under a per-node spin lock; a full row is re-shrunk with the same heuristic
+//   2. hnsw_select_kernel: shrink_neighbor_list (K/impl/HNSW.cpp:285-307): fewer candidates than the row holds are all
+//      kept, else the heuristic (keep c unless some kept s has dist(c,s) < dist(c,q)); one (s << 32 | w) pair per link
+//   3. cub::DeviceRadixSort of the pairs, so that each target s gets its arrivals in batch order
+//   4. hnsw_link_kernel: one warp per target s appends the new nodes to s's row; a full row is re-shrunk with the heuristic
 // Nodes of one batch do not see each other; batches grow with the graph (<= 1/4 of it), so the effect is that of a few
-// concurrent inserters in the reference.  Graphs are not bit-identical to the reference's (they are not reproducible
-// run-to-run there either); recall parity is what the tests hold.
+// concurrent inserters in the reference.  No step depends on scheduling, so a build is a function of the data and the
+// parameters: tests/hnsw_build_model.py restates it and the device graph equals it bit for bit on small-integer data.
 // ============================================================================================
 struct HnswBuildParams {
     const float* vecs;
@@ -974,9 +977,9 @@ struct HnswBuildParams {
     int nb, ef;
     const int64_t* cand_ids;     // [nb][ef] ascending by key (from the search kernel), -1 padded
     const float* cand_dist;      // [nb][ef] distances as Search reports them (IP un-negated)
-    int32_t* sel_ids;            // [nb][64] selected neighbours of each new node (for the link pass)
-    int32_t* sel_cnt;            // [nb]
-    int32_t* locks;              // [n]
+    unsigned long long* pairs;   // [nb][64] (s << 32 | w) per selected neighbour s of batch[w], then pair_end
+    const unsigned long long* sorted;   // the pairs, ascending
+    unsigned long long pair_end; // (n << 32): sorts after every pair, its target is no node
 };
 constexpr int kBuildWarps = 4;
 
@@ -1012,17 +1015,28 @@ hnsw_select_kernel(HnswBuildParams p) {
     if (w >= p.nb) return;
     const int32_t q = p.batch[w];
     const int maxn = p.cum[p.level + 1] - p.cum[p.level];
+    // the candidates are the pool up to its first -1, without q; fewer than maxn are all kept (K/impl/HNSW.cpp:290-292)
+    int nvalid = 0;
+    for (int base = 0; base < p.ef; base += kWarp) {
+        const int64_t c = (base + lane < p.ef) ? p.cand_ids[(int64_t)w * p.ef + base + lane] : -1;
+        nvalid += __popc(__ballot_sync(0xffffffffu, c >= 0 && c != q));
+    }
+    const bool keep_all = nvalid < maxn;
     int nsel = 0;
     for (int ci = 0; ci < p.ef && nsel < maxn; ci++) {
         const int64_t c = p.cand_ids[(int64_t)w * p.ef + ci];
         if (c < 0) break;
         if (c == q) continue;
-        const float dc = p.cand_dist[(int64_t)w * p.ef + ci];
-        const float kc = (METRIC == KB2_METRIC_L2) ? dc : -dc;
-        __syncwarp();
-        for (int j = lane; j < p.d; j += kWarp) s_c[j] = p.vecs[c * p.d + j];
-        __syncwarp();
-        if (hnsw_heuristic_keep<METRIC>(p.vecs, p.d, s_c, kc, s_sel, nsel, lane)) {
+        bool keep = keep_all;
+        if (!keep) {
+            const float dc = p.cand_dist[(int64_t)w * p.ef + ci];
+            const float kc = (METRIC == KB2_METRIC_L2) ? dc : -dc;
+            __syncwarp();
+            for (int j = lane; j < p.d; j += kWarp) s_c[j] = p.vecs[c * p.d + j];
+            __syncwarp();
+            keep = hnsw_heuristic_keep<METRIC>(p.vecs, p.d, s_c, kc, s_sel, nsel, lane);
+        }
+        if (keep) {
             if (lane == 0) s_sel[nsel] = (int32_t)c;
             nsel++;
             __syncwarp();
@@ -1030,13 +1044,14 @@ hnsw_select_kernel(HnswBuildParams p) {
     }
     int32_t* row = p.neighbors + p.offsets[q] + p.cum[p.level];
     for (int j = lane; j < maxn; j += kWarp) row[j] = j < nsel ? s_sel[j] : -1;
-    for (int j = lane; j < nsel; j += kWarp) p.sel_ids[(int64_t)w * 64 + j] = s_sel[j];
-    if (lane == 0) p.sel_cnt[w] = nsel;
+    for (int j = lane; j < 64; j += kWarp)
+        p.pairs[(int64_t)w * 64 + j] = j < nsel ? ((unsigned long long)s_sel[j] << 32) | (unsigned)w : p.pair_end;
 }
 
-// reverse links: for every selected neighbour s of the new node q, add q to s's row (under s's lock); a full row is
-// re-selected among its members + q with the heuristic, centre s.  dynamic smem per warp: 2 * d floats + 3 * kLinkSlots
-// words (a full row of 2M = 64 members plus q is 65 candidates)
+// reverse links: warp i takes sorted pair i when it starts the run of its target s, and adds the new nodes batch[w] of
+// the run to s's row in ascending w; a full row is re-selected among its members + the new node with the heuristic,
+// centre s.  One warp owns each row, so no order between warps shows in the graph.  dynamic smem per warp: 2 * d floats
+// + 3 * kLinkSlots words (a full row of 2M = 64 members plus the new node is 65 candidates)
 constexpr int kLinkSlots = 72;
 template <int METRIC>
 __global__ void __launch_bounds__(kBuildWarps * 32)
@@ -1050,19 +1065,17 @@ hnsw_link_kernel(HnswBuildParams p) {
     int32_t* s_id = (int32_t*)(s_c + dpad);          // [kLinkSlots] candidate ids (sorted by key to s)
     float* s_key = (float*)(s_id + kLinkSlots);      // [kLinkSlots]
     int32_t* s_sel = (int32_t*)(s_key + kLinkSlots); // [kLinkSlots] kept ids
-    const int w = blockIdx.x * kBuildWarps + warp;
-    if (w >= p.nb) return;
-    const int32_t q = p.batch[w];
+    const int64_t npairs = (int64_t)p.nb * 64;
+    const int64_t i0 = (int64_t)blockIdx.x * kBuildWarps + warp;
+    if (i0 >= npairs) return;
+    const unsigned long long head = p.sorted[i0];
+    if (head >= p.pair_end || (i0 > 0 && (p.sorted[i0 - 1] >> 32) == (head >> 32))) return;
+    const int32_t s = (int32_t)(head >> 32);
     const int cap = p.cum[p.level + 1] - p.cum[p.level];   // <= 64 (M <= 32)
-    const int nq_sel = p.sel_cnt[w];
-    for (int si = 0; si < nq_sel; si++) {
-        const int32_t s = p.sel_ids[(int64_t)w * 64 + si];
-        if (lane == 0) {
-            while (atomicCAS(&p.locks[s], 0, 1) != 0) {}
-        }
-        __syncwarp();
-        __threadfence();
-        volatile int32_t* row = p.neighbors + p.offsets[s] + p.cum[p.level];
+    int32_t* row = p.neighbors + p.offsets[s] + p.cum[p.level];
+    for (int j = lane; j < p.d; j += kWarp) s_s[j] = p.vecs[(int64_t)s * p.d + j];
+    for (int64_t i = i0; i < npairs && (p.sorted[i] >> 32) == (head >> 32); i++) {
+        const int32_t q = p.batch[(uint32_t)p.sorted[i]];
         // current members (compact, -1 terminated)
         int cnt = 0;
         for (int j0 = 0; j0 < cap; j0 += kWarp) {
@@ -1076,7 +1089,6 @@ hnsw_link_kernel(HnswBuildParams p) {
             if (lane == 0) row[cnt] = q;
         } else {
             // full: candidates = members + q, keys to s, sort, heuristic, rewrite
-            for (int j = lane; j < p.d; j += kWarp) s_s[j] = p.vecs[(int64_t)s * p.d + j];
             if (lane == 0) s_id[cnt] = q;
             __syncwarp();
             const int nc = cnt + 1;
@@ -1123,10 +1135,7 @@ hnsw_link_kernel(HnswBuildParams p) {
             }
             for (int j = lane; j < cap; j += kWarp) row[j] = j < nsel ? s_sel[j] : -1;
         }
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) atomicExch(&p.locks[s], 0);
-        __syncwarp();
+        __syncwarp();   // the row as this arrival left it is what the next one reads
     }
 }
 
@@ -1443,20 +1452,27 @@ struct HnswIndex : IndexBase {
         KB2_CUDA_CHECK(cudaMemcpyAsync(d_cum.p, h_cum.data(), h_cum.size() * 4, cudaMemcpyHostToDevice, st));
         std::vector<int32_t> rank(n);
         for (int64_t i = 0; i < n; i++) rank[order[i]] = (int32_t)i;
-        DevBuf<int32_t> d_order, d_rank, d_locks, d_sel, d_selcnt;
+        DevBuf<int32_t> d_order, d_rank;
         DevBuf<int64_t> d_cand_ids;
         DevBuf<float> d_cand_dist;
+        DevBuf<unsigned long long> d_pairs, d_sorted;
+        DevBuf<unsigned char> d_sort_tmp;
         d_order.alloc_exact((size_t)n);
         d_rank.alloc_exact((size_t)n);
-        d_locks.alloc_exact((size_t)n);
         KB2_CUDA_CHECK(cudaMemcpyAsync(d_order.p, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
         KB2_CUDA_CHECK(cudaMemcpyAsync(d_rank.p, rank.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        KB2_CUDA_CHECK(cudaMemsetAsync(d_locks.p, 0, (size_t)n * 4, st));
         const int64_t maxb = std::min<int64_t>(kBuildBatch, n);
         d_cand_ids.alloc_exact((size_t)maxb * ef);
         d_cand_dist.alloc_exact((size_t)maxb * ef);
-        d_sel.alloc_exact((size_t)maxb * 64);
-        d_selcnt.alloc_exact((size_t)maxb);
+        // the link pairs (s << 32 | w) sort on their low 32 + bit_width(n) bits, so the end marker n << 32 sorts last
+        int sort_bits = 32;
+        while ((1ll << (sort_bits - 32)) <= n) sort_bits++;
+        d_pairs.alloc_exact((size_t)maxb * 64);
+        d_sorted.alloc_exact((size_t)maxb * 64);
+        size_t sort_bytes = 0;
+        KB2_CUDA_CHECK(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, d_pairs.p, d_sorted.p, (int)(maxb * 64), 0,
+                                                      sort_bits, st));
+        d_sort_tmp.alloc_exact(sort_bytes);
         d_next.ensure(1);
         const int dpad = (dim + 3) & ~3;
         const size_t smem_sel = (size_t)kBuildWarps * ((size_t)dpad * 4 + 256);
@@ -1497,15 +1513,17 @@ struct HnswIndex : IndexBase {
                 b.ef = ef;
                 b.cand_ids = d_cand_ids.p;
                 b.cand_dist = d_cand_dist.p;
-                b.sel_ids = d_sel.p;
-                b.sel_cnt = d_selcnt.p;
-                b.locks = d_locks.p;
+                b.pairs = d_pairs.p;
+                b.sorted = d_sorted.p;
+                b.pair_end = (unsigned long long)n << 32;
                 const int gb = (int)((nb + kBuildWarps - 1) / kBuildWarps);
                 with_metric(metric, [&](auto m) {
                     constexpr int MM = decltype(m)::value;
                     launch<hnsw_search_kernel<MM, false>>(La.grid, kHnswWarps * 32, La.smem, st, p);
                     launch<hnsw_select_kernel<MM>>(gb, kBuildWarps * 32, smem_sel, st, b);
-                    launch<hnsw_link_kernel<MM>>(gb, kBuildWarps * 32, smem_link, st, b);
+                    KB2_CUDA_CHECK(cub::DeviceRadixSort::SortKeys(d_sort_tmp.p, sort_bytes, d_pairs.p, d_sorted.p,
+                                                                  (int)(nb * 64), 0, sort_bits, st));
+                    launch<hnsw_link_kernel<MM>>((int)(nb * 64 / kBuildWarps), kBuildWarps * 32, smem_link, st, b);
                 });
                 inserted += nb;
                 n_batches++;
@@ -1514,7 +1532,7 @@ struct HnswIndex : IndexBase {
         KB2_CUDA_CHECK(cudaGetLastError());
         KB2_CUDA_CHECK(cudaMemcpyAsync(h_neighbors.data(), d_neighbors.p, h_neighbors.size() * 4, cudaMemcpyDeviceToHost, st));
         KB2_CUDA_CHECK(cudaStreamSynchronize(st));
-        last.launches = 3 * n_batches;
+        last.launches = 4 * n_batches;   // search, select, the pair sort (counted once), link
         // rows are compact (-1 only at the tail) by construction of the two kernels; validate the structure once
         validate_graph();
         uploaded = false;

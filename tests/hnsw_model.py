@@ -2,7 +2,10 @@
 K/impl/HnswSearcher.h:116-432, with NeighborSetPopList, K/impl/Neighbor.h:46-150), for graphs in the HNSW layout.
 
 Keys are computed in float64 and rounded to float32 (squared L2, or minus the inner product), so on small-integer data
-they equal the fp32 keys of every searcher.  Returns ids, distances (IP sign restored) and the summed (ndis, nhops)."""
+they equal the fp32 keys of every searcher.  Returns ids, distances (IP sign restored) and the summed (ndis, nhops).
+
+descend and beam are the two halves of a search; tests/hnsw_build_model.py runs them in build mode (a beam on an upper
+level, a descent restricted to the nodes already linked)."""
 import bisect
 
 import numpy as np
@@ -16,37 +19,42 @@ def _key(X, v, q, metric):
     return float(np.float32(k))
 
 
-def search_one(X, g, q, k, ef, metric):
-    """g: dict with levels, offsets, neighbors, cum, entry_point, max_level (kb2_hnsw_export / RefHnsw.export)"""
-    q = np.asarray(q, np.float64)
+def row_links(g, v, level):
+    """the live links of v on level, up to the first -1"""
     nb, off, cum = g["neighbors"], g["offsets"], g["cum"]
+    out = []
+    for j in range(off[v] + cum[level], off[v] + cum[level + 1]):
+        if nb[j] < 0:
+            break
+        out.append(int(nb[j]))
+    return out
 
-    def links(v, level):
-        out = []
-        for j in range(off[v] + cum[level], off[v] + cum[level + 1]):
-            if nb[j] < 0:
-                break
-            out.append(int(nb[j]))
-        return out
 
+def descend(g, key, nearest, d_nearest, top, bottom):
+    """greedy_update_nearest on levels top .. bottom + 1: first strict minimum over the link slots, until no change.
+    key(v) is the key of node v to the query.  Returns (nearest, d_nearest, ndis, nhops)."""
     ndis = nhops = 0
-    nearest = int(g["entry_point"])
-    d_nearest = _key(X, nearest, q, metric)
-    for level in range(int(g["max_level"]), 0, -1):   # greedy_update_nearest: first strict minimum, until no change
+    for level in range(top, bottom, -1):
         while True:
             prev = nearest
-            row = links(prev, level)
+            row = row_links(g, prev, level)
             for v in row:
-                dv = _key(X, v, q, metric)
+                dv = key(v)
                 if dv < d_nearest:
                     nearest, d_nearest = v, dv
             ndis += len(row)
             nhops += 1
             if nearest == prev:
                 break
-    cap = max(ef, k)
-    dist, ids, checked = [d_nearest], [nearest], [False]
-    visited = {nearest}
+    return nearest, d_nearest, ndis, nhops
+
+
+def beam(g, key, entry, d_entry, cap, level=0):
+    """the pop-list beam of capacity cap on level from one entry node.  Returns the sorted pool (dist, ids) and
+    (ndis, nhops)."""
+    ndis = nhops = 0
+    dist, ids, checked = [d_entry], [entry], [False]
+    visited = {entry}
     cur = 0
     while cur < len(dist):
         node = ids[cur]
@@ -55,12 +63,12 @@ def search_one(X, g, q, k, ef, metric):
         while cur < len(dist) and checked[cur]:
             cur += 1
         nhops += 1
-        for v in links(node, 0):
+        for v in row_links(g, node, level):
             if v in visited:
                 continue
             visited.add(v)
             ndis += 1
-            dv = _key(X, v, q, metric)
+            dv = key(v)
             pos = bisect.bisect_right(dist, dv)   # upper_bound: after every equal key
             if pos >= cap:
                 continue
@@ -70,6 +78,18 @@ def search_one(X, g, q, k, ef, metric):
             del dist[cap:], ids[cap:], checked[cap:]
             if pos < cur:
                 cur = pos
+    return dist, ids, ndis, nhops
+
+
+def search_one(X, g, q, k, ef, metric):
+    """g: dict with levels, offsets, neighbors, cum, entry_point, max_level (kb2_hnsw_export / RefHnsw.export)"""
+    q = np.asarray(q, np.float64)
+    key = lambda v: _key(X, v, q, metric)   # noqa: E731
+    ep = int(g["entry_point"])
+    nearest, d_nearest, ndis, nhops = descend(g, key, ep, key(ep), int(g["max_level"]), 0)
+    dist, ids, a, b = beam(g, key, nearest, d_nearest, max(ef, k))
+    ndis += a
+    nhops += b
     n = min(k, len(dist))
     out_i = np.full(k, -1, np.int64)
     out_d = np.full(k, FLT_MAX if metric == "L2" else -FLT_MAX, np.float32)
